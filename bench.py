@@ -4,6 +4,7 @@
     python bench.py --grid 0.25deg --batch 4 --precision bf16        # BASELINE configs[2]
     python bench.py --impl reference --steps 2 --warmup 1            # the reference's CPU forward on the host cores
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N [--grid 0.25deg --batch 4 --precision bf16]
+    python bench.py --steps 20 --warmup 3 --dump-outputs DIR         # also write the last timed step's forecast (sampled) to DIR
 
 The model is built exactly as a user of the reference builds it -- `GraphWeatherForecaster(lat_lons)`, no extra keyword --
 unless --precision names a non-default arithmetic mode.  One step = one model(features) call at `--batch` samples per GPU;
@@ -17,6 +18,10 @@ The JSON line carries the contract keys plus
   parity        max |GPU - oracle| of one sample of THIS run's output (1 deg grid; the oracle is the CPU restatement)
   cpu_baseline  the reference forward on this box's host cores, bounded sample (rank 0, N = 1 only)
   e2e           the same metric through the public module call with pinned-host inputs copied in and the forecast copied out
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned: DIR/forecast.npy (float32) holds a fixed,
+seeded sample of its rows (every row when the dump fits 48 MB), DIR/forecast_rows.npy (float64) their flat indices into
+[batch * points].  Model and inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 
 import argparse
@@ -146,6 +151,19 @@ def bind_to_gpu_numa(index):
     return None
 
 
+DUMP_BYTES = 48_000_000  # both files together
+
+
+def dump_outputs(out_dir, y):
+    """The forecast of the last timed step, [batch, points, 78] -> rows; a seeded sample of rows when it exceeds DUMP_BYTES."""
+    rows = y.detach().float().reshape(-1, y.shape[-1]).cpu().numpy()
+    keep = min(rows.shape[0], DUMP_BYTES // (rows.shape[1] * 4 + 8))
+    idx = np.arange(rows.shape[0]) if keep == rows.shape[0] else np.sort(np.random.default_rng(0).choice(rows.shape[0], keep, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "forecast.npy"), np.ascontiguousarray(rows[idx], dtype=np.float32))
+    np.save(os.path.join(out_dir, "forecast_rows.npy"), idx.astype(np.float64))
+
+
 def reference_model_and_inputs(lat_lons, batch, seed=42):
     """The CPU leg's model: the reference's own unmodified modules (oracle/ref_shims.py) when /root/reference exists (build
     container), else the oracle port (oracle/restate.py; GPU box).  Default initialisation under the seed the reference tests
@@ -236,12 +254,13 @@ def main():
     ap.add_argument("--grid", default="1deg", choices=sorted(GRIDS))
     ap.add_argument("--batch", type=int, default=None, help="samples per GPU per step (default: 8 at 1 deg, 4 at 0.25 deg = BASELINE configs[1], [2])")
     ap.add_argument("--precision", default=None, choices=["auto", "fp32", "fp32_simt", "bf16"],
-                    help="default: auto at 1 deg (the constructor default: fp32-faithful tcgen05), bf16 at 0.25 deg (configs[2])")  # fmt: skip
+                    help="default: auto at 1 deg (the constructor default: fp32-faithful wgmma), bf16 at 0.25 deg (configs[2])")  # fmt: skip
     ap.add_argument("--boundary", default="gather", choices=["gather", "gather_sync", "loss"], help="what crosses GPUs at the loss boundary (N > 1)")
     ap.add_argument("--gather-mode", default="auto", choices=["auto", "fused", "fused_peer", "p2p_copy", "nccl"],
                     help="transport of the gather boundary: fused into the forecast's last kernel (NVLink multicast / peer stores), copy engines, or NCCL")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-check", action="store_true", help="skip the oracle comparison of this run's output")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's forecast (seeded sample, <= 48 MB) as .npy files")
     a = ap.parse_args()
     if a.batch is None:
         a.batch = 8 if a.grid == "1deg" else 4
@@ -268,7 +287,7 @@ def main():
     cfg = {"workload": None, "grid": {"1deg": "1deg lat -90..89 x lon 0..359 (README.md:48-51)", "0.25deg": "0.25deg ERA5 721 x 1440"}[a.grid],
            "points": n_pts, "batch_per_gpu": a.batch, "global_batch": a.batch * world, "hidden": 256, "processor_blocks": 9,
            "parallelism": f"dp{world} (batch shards; loss boundary: {a.boundary})",
-           "cache": f"inputs per step {a.batch * n_pts * FIN * 4 / 1e6:.0f} MB + weight-constant edge tables stream through HBM each step (> 126 MB L2); no explicit flush"}  # fmt: skip
+           "cache": f"inputs per step {a.batch * n_pts * FIN * 4 / 1e6:.0f} MB + weight-constant edge tables stream through HBM each step (> 50 MB L2); no explicit flush"}  # fmt: skip
 
     if a.impl == "reference":
         if rank != 0:
@@ -385,12 +404,14 @@ def main():
             dist.barrier()
             torch.cuda.synchronize(dev)
 
+    last = {}
+
     def timed(fn, steps):
         sync_all()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            fn()
+            last["y"] = fn()
         cur = torch.cuda.current_stream(dev)
         if gather is not None:
             gather.wait()  # the timed region ends when the last gather has landed ...
@@ -415,6 +436,8 @@ def main():
     tags = plan.timing_read()
     plan.timing_enable(False)
     plan.status()  # raises if any kernel flagged fp16-range overflow or a pipeline fault
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, last["y"])
     for _ in range(2):
         step_e2e()
     ms_e2e = timed(step_e2e, a.steps)
@@ -422,7 +445,7 @@ def main():
     value = world * a.steps / (ms_total / 1000.0)
     e2e_value = world * a.steps / (ms_e2e / 1000.0)
     resolved = model._engine.resolved_precision
-    dtype = {"fp32": "f32 (fp16x2-split tcgen05, fp32 accumulate)", "fp32_tc": "f32 (fp16x2-split tcgen05, fp32 accumulate)",
+    dtype = {"fp32": "f32 (fp16x2-split wgmma, fp32 accumulate)", "fp32_tc": "f32 (fp16x2-split wgmma, fp32 accumulate)",
              "fp32_simt": "f32", "bf16": "bf16"}[resolved]  # fmt: skip
     cfg["workload"] = f"{a.grid}_grid_{n_pts}pts_102to78_batch{a.batch}_per_gpu_{'bf16' if resolved == 'bf16' else 'fp32'}"
     cfg["precision"] = {"requested": a.precision, "resolved": resolved}
@@ -458,8 +481,9 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = peaks.get("bf16_tflops_sustained") or 1400.0
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (kernels timed inside a seconds-long step loop)" if peaks else "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)"
+    peak_tf = peaks.get("bf16_tflops_sustained") or 989.0
+    peak_src = ("MEASURED_PEAKS.json bf16_tflops_sustained (kernels timed inside a seconds-long step loop)" if peaks
+                else "H100 SXM data sheet, dense bf16 at 700 W: 989 TFLOP/s (a bound, not a measured rate)")  # fmt: skip
     f_alg, per = algorithmic_flops(n, ed)
     dom = max((k for k in tags if tags[k][0] and k != "const"), key=lambda k: tags[k][1])
     cnt, ms_dom = tags[dom]

@@ -1,4 +1,4 @@
-"""graph_weather_b200 -- the encode-process-decode GNN forward of openclimatefix/graph_weather, rebuilt for B200 (sm_100a).
+"""graph_weather_b200 -- the encode-process-decode GNN forward of openclimatefix/graph_weather, rebuilt for H100 (sm_90a).
 
 Public names mirror graph_weather/__init__.py:3-9 and graph_weather/models/__init__.py:3-17 for the hot path only.
 """

@@ -91,7 +91,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} not found: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "graph_weather_b200 has no CPU or eager-PyTorch fallback."
         )
     lib = ctypes.CDLL(LIB_PATH)
@@ -141,7 +141,7 @@ class Plan:
         self.lib = load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("graph_weather_b200 runs on CUDA devices only (no CPU path); move the module and its inputs to a B200")
+            raise RuntimeError("graph_weather_b200 runs on CUDA devices only (no CPU path); move the module and its inputs to the H100")
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.dims = GwDims(**dims)

@@ -1,5 +1,5 @@
 """PhysicalConstraintLayer (graph_weather/models/layers/constraint_layer.py:12-188) and the grid <-> graph mapping of
-GraphWeatherForecaster (forecast.py:178-213) for the B200 path.
+GraphWeatherForecaster (forecast.py:178-213) for the CUDA path.
 
 The reference moves every tensor through Python loops over the nodes (`graph_to_grid` / `grid_to_graph`, O(N) Python per
 call) and a handful of eager ops.  Here the mapping is two precomputed index vectors and the constraint itself is

@@ -130,8 +130,8 @@ struct gw_plan {
   DevBuf<float> ebuf0, ebuf1; // [max_batch*n_lat_edges, De]    latent edge state, double buffered
   DevBuf<float> P;            // [max_batch*n_mesh, 2*He]       per-node layer-1 products [W1s x | W1d x]
   size_t total_bytes = 0;
-  // tensor-core path: packed weight images (UMMA operand layout) and their descriptors
-  struct TcW { const void* p = nullptr; const void* p32 = nullptr; int K = 0, N = 0, N32 = 0, n_valid = 0; float winv = 1.f; float gain = 0.f; };  // gain = K * max|W|: |A.W^T| <= gain * max|A|
+  // tensor-core path: packed weight images (GMMA operand layout) and their descriptors
+  struct TcW { const void* p = nullptr; int K = 0, N = 0, N32 = 0, n_valid = 0; float winv = 1.f; float gain = 0.f; };  // gain = K * max|W|: |A.W^T| <= gain * max|A|
   struct TcMlp { TcW w0, w0b, w0c, w1, w2; };  // w0*: slices of the first Linear as each chain needs them
   DevBuf<unsigned char> tc_packed;
   DevBuf<float> tc_absmax;
@@ -296,7 +296,7 @@ static bool is_tc(const gw_plan* p) { return p->d.precision != GW_PREC_FP32_SIMT
 // layer = Linear `w` (+ bias b[l] of MLP m when l >= 0) (+ ReLU); magnitudes for the operand-range ladder travel along
 static TcLayer tc_layer(const gw_plan::TcW& w, const Mlp* m, int l, bool relu, bool feeds) {
   TcLayer L;
-  L.Wp = w.p, L.Wp32 = w.p32, L.K = w.K, L.N = w.N, L.N32 = w.N32, L.n_valid = w.n_valid, L.wscale_inv = w.winv;
+  L.Wp = w.p, L.K = w.K, L.N = w.N, L.N32 = w.N32, L.n_valid = w.n_valid, L.wscale_inv = w.winv;
   L.bias = (m && l >= 0) ? m->b[l] : nullptr, L.relu = relu ? 1 : 0, L.feeds_next = feeds ? 1 : 0;
   L.gain = w.gain, L.off = (m && l >= 0 && (size_t)l < m->bmax.size()) ? m->bmax[l] : 0.f;
   return L;
@@ -496,8 +496,7 @@ static int pack_tc_weights(gw_plan* p, cudaStream_t st) {
   size_t total = 0;
   for (size_t i = 0; i < n; ++i) {
     GW_CUDA(launch_absmax(reqs[i].W, reqs[i].ldw, reqs[i].K, reqs[i].N, p->tc_absmax.p + i, st));
-    total += (tc_packed_bytes(reqs[i].K, reqs[i].N, parts, 1) + 1023) / 1024 * 1024;  // two images: perm16 and perm32 feature order
-    total += (tc_packed_bytes(reqs[i].K, reqs[i].N, parts, 2) + 1023) / 1024 * 1024;
+    total += (tc_packed_bytes(reqs[i].K, reqs[i].N, parts) + 1023) / 1024 * 1024;
   }
   for (size_t i = 0; i < nv; ++i) GW_CUDA(launch_absmax(vreqs[i].v, vreqs[i].n, vreqs[i].n, 1, p->tc_absmax.p + n + i, st));
   std::vector<float> amax(n + nv);
@@ -520,19 +519,16 @@ static int pack_tc_weights(gw_plan* p, cudaStream_t st) {
       scale = std::ldexp(1.f, 12 - e);   // amax * scale in [2048, 4096)
     }
     void* dst = p->tc_packed.p + off;
-    const size_t img = (tc_packed_bytes(reqs[i].K, reqs[i].N, parts, 1) + 1023) / 1024 * 1024;
-    const size_t img32 = (tc_packed_bytes(reqs[i].K, reqs[i].N, parts, 2) + 1023) / 1024 * 1024;
-    GW_CUDA(launch_pack_weights(reqs[i].W, reqs[i].ldw, reqs[i].K, reqs[i].N, scale, parts, 1, dst, st));
-    GW_CUDA(launch_pack_weights(reqs[i].W, reqs[i].ldw, reqs[i].K, reqs[i].N, scale, parts, 2, static_cast<unsigned char*>(dst) + img, st));
+    const size_t img = (tc_packed_bytes(reqs[i].K, reqs[i].N, parts) + 1023) / 1024 * 1024;
+    GW_CUDA(launch_pack_weights(reqs[i].W, reqs[i].ldw, reqs[i].K, reqs[i].N, scale, parts, dst, st));
     reqs[i].out->p = dst;
-    reqs[i].out->p32 = static_cast<unsigned char*>(dst) + img;
     reqs[i].out->K = (reqs[i].K + 63) / 64 * 64;
-    reqs[i].out->N = tc_packed_rows(reqs[i].N, 1);
-    reqs[i].out->N32 = tc_packed_rows(reqs[i].N, 2);
+    reqs[i].out->N = (reqs[i].N + 15) / 16 * 16;  // the layer's output width as the chain checks see it
+    reqs[i].out->N32 = tc_packed_rows(reqs[i].N);   // rows of the packed image
     reqs[i].out->n_valid = reqs[i].N;
     reqs[i].out->winv = 1.f / scale;
     reqs[i].out->gain = (float)reqs[i].K * amax[i];
-    off += img + img32;
+    off += img;
   }
   return 0;
 }
@@ -1125,10 +1121,11 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) {
     GW_CHECK(d.node_dim == 256 && d.edge_dim == 256 && d.hidden_node == 256 && d.hidden_edge == 256,
              "the tensor-core chains are built for 256-wide node/edge/hidden dims (the reference default); use fp32_simt otherwise");
     GW_CHECK(d.hidden_layers_node == 2 && d.hidden_layers_edge == 2, "the tensor-core chains are built for hidden_layers = 2");
-    int cc_major = 0, dev = 0;
+    int cc_major = 0, cc_minor = 0, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, dev);
-    GW_CHECK(cc_major == 10, "the tensor-core chains need an sm_100a device (tcgen05/TMEM)");
+    cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, dev);
+    GW_CHECK(cc_major == 9 && cc_minor == 0, "the tensor-core chains need an sm_90a device (wgmma)");
   }
   int ndev = 0;
   cudaError_t ce = cudaGetDeviceCount(&ndev);
@@ -1153,7 +1150,7 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) {
   const size_t Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, Hn = d.hidden_node;
   const size_t max_hid = std::max({Dn, De, He, Hn, (size_t)d.hidden_dec, (size_t)d.out_dim});
   const size_t max_rows = std::max({(size_t)d.n_in, (size_t)d.n_out, (size_t)d.n_mesh, (size_t)d.n_lat_edges, (size_t)d.n_dec_edges});
-  // chunking: keep the per-pass scratch of the lat/lon-sized stages under ~48 GB.  The tensor-core path never writes the
+  // chunking: keep the per-pass scratch of the lat/lon-sized stages under ~24 GB (an 80 GB H100 also holds the caller's tensors).  The tensor-core path never writes the
   // decoder's e' rows (their per-point sums are formed in the edge chain's epilogue), and its hidden activations stay on
   // the SM, so its per-sample scratch is three lat/lon-sized row buffers; the CUDA-core path also needs e' and the ping-pong.
   const bool tc = d.precision != GW_PREC_FP32_SIMT;
@@ -1161,7 +1158,7 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) {
   const size_t dec_tiles = ((size_t)d.n_dec_edges + 127) / 128, lat_tiles = ((size_t)d.n_lat_edges + 127) / 128;
   const size_t per_sample = tc ? (n_io * Dn + (size_t)d.n_in * De + (size_t)d.n_out * De + dec_tiles * 2048) * sizeof(float)
                                : (2 * max_rows * max_hid + std::max((size_t)d.n_in, (size_t)d.n_dec_edges) * De + n_io * Dn) * sizeof(float);
-  size_t chunk = std::max<size_t>(1, std::min<size_t>(d.max_batch, (48ull << 30) / std::max<size_t>(per_sample, 1)));
+  size_t chunk = std::max<size_t>(1, std::min<size_t>(d.max_batch, (24ull << 30) / std::max<size_t>(per_sample, 1)));
   if (const char* force = getenv("GW_B200_CHUNK")) {  // test knob: exercise the chunked stage loops on small grids
     const long v = atol(force);
     if (v >= 1) chunk = std::min<size_t>((size_t)v, (size_t)d.max_batch);

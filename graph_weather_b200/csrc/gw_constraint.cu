@@ -98,7 +98,7 @@ int gw_constraint_apply(int32_t type, const float* hr, const float* lr, int32_t 
     gw::gw_constraint_means_kernel<<<(unsigned)batch, 256, 0, st>>>(partial, channels, n_nodes, means);
     gw::count_launch(2);
   }
-  gw::gw_constraint_apply_kernel<<<148 * 8, 256, 0, st>>>(type, hr, lr, lr_ld, lr_channels, src, n_nodes, channels, means, exp_factor, out,
+  gw::gw_constraint_apply_kernel<<<gw::GRID_SMS * 8, 256, 0, st>>>(type, hr, lr, lr_ld, lr_channels, src, n_nodes, channels, means, exp_factor, out,
                                                         (int)batch);
   gw::count_launch();
   cudaError_t e = cudaGetLastError();

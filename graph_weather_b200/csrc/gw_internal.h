@@ -8,6 +8,9 @@
 
 namespace gw {
 
+// grid-stride kernels launch a fixed number of blocks per SM of an H100 SXM (132 SMs)
+constexpr int GRID_SMS = 132;
+
 void count_launch(int n = 1);
 void set_error(const std::string& msg);
 
@@ -38,15 +41,14 @@ cudaError_t launch_seg_carry(const float* carry, const int32_t* seg_dst, int row
 cudaError_t launch_segsum(const float* base, int ld, int width, const int32_t* ptr, const int32_t* perm, int src_rows,
                           int rows, int batch, float* out, int ldo, cudaStream_t stream);
 
-// tcgen05 chain kernel (gw_tc3.cu)
+// wgmma chain kernel (gw_tc3.cu)
 cudaError_t launch_chain_tc3(const TcChain& ch, cudaStream_t stream);
 bool tc3_chain_is_lean(const TcChain& ch);  // would the launch take the lean (perm32, 256-bit access) path?
-// Packs W[n, k] (n < N_src rows of stride ldw, k < K_src) into the UMMA operand image the chain kernel streams with
-// cp.async.bulk; `parts` = 2 (fp16 hi, lo) or 1 (bf16).  dst must hold tc_packed_bytes(K_src, N_src, parts, perm).
-size_t tc_packed_bytes(int K_src, int N_src, int parts, int perm);
-int tc_packed_rows(int N_src, int perm);  // rows of the packed image: N padded to 16 (perm16) or 64 (perm32)
-cudaError_t launch_pack_weights(const float* W, int ldw, int K_src, int N_src, float wscale, int parts, int perm, void* dst,
-                                cudaStream_t stream);  // perm: 1 = perm16 (general path), 2 = perm32 (lean path) feature order of gw_tc3.cu (gw_pack.cu)
+// Packs W[n, k] (n < N_src rows of stride ldw, k < K_src) into the GMMA operand image the chain kernel streams with
+// cp.async.bulk (perm32 feature order, gw_pack.cu); `parts` = 2 (fp16 hi, lo) or 1 (bf16).  dst must hold tc_packed_bytes(K_src, N_src, parts).
+size_t tc_packed_bytes(int K_src, int N_src, int parts);
+int tc_packed_rows(int N_src);  // rows of the packed image: N padded to 64
+cudaError_t launch_pack_weights(const float* W, int ldw, int K_src, int N_src, float wscale, int parts, void* dst, cudaStream_t stream);
 cudaError_t launch_absmax(const float* W, int ldw, int K_src, int N_src, float* out_max, cudaStream_t stream);
 
 // device-side observation graph of the assimilator (gw_graph.cu)

@@ -66,7 +66,7 @@ __global__ void gw_loss_final_kernel(const double* __restrict__ partial, int n, 
   if (threadIdx.x == 0) *out = tot;
 }
 
-constexpr int LOSS_GRID = 148 * 8;
+constexpr int LOSS_GRID = GRID_SMS * 8;
 
 // d(sum) / d pred[b, n, f] * scale = scale * w(n) * 2 (pred - target) * inv_var(f) / F          (losses.py:70-94 differentiated)
 __global__ void __launch_bounds__(256) gw_loss_grad_kernel(const float* __restrict__ pred, const float* __restrict__ target,
@@ -98,7 +98,7 @@ int gw_normalized_mse_loss_grad(const float* pred, const float* target, const fl
     gw::set_error("gw_normalized_mse_loss_grad: bad shape");
     return 1;
   }
-  gw::gw_loss_grad_kernel<<<148 * 8, 256, 0, (cudaStream_t)stream>>>(pred, target, inv_variance, node_weight, (long long)batch * n_nodes, (int)n_nodes,
+  gw::gw_loss_grad_kernel<<<gw::GRID_SMS * 8, 256, 0, (cudaStream_t)stream>>>(pred, target, inv_variance, node_weight, (long long)batch * n_nodes, (int)n_nodes,
                                                                    n_features, scale_dev, scale, grad_pred);
   gw::count_launch();
   const cudaError_t e = cudaGetLastError();

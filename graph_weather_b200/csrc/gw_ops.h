@@ -64,10 +64,9 @@ struct GemmOp {
 constexpr int TC_MAX_LAYERS = 8;
 
 struct TcLayer {
-  const void* Wp = nullptr;   // packed weights (gw_pack.cu): [K/64][parts][N x 64] fp16/bf16, UMMA SW128 K-major, perm16 feature order
-  const void* Wp32 = nullptr; // the same weights in perm32 feature order (lean path of gw_tc3.cu); the launcher picks
+  const void* Wp = nullptr;   // packed weights (gw_pack.cu): [K/64][parts][N32 x 64] fp16/bf16, GMMA SW128 K-major, perm32 feature order
   int32_t K = 0, N = 0;       // K multiple of 64 (zero padded), N multiple of 16 (<= 256)
-  int32_t N32 = 0;            // rows of the perm32 image (N padded to 64): the N the lean path runs this layer with
+  int32_t N32 = 0;            // rows of the perm32 image (N padded to 64): the N the chain kernel runs this layer with
   int32_t n_valid = 0;        // real output columns (<= N); bias / LN parameters / addends exist only for these
   float wscale_inv = 1.f;     // weights are stored times a power of two; the accumulator is multiplied by this
   const float* bias = nullptr;

@@ -1,7 +1,7 @@
 // gw_pack.cu -- one-off packing of nn.Linear weights into the operand images the tensor-core chain kernel (gw_tc3.cu) streams:
 // fp16 hi|lo (fp32-faithful mode) or bf16, K-major, SWIZZLE_128B, one contiguous panel per 64-wide K chunk, power-of-two
-// pre-scaled, output rows and K columns permuted inside every group of 16 (perm16) or 32 (perm32) -- the two feature orders of the
-// chain kernel's general and lean paths, see gw_tc3.cu.
+// pre-scaled, output rows and K columns permuted inside every group of 32 (perm32) -- the feature order of the chain kernel's
+// wgmma accumulator fragments, see gw_tc3.cu.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -15,28 +15,22 @@ namespace gw {
 // weight packing (one-off per weight set)
 // ------------------------------------------------------------------------------------------------------------------
 static inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
-// rows of a packed image: the perm16 image (general path) pads N to 16, the perm32 image (lean path: 64-column epilogue chunks)
-// to 64 -- only the forecast's 78-column output layer differs (80 vs 128 rows)
-int tc_packed_rows(int N_src, int perm) { return round_up(N_src, perm == 2 ? 64 : 16); }
-size_t tc_packed_bytes(int K_src, int N_src, int parts, int perm) {
-  return (size_t)(round_up(K_src, 64) / 64) * parts * tc_packed_rows(N_src, perm) * 128;
+// rows of a packed image: N padded to 64 (the kernel's 64-column epilogue chunks; the forecast's 78-column output layer has 128)
+int tc_packed_rows(int N_src) { return round_up(N_src, 64); }
+size_t tc_packed_bytes(int K_src, int N_src, int parts) {
+  return (size_t)(round_up(K_src, 64) / 64) * parts * tc_packed_rows(N_src) * 128;
 }
 
 // dst image: for chunk kc, part p: panel of N rows x 128 B; element (n, k): 16B chunk ((k%64)/8) ^ (n&7), half k%8
-// perm16 (gw_tc3.cu): inside every group of 16 output rows and of 16 K columns, packed position a holds logical index
-// f(a) = 4*((a>>1)&3) + 2*(a>>3) + (a&1), the order in which a tcgen05.ld.16x256b fragment gives each thread 4 consecutive features.
-__host__ __device__ inline int perm16_f(int a) { return (a & ~15) | (4 * ((a >> 1) & 3) + 2 * ((a >> 3) & 1) + (a & 1)); }
-// perm32 (lean path, tcgen05.ld.16x256b.x4 fragments: a thread owns 8 consecutive features of a row): inside every group of 32,
+// perm32 (wgmma accumulator fragments: a thread owns 8 consecutive features of a row): inside every group of 32,
 // packed position a = 8g + 2c + e holds logical index 8c + 2g + e.
 __host__ __device__ inline int perm32_f(int a) { return (a & ~31) | (8 * ((a >> 1) & 3) + 2 * ((a >> 3) & 3) + (a & 1)); }
 __global__ void gw_pack_weights_kernel(const float* __restrict__ W, int ldw, int K_src, int N_src, int Kp, int Np,
-                                       float wscale, int parts, int perm, uint8_t* __restrict__ dst) {
+                                       float wscale, int parts, uint8_t* __restrict__ dst) {
   const size_t total = (size_t)Np * Kp;
   for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
     const int n = (int)(e / Kp), k = (int)(e % Kp);
-    // perm: 0 none, 1 perm16, 2 perm32 (rows padded to 64, K is always a multiple of 64)
-    const int ns = perm == 2 ? perm32_f(n) : (perm ? perm16_f(n) : n);
-    const int ks = perm == 2 ? perm32_f(k) : (perm ? perm16_f(k) : k);
+    const int ns = perm32_f(n), ks = perm32_f(k);  // (rows padded to 64, K is always a multiple of 64)
     const float w = (ns < N_src && ks < K_src) ? W[(size_t)ns * ldw + ks] * wscale : 0.f;
     const int kc = k >> 6, kk = k & 63;
     const size_t panel = (size_t)Np * 128;
@@ -52,10 +46,10 @@ __global__ void gw_pack_weights_kernel(const float* __restrict__ W, int ldw, int
   }
 }
 
-cudaError_t launch_pack_weights(const float* W, int ldw, int K_src, int N_src, float wscale, int parts, int perm, void* dst,
+cudaError_t launch_pack_weights(const float* W, int ldw, int K_src, int N_src, float wscale, int parts, void* dst,
                                 cudaStream_t stream) {
-  const int Kp = round_up(K_src, 64), Np = tc_packed_rows(N_src, perm);
-  gw_pack_weights_kernel<<<256, 256, 0, stream>>>(W, ldw, K_src, N_src, Kp, Np, wscale, parts, perm, static_cast<uint8_t*>(dst));
+  const int Kp = round_up(K_src, 64), Np = tc_packed_rows(N_src);
+  gw_pack_weights_kernel<<<256, 256, 0, stream>>>(W, ldw, K_src, N_src, Kp, Np, wscale, parts, static_cast<uint8_t*>(dst));
   count_launch();
   return cudaGetLastError();
 }

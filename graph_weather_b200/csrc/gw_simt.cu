@@ -3,7 +3,7 @@
 // One kernel executes any gw::GemmOp: it assembles A rows from their row sources while staging them to shared
 // memory (so the reference's cat / gather / scatter_sum intermediates never exist in HBM), runs an fp32 FFMA
 // tile GEMM, and applies bias + gathered addends + ReLU + LayerNorm + residual in registers before one coalesced
-// store.  It serves (a) every op of the forward when hidden sizes are not the 256 the tcgen05 kernel is built for,
+// store.  It serves (a) every op of the forward when hidden sizes are not the 256 the wgmma kernel is built for,
 // (b) the one-off weight-constant precompute, and (c) as the on-device fp32 cross-check of the tensor-core path.
 //
 // Tile: 64 rows x 256 cols per CTA (so a LayerNorm row never leaves the CTA), BK = 16, 256 threads; each thread
@@ -452,7 +452,7 @@ cudaError_t launch_ln_bwd(const float* dy, int ld_dy, const float* z, int ld_z, 
                           float* dgamma, float* dbeta, cudaStream_t st) {
   if (R <= 0) return cudaSuccess;
   if (N > 256) return cudaErrorInvalidValue;
-  gw_ln_bwd_kernel<<<(unsigned)std::min<long long>(148 * 8, (R + 7) / 8), 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, dgamma, dbeta);
+  gw_ln_bwd_kernel<<<(unsigned)std::min<long long>(GRID_SMS * 8, (R + 7) / 8), 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, dgamma, dbeta);
   count_launch();
   return cudaGetLastError();
 }
@@ -472,7 +472,7 @@ __global__ void gw_batch_reduce_kernel(const float* __restrict__ in, int ld_in, 
 cudaError_t launch_batch_reduce(const float* in, int ld_in, long long rows, int width, int batch, float* out, int ld_out, bool accumulate,
                                 cudaStream_t st) {
   if (rows <= 0 || width <= 0) return cudaSuccess;
-  gw_batch_reduce_kernel<<<148 * 4, 256, 0, st>>>(in, ld_in, rows, width, batch, out, ld_out, accumulate ? 1 : 0);
+  gw_batch_reduce_kernel<<<GRID_SMS * 4, 256, 0, st>>>(in, ld_in, rows, width, batch, out, ld_out, accumulate ? 1 : 0);
   count_launch();
   return cudaGetLastError();
 }
@@ -500,7 +500,7 @@ cudaError_t launch_gather_rows(const float* in, int ld_in, int src_rows, const i
                                int ld_out, bool accumulate, cudaStream_t st) {
   if (rows <= 0 || batch <= 0) return cudaSuccess;
   if ((width & 3) || (ld_in & 3) || (ld_out & 3)) return cudaErrorInvalidValue;
-  gw_gather_rows_kernel<<<148 * 8, 256, 0, st>>>(in, ld_in, src_rows, idx, rows, width, batch, out, ld_out, accumulate ? 1 : 0);
+  gw_gather_rows_kernel<<<GRID_SMS * 8, 256, 0, st>>>(in, ld_in, src_rows, idx, rows, width, batch, out, ld_out, accumulate ? 1 : 0);
   count_launch();
   return cudaGetLastError();
 }
@@ -515,7 +515,7 @@ __global__ void gw_strided_add_kernel(const float* __restrict__ src, int ld_src,
 }
 cudaError_t launch_strided_add(const float* src, int ld_src, float* dst, int ld_dst, long long rows, int width, cudaStream_t st) {
   if (rows <= 0 || width <= 0) return cudaSuccess;
-  gw_strided_add_kernel<<<148 * 4, 256, 0, st>>>(src, ld_src, dst, ld_dst, rows, width);
+  gw_strided_add_kernel<<<GRID_SMS * 4, 256, 0, st>>>(src, ld_src, dst, ld_dst, rows, width);
   count_launch();
   return cudaGetLastError();
 }
@@ -565,7 +565,7 @@ __global__ void __launch_bounds__(256) gw_pad_rows_kernel(const float* __restric
 cudaError_t launch_pad_rows(const float* src, int ld_src, int width, float* dst, int ld_dst, long long rows, float* amax, cudaStream_t stream) {
   if (rows <= 0) return cudaSuccess;
   if (ld_dst & 3) return cudaErrorInvalidValue;
-  gw_pad_rows_kernel<<<148 * 8, 256, 0, stream>>>(src, ld_src, width, dst, ld_dst, rows, amax);
+  gw_pad_rows_kernel<<<GRID_SMS * 8, 256, 0, stream>>>(src, ld_src, width, dst, ld_dst, rows, amax);
   count_launch();
   return cudaGetLastError();
 }
@@ -590,7 +590,7 @@ __global__ void __launch_bounds__(256) gw_absmax_flat_kernel(const float* __rest
 }
 cudaError_t launch_absmax_flat(const float* p, long long n, float* amax, cudaStream_t stream) {
   if (n <= 0) return cudaSuccess;
-  gw_absmax_flat_kernel<<<148 * 4, 256, 0, stream>>>(p, n, amax);
+  gw_absmax_flat_kernel<<<GRID_SMS * 4, 256, 0, stream>>>(p, n, amax);
   count_launch();
   return cudaGetLastError();
 }

@@ -1,47 +1,37 @@
-// gw_tc3.cu -- the fused MLP-chain kernel on Blackwell tensor cores (tcgen05 + TMEM), precision GW_PREC_FP32_TC / BF16_TC.
+// gw_tc3.cu -- the fused MLP-chain kernel on Hopper tensor cores (wgmma, fp32 accumulation in registers), precision
+// GW_PREC_FP32_TC / BF16_TC.
 //
 // One persistent CTA per SM walks 128-row tiles of a gw::TcChain.  For every tile the whole chain
 //     A0 = assemble(row sources)                                   (stream / gather / relu(gather+const) ...)
-//     for each layer:  D = A . W^T  (tcgen05.mma, fp32 accumulate in TMEM)
+//     for each layer:  D = A . W^T  (wgmma.mma_async, fp32 accumulate in registers)
 //                      v = D*s + bias + gathered addends ; ReLU | LayerNorm ; + residual
 //                      v -> global (fp32)  and/or  v -> split fp16 hi/lo -> shared memory = A operand of the next layer
 // runs without the activations ever leaving the SM: the reference's x[row]/x[col] gathers, cat, 3 Linear + LayerNorm and
 // residual (graph_net_block.py:131-135, 184-191) are one kernel per edge pass and one per node pass.
 //
 // fp32 fidelity on fp16 tensor cores: every fp32 operand a is split a = hi + lo (two fp16, 22 significand bits) and each
-// product is hi*hi + lo*hi + hi*lo with fp32 accumulation in TMEM.  Weights are pre-scaled by a power of two so their lo
-// parts stay normal; the scale is undone exactly in the epilogue.
+// product is hi*hi + lo*hi + hi*lo with fp32 accumulation.  Weights are pre-scaled by a power of two so their lo parts stay
+// normal; the scale is undone exactly in the epilogue.
 //
-// Layout of the work (third generation; the second, with mover warps and shared-memory staging -- git history, profiles/r01_c_* --
-// spent 40 % of its time in mbarrier hand-offs, measured with tools/ablate.py):
-//   * 16 worker warps, four per TMEM lane quadrant.  A worker reads the accumulator with tcgen05.ld.16x256b, whose register
-//     fragment gives four adjacent lanes one row.  The weights are packed with output rows and K columns permuted inside groups
-//     of 16 (perm16, gw_pack.cu) so that a thread's fragment is four CONSECUTIVE features of a row: in that layout the workers
-//     load gathered addends / residual rows and store outputs DIRECTLY from/to global memory with 16-byte accesses (8 rows x 64 B
-//     per warp instruction, every fetched sector fully used): no staging buffers, no mover warps, no hand-off barriers.  Loads
-//     for the next 64-column chunk (global operands and the accumulator chunk itself) are issued while the current one is
-//     converted.
-//   * the A operand ring holds a full K = 256 operand (4 chunks x [128 x 64] hi|lo = 128 KB).  Because a layer's epilogue
-//     starts only when that layer's MMAs have completed, every operand slot is known to be free when the epilogue refills
-//     it: per tile a worker waits on 1 barrier per layer (accumulator complete) and arrives on 1 per produced chunk, one
-//     elected lane per warp.
-//   * the stage-0 operand of the NEXT tile is assembled before the current tile's last epilogue, slot by slot as the last
-//     layer's MMAs release them (empty_a): the assembly overlaps the tail of those MMAs, and the tensor pipe then runs the next
-//     tile's first layer on the other accumulator under the LayerNorm epilogue of this tile.
-//   * two instantiations per precision: the lean path (every source / output 16-byte aligned and as wide as the layer; rows are a
-//     warp-uniform 64-bit base + 32-bit offsets; the epilogue is specialised per feature mask) and the general path (any width /
-//     alignment).  setmaxnreg gives the workers 120 registers and the auxiliary warpgroup 32; the lean path has no spills.
-//   * warp 16: weight producer (cp.async.bulk of pre-swizzled 32 KB panels), warp 17: MMA issuer (one thread).
-// TMEM: 512 columns = two 128x256 fp32 accumulators alternating by layer.
-//
-// Round 2:
-//   * tile rows are handed to threads so that a thread's four rows are CONSECUTIVE logical rows (re[k] = 32 q + 4 (lane/4) + k;
-//     the TMEM lane / operand row stays rt[k]); the last layer of an edge chain can then reduce its rows per target node in
-//     registers + two shuffles (graph_net_block.py:188 scatter_sum, edges are target-sorted, segments of <= 8 rows) and store
-//     per-node sums: the decoder's e' rows are never written, the separate segment-sum launches disappear.
-//   * the lean path is shaped at compile time (chunks per source / per layer are template constants): every chunk loop is
-//     fully unrolled, rows are 64-bit pointers resolved once per layer and chunk offsets are immediates; the rolled loops
-//     of round 1 spent ~45 % of their instructions on register rotation and address arithmetic (profiles/r02_*).
+// Layout of the work:
+//   * two consumer warpgroups.  Warpgroup w owns the tile rows 64 w .. 64 w + 63 for the whole chain: it assembles their stage-0
+//     operand, issues the m64nNk16 wgmma of every layer over them and runs each layer's epilogue on its own accumulator registers
+//     (a 64 x 256 fp32 accumulator is 128 registers per thread).  A warpgroup writes and reads only its own operand rows, so the
+//     two warpgroups share nothing but the weight stream.
+//   * the wgmma accumulator gives lane t of warp q the rows 16 q + t/4 (+ 8) and, in every 8 columns, the pair 2 (t%4) + {0,1}.
+//     The weights are packed with output rows and K columns permuted inside groups of 32 (perm32, gw_pack.cu) so that in every
+//     32-column step a thread holds EIGHT CONSECUTIVE features of two rows: gathered addends / residual rows are loaded and
+//     outputs stored directly from/to global memory with pairs of 128-bit accesses (four adjacent lanes cover one 128-byte line), no
+//     staging.  Tile rows are handed out so that a thread's two rows are CONSECUTIVE logical rows (fr0, fr0 + 1 <-> operand rows
+//     16 q + t/4 and + 8): the last layer of an edge chain reduces its rows per target node in registers and shuffles
+//     (graph_net_block.py:188 scatter_sum, edges are target-sorted, segments of <= 8 rows) and stores per-node sums.
+//   * the A operand lives in four 64-column slots ([128 x 64] hi|lo, 128 KB); a stage-0 operand wider than 256 columns is
+//     assembled and multiplied in windows of four slots.  The result of a layer overwrites its own operand once that layer's
+//     wgmma have completed.
+//   * two instantiations per precision: the lean path (every source / output 32-byte aligned and as wide as the layer; the
+//     epilogue is specialised per feature mask and fully unrolled) and the general path (any width / alignment).
+//   * warp 8: weight producer (cp.async.bulk of pre-swizzled panels of up to 32 KB, two stages).  setmaxnreg gives the
+//     consumers 240 registers and the producer warpgroup 24.
 //   * operand range: every tensor carries a rigorous magnitude bound (device float); each CTA derives, per layer, the power
 //     of two that brings the next fp16-split operand under 2^15 and folds its inverse into the accumulator scale, so raw
 //     (unnormalised) inputs cannot overflow fp16.  The amax status bit stays as a guard.
@@ -65,170 +55,34 @@ namespace t3 {
 #else
 #define ABL3(bit) false
 #endif
-enum { ABL_FENCE = 1, ABL_LOADS = 2, ABL_CONVERT = 4, ABL_STORES = 8, ABL_LN = 16, ABL_TMEM = 32, ABL_MMA = 64, ABL_WEIGHTS = 128 };
+// the consumer's helpers are lambdas over the kernel's state: inlined, so that the accumulator array stays in registers
+#define GW_INLINE __attribute__((always_inline))
+enum { ABL_FENCE = 1, ABL_LOADS = 2, ABL_CONVERT = 4, ABL_STORES = 8, ABL_LN = 16, ABL_WEIGHTS = 128 };
 
 // epilogue feature mask of a layer (TcLayer::kind); the lean path is instantiated for the masks that occur
 enum { F_ADD0 = 1, F_ADD1 = 2, F_RELU = 4, F_LN = 8, F_RES = 16, F_OUT = 32, F_FEEDS = 64, F_SEG = 128, F_NARROW = 256 };
-#ifndef GW_CHUNK_UNROLL
-#define GW_CHUNK_UNROLL 1  // the per-chunk loops stay rolled: unrolled, their code no longer fits the instruction cache
-#endif
-constexpr int CHUNK_UNROLL = GW_CHUNK_UNROLL;
 constexpr int TILE_M = 128;
 constexpr int A_SLOTS = 4, B_STAGES = 2;
 constexpr int A_HALF_BYTES = TILE_M * 128;      // [128 rows x 64 halfs]
 constexpr int A_SLOT_BYTES = 2 * A_HALF_BYTES;  // hi | lo
 constexpr int B_STAGE_BYTES = 256 * 128;        // [256 rows x 64 halfs], hi OR lo panel
-constexpr int WSPLIT = 4;                       // worker warps per TMEM lane quadrant; each owns 16 columns of every 64-column chunk
-constexpr int WORKER_WARPS = 4 * WSPLIT, NUM_WORKERS = 32 * WORKER_WARPS;
-constexpr int WARP_PRODUCER = WORKER_WARPS, WARP_MMA = WORKER_WARPS + 1;
-constexpr int NUM_THREADS = NUM_WORKERS + 128;  // + one auxiliary warpgroup: producer, MMA issuer, two idle warps
-constexpr int WORKER_REGS = 104, AUX_REGS = 56;  // setmaxnreg moves registers inside the CTA's launch allocation only (640 x 96): 512 x 104 + 128 x 56 = 60416 <= 61440.  (112 / 48 needs 63488: the workers' setmaxnreg.inc then never completes -- round-2 deadlock)
+constexpr int CONSUMERS = 2;                    // warpgroups, 64 tile rows each
+constexpr int CONSUMER_WARPS = 4 * CONSUMERS, NUM_WORKERS = 32 * CONSUMER_WARPS;
+constexpr int WARP_PRODUCER = CONSUMER_WARPS;
+constexpr int NUM_THREADS = NUM_WORKERS + 128;  // + one producer warpgroup (one active warp)
+constexpr int WORKER_REGS = 240, AUX_REGS = 24;  // 256 x 240 + 128 x 24 = 384 x 168: the launch allocation of __launch_bounds__(384, 1)
 constexpr int PAR_LAYERS = 6;
 constexpr int OFF_A = 0;
 constexpr int OFF_B = A_SLOTS * A_SLOT_BYTES;
 constexpr int OFF_BAR = OFF_B + B_STAGES * B_STAGE_BYTES;
-constexpr int NUM_BARS = 2 * A_SLOTS + 2 * B_STAGES + 4;
-constexpr int OFF_TMEM = OFF_BAR + NUM_BARS * 8;
-constexpr int OFF_PAR = OFF_TMEM + 16;                // float bias[PAR_LAYERS][256]
+constexpr int NUM_BARS = 2 * B_STAGES;
+constexpr int OFF_PAR = OFF_BAR + 2 * NUM_BARS * 8;   // float bias[PAR_LAYERS][256]
 constexpr int OFF_LNP = OFF_PAR + PAR_LAYERS * 1024;  // float gamma_beta[2][2][256]
-constexpr int OFF_LN = OFF_LNP + 4 * 1024;            // float ln_xy[2][2][WSPLIT][128]: row statistics exchange (mean, M2), two generations
-constexpr int OFF_PRE = OFF_LN + 2 * 2 * WSPLIT * 128 * 4;  // uint32 pre[4][NUM_WORKERS]: layer-0 gather rows of the coming tile (2 rows x 2 addends per thread)
-constexpr int OFF_SCL = OFF_PRE + 4 * NUM_WORKERS * 4;  // float scl[2 * PAR_LAYERS + 4]: per layer {accumulator scale, operand scale of the result}, then the stage-0 operand scale
+constexpr int OFF_SCL = OFF_LNP + 4 * 1024;           // float scl[2 * PAR_LAYERS + 4]: per layer {accumulator scale, operand scale of the result}, then the stage-0 operand scale
 constexpr int SMEM_BYTES = OFF_SCL + (2 * PAR_LAYERS + 4) * 4;
 static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
 static_assert(OFF_B % 1024 == 0 && A_SLOT_BYTES % 1024 == 0 && B_STAGE_BYTES % 1024 == 0, "SWIZZLE_128B needs 1 KB alignment");
 
-// tcgen05.ld 16 lanes x 256 bit, x2: 16 accumulator columns of 16 rows.  Lane t holds (cute SM100_TMEM_LOAD_16dp256b2x):
-//   r0,r1 = (row t/4    , cols 2(t%4)+{0,1})      r2,r3 = (row t/4 + 8, same cols)
-//   r4,r5 = (row t/4    , cols 8+2(t%4)+{0,1})    r6,r7 = (row t/4 + 8, same cols)
-__device__ __forceinline__ void tmem_ld_16x256b_x2(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.16x256b.x2.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-// x4: 32 accumulator columns of 16 rows; register 4 g + 2 m + e = (row t/4 + 8 m, column 8 g + 2 (t%4) + e)
-__device__ __forceinline__ void tmem_ld_16x256b_x4(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.16x256b.x4.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// Wait for TMEM loads that were issued earlier into v (asynchronously: the compiler believes v was written by the issuing
-// statement).  Passing v through the wait as in/out operands makes every later read of v depend on the wait.
-__device__ __forceinline__ void tmem_wait_ld_into(float (&v)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]), "+f"(v[8]), "+f"(v[9]),
-                 "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15])
-               :
-               : "memory");
-}
-
-// A worker thread's fragment of one 64-column chunk: 16 values, index i = 8g + 4j + 2m + e
-//   tile row  r(k) = 32 q + 16 g + lane/4 + 8 m   (k = 2g + m),   accumulator column = 16 hq + 8 j + 2 (lane%4) + e
-// The weights are packed with their output rows AND K columns permuted inside every group of 16 (perm16, gw_pack.cu) so that
-// accumulator column 8j + 2(lane%4) + e holds LOGICAL feature 4 (lane%4) + 2j + e: a thread owns 4 consecutive features of a row
-// (16 bytes of fp32) -> global loads / stores are 128-bit, four adjacent lanes cover 64 B of one row.  Operands live in shared
-// memory in accumulator order on both sides of every product, so nothing else changes.
-__device__ __forceinline__ bool vec2_ok(const float* base, int ld) { return ((reinterpret_cast<uintptr_t>(base) & 7) == 0) && ((ld & 1) == 0); }
-__device__ __forceinline__ bool src_gathered(int kind) { return kind == SRC_GATHER || kind == SRC_BGATHER || kind == SRC_GATHER_BCAST_RELU; }
-__device__ __forceinline__ bool src_per_sample(int kind) { return kind == SRC_STREAM || kind == SRC_GATHER || kind == SRC_GATHER_BCAST_RELU; }
-
-// source rows of my four tile rows (gather indices are the only per-tile state a source needs in registers; everything
-// else is re-read from the kernel parameters where it is used)
-__device__ __forceinline__ void rows_of(const RowSrc& s, int i0, const int (&rl)[4], int (&ri)[4]) {
-  const bool g = src_gathered(s.kind);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) ri[k] = g ? __ldg(s.idx + i0 + rl[k]) : i0 + rl[k];
-}
-// my 16 values (4 rows x logical columns col .. col+3; `col` includes 16hq + 4(lane%4)).  Warp-uniform tiers: 128-bit loads when
-// the warp's 16 columns lie inside the source and rows are 16-byte aligned, 64-bit when 8-byte aligned (the 102-wide
-// features), else bounds-checked scalars.
-__device__ __forceinline__ bool vec4_ok(const float* base, int ld) { return ((reinterpret_cast<uintptr_t>(base) & 15) == 0) && ((ld & 3) == 0); }
-__device__ __forceinline__ void load16(const float* base, int ld, int width, const int (&ri)[4], int col, int lc, float (&o)[16]) {
-  const bool inside = col - 4 * lc + 16 <= width;
-  if (inside && vec4_ok(base, ld)) {
-    float4 t[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) t[k] = __ldg(reinterpret_cast<const float4*>(base + (size_t)ri[k] * (size_t)ld + col));
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int i = 8 * (k >> 1) + 2 * (k & 1);
-      o[i] = t[k].x, o[i + 1] = t[k].y, o[i + 4] = t[k].z, o[i + 5] = t[k].w;
-    }
-  } else if (inside && vec2_ok(base, ld)) {
-    float2 t[8];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float* rowp = base + (size_t)ri[k] * (size_t)ld + col;
-      t[2 * k] = __ldg(reinterpret_cast<const float2*>(rowp));
-      t[2 * k + 1] = __ldg(reinterpret_cast<const float2*>(rowp + 2));
-    }
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int i = 8 * (k >> 1) + 2 * (k & 1);
-      o[i] = t[2 * k].x, o[i + 1] = t[2 * k].y, o[i + 4] = t[2 * k + 1].x, o[i + 5] = t[2 * k + 1].y;
-    }
-  } else {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float* rowp = base + (size_t)ri[k] * (size_t)ld;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int i = 8 * (k >> 1) + 4 * j + 2 * (k & 1), c = col + 2 * j;
-        o[i] = (c < width) ? __ldg(rowp + c) : 0.f;
-        o[i + 1] = (c + 1 < width) ? __ldg(rowp + c + 1) : 0.f;
-      }
-    }
-  }
-}
-__device__ __forceinline__ void load16(const RowSrc& s, int b, const int (&ri)[4], int col, int lc, float (&o)[16]) {
-  const float* base = s.base + (src_per_sample(s.kind) ? (size_t)b * (size_t)s.src_rows * (size_t)s.ld : (size_t)0) + s.col0;
-  load16(base, s.ld, s.width, ri, col, lc, o);
-}
-
-// Split my 16 values into fp16 hi/lo (or bf16) and store them into the swizzled K-major operand slot: row r, logical
-// 16-byte chunk c16 = 2hq + j lives at chunk position c16 ^ (r & 7); my two halfs sit at byte 4 (lane%4) of the chunk.
-__device__ __forceinline__ void store_operand16(uint8_t* slot, const int (&rt)[4], int hq, int lc, const float (&v)[16], bool split,
-                                                float& amax) {
-#pragma unroll
-  for (int g = 0; g < 2; ++g)
-#pragma unroll
-    for (int m = 0; m < 2; ++m) {
-      const int r = rt[2 * g + m];
-      uint8_t* row_hi = slot + r * 128 + 4 * lc;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const float a0 = v[8 * g + 4 * j + 2 * m], a1 = v[8 * g + 4 * j + 2 * m + 1];
-        amax = fmaxf(amax, fmaxf(fabsf(a0), fabsf(a1)));
-        const int pos = ((2 * hq + j) ^ (r & 7)) << 4;
-        if (split) {
-          const __half2 hh = __floats2half2_rn(a0, a1);
-          const float2 hf = __half22float2(hh);
-          const __half2 ll = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
-          *reinterpret_cast<__half2*>(row_hi + pos) = hh;
-          *reinterpret_cast<__half2*>(row_hi + A_HALF_BYTES + pos) = ll;
-        } else {
-          *reinterpret_cast<__nv_bfloat162*>(row_hi + pos) = __floats2bfloat162_rn(a0, a1);
-        }
-      }
-    }
-}
-
-
-// ---- lean full-width path --------------------------------------------------------------------------------------------
-// When every source / output of a layer is 16-byte aligned and at least as wide as the layer (the processor and decoder edge
-// and node passes: >95 % of the run time), a source is four 64-bit row pointers per thread (one per row of mine, my first
-// column folded in), resolved once per layer; every access is pointer + immediate.
 template <int I, int N, class Fn>
 __device__ __forceinline__ void static_for(Fn&& f) {
   if constexpr (I < N) {
@@ -239,6 +93,8 @@ __device__ __forceinline__ void static_for(Fn&& f) {
 template <int V>
 using ic = std::integral_constant<int, V>;
 
+__device__ __forceinline__ bool src_gathered(int kind) { return kind == SRC_GATHER || kind == SRC_BGATHER || kind == SRC_GATHER_BCAST_RELU; }
+__device__ __forceinline__ bool src_per_sample(int kind) { return kind == SRC_STREAM || kind == SRC_GATHER || kind == SRC_GATHER_BCAST_RELU; }
 __device__ __forceinline__ const char* src_sample_base(const RowSrc& s, int b) {
   return reinterpret_cast<const char*>(s.base + (src_per_sample(s.kind) ? (size_t)b * (size_t)s.src_rows * (size_t)s.ld : (size_t)0) + s.col0);
 }
@@ -254,18 +110,38 @@ __device__ __forceinline__ void row_ptrs2(const RowSrc& s, int b, int i0, const 
     for (int k = 0; k < 2; ++k) p[k] = base + (size_t)(uint32_t)(i0 + rl[k]) * ldb;
   }
 }
-// 8 consecutive floats (32-byte aligned) in one 256-bit load: four adjacent lanes cover one full 128-byte line
+// 8 consecutive floats (32-byte aligned) in two 128-bit accesses: four adjacent lanes cover one full 128-byte line
 __device__ __forceinline__ void ld256(const char* p, float* o) {
-  asm volatile("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
+  asm volatile("ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%8];\n\t"
+               "ld.global.nc.v4.f32 {%4, %5, %6, %7}, [%8+16];"
                : "=f"(o[0]), "=f"(o[1]), "=f"(o[2]), "=f"(o[3]), "=f"(o[4]), "=f"(o[5]), "=f"(o[6]), "=f"(o[7])
                : "l"(p));
 }
 __device__ __forceinline__ void st256(char* p, float a, float b, float c, float d, float e, float f, float g, float h) {
-  asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d), "f"(e), "f"(f), "f"(g), "f"(h)
+  asm volatile("st.global.v4.f32 [%0], {%1, %2, %3, %4};\n\t"
+               "st.global.v4.f32 [%0+16], {%5, %6, %7, %8};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d), "f"(e), "f"(f), "f"(g), "f"(h)
                : "memory");
 }
-// Lean-path fragment (tcgen05.ld.16x256b.x4, perm32): index 4 g + 2 m + e = (row m of my two, feature 2 g + e of my eight).
-// FR(m, t): fragment index of (row m, feature t); PX(i): row-order index 8 m + t of fragment index i.
+// General path: logical columns col .. col+7 of one row (zero at and beyond `width`), widest access the row's alignment allows
+__device__ __forceinline__ void load8(const float* rowp, int col, int width, float* o) {
+  const float* p = rowp + col;
+  if (col + 8 <= width && (reinterpret_cast<uintptr_t>(p) & 31) == 0) {
+    ld256(reinterpret_cast<const char*>(p), o);
+  } else if (col + 8 <= width && (reinterpret_cast<uintptr_t>(p) & 15) == 0) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p + 4));
+    o[0] = a.x, o[1] = a.y, o[2] = a.z, o[3] = a.w, o[4] = b.x, o[5] = b.y, o[6] = b.z, o[7] = b.w;
+  } else {
+#pragma unroll
+    for (int t = 0; t < 8; ++t) o[t] = (col + t < width) ? __ldg(p + t) : 0.f;
+  }
+}
+// row `r` (a tile row, clamped) of a source, as a float pointer at its first column (general path)
+__device__ __forceinline__ const float* src_row(const RowSrc& s, int b, int i0, int r) {
+  const int i = src_gathered(s.kind) ? __ldg(s.idx + i0 + r) : i0 + r;
+  return reinterpret_cast<const float*>(src_sample_base(s, b)) + (size_t)(uint32_t)i * (size_t)s.ld;
+}
+// Fragment of one 32-column step (16 accumulator registers, 16 u .. 16 u + 15): index 4 g + 2 m + e = (row m of my two,
+// feature 2 g + e of my eight).  FR(m, t): fragment index of (row m, feature t); PX(i): row-order index 8 m + t of fragment index i.
 __host__ __device__ constexpr int FR(int m, int t) { return 4 * (t >> 1) + 2 * m + (t & 1); }
 __host__ __device__ constexpr int PX(int i) { return 8 * ((i >> 1) & 1) + 2 * (i >> 2) + (i & 1); }
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
@@ -280,7 +156,7 @@ __device__ __forceinline__ float col8(const float4& lo, const float4& hi, int i)
   return (c & 2) ? ((c & 1) ? b.w : b.z) : ((c & 1) ? b.y : b.x);
 }
 __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
-// Lean-path operand store.  Value (row m, feature t = 2 g + e of my eight) is accumulator column 32 fc + 8 g + 2 (lane % 4) + e of
+// Operand store of one step.  Value (row m, feature t = 2 g + e of my eight) is accumulator column 32 fc + 8 g + 2 (lane % 4) + e of
 // the 64-column chunk: half2 (e = 0, 1) at byte 4 (lane % 4) of 16-byte chunk 4 fc + g, swizzled with the operand row's low bits
 // (= lane / 4).  `sa` = shared address of (my first row, g = 0) inside the slot: g flips bits 4-5, my second row is 8 operand
 // rows (1 KB) further.  ROWORDER: v is in row order (stage 0) instead of fragment order (epilogues).
@@ -321,9 +197,45 @@ __device__ __forceinline__ float srcbound(const RowSrc& s) {
   return s.bound_mul_i ? m * (float)max(__ldg(s.bound_mul_i), 1) : m;
 }
 
+// ---- the product ------------------------------------------------------------------------------------------------------
+// D (+)= A[:, 64 kc0 .. 64 kc1) . W^T over my warpgroup's 64 rows (a_rows): per 64-column chunk one weight panel (bf16) or two
+// (fp16 hi, lo), four k16 steps each; A_hi.B_hi + A_lo.B_hi on the hi panel, A_hi.B_lo on the lo panel.  Everything here is
+// warpgroup-uniform straight-line code (the waits loop inside their asm statements), so ptxas keeps the wgmma asynchronous.  A
+// panel's stage is released by every consumer thread once the wgmma that read it have completed; the next panel is already
+// resident (two stages), so the tensor pipe only idles for the issue latency between panels.
+template <bool SPLIT, int N>
+__device__ __forceinline__ void mma_chunks(float (&d)[128], uint32_t a_rows, uint32_t b_base, uint32_t bar_full_b, uint32_t bar_empty_b,
+                                           uint32_t& bi, int kc0, int kc1) {
+  for (int kc = kc0; kc < kc1; ++kc) {
+    const uint32_t a_hi = a_rows + (uint32_t)(kc % A_SLOTS) * A_SLOT_BYTES, a_lo = a_hi + A_HALF_BYTES;
+#pragma unroll
+    for (int part = 0; part < (SPLIT ? 2 : 1); ++part) {
+      const uint32_t stage = bi % B_STAGES, nb = bi / B_STAGES;
+      mbar_wait_or_trap(bar_full_b + 8 * stage, nb & 1);
+      const uint32_t b = b_base + stage * B_STAGE_BYTES;
+      wgmma_fence();
+      if (part == 0) {
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) Wgmma<N, !SPLIT>::mma(d, gmma_desc(a_hi + 32 * ks), gmma_desc(b + 32 * ks), (kc | ks) != 0);
+        if (SPLIT) {
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) Wgmma<N, !SPLIT>::mma(d, gmma_desc(a_lo + 32 * ks), gmma_desc(b + 32 * ks), 1);
+        }
+      } else {
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) Wgmma<N, !SPLIT>::mma(d, gmma_desc(a_hi + 32 * ks), gmma_desc(b + 32 * ks), 1);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      mbar_arrive(bar_empty_b + 8 * stage);
+      ++bi;
+    }
+  }
+  fence_operand(d);
+}
+
 // MODE 0: every part takes the general path; 1: every part takes the lean full-width path; 2: as 1, plus the forecast's narrow
-// output layer (layer_out_narrow) as the chain's last layer.  (A third mode that chose per
-// part inside one kernel was measured slower than the general path: the live state of both paths spills.)
+// output layer (layer_out_narrow) as the chain's last layer.
 template <bool SPLIT, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __grid_constant__ TcChain ch) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -332,30 +244,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
   const int rows = ch.rows_per_sample, batch = ch.batch;
   const int tiles_per_sample = (rows + TILE_M - 1) / TILE_M;
   const int num_tiles = tiles_per_sample * batch;  // batch-major: tile -> (sample = tile % batch, row block = tile / batch)
-  constexpr bool split = SPLIT;
   constexpr int parts = SPLIT ? 2 : 1;
 
-  const uint32_t bar_full_a = sbase + OFF_BAR;             // [A_SLOTS] workers -> MMA (one arrival per worker warp)
-  const uint32_t bar_empty_a = bar_full_a + 8 * A_SLOTS;   // [A_SLOTS] MMA -> workers (tcgen05.commit); waited only when stage 0 wraps the ring
-  const uint32_t bar_full_b = bar_empty_a + 8 * A_SLOTS;   // [B_STAGES] bulk copy -> MMA
-  const uint32_t bar_empty_b = bar_full_b + 8 * B_STAGES;  // [B_STAGES] MMA -> producer
-  const uint32_t bar_full_d = bar_empty_b + 8 * B_STAGES;  // [2] MMA -> workers: accumulator complete
-  const uint32_t bar_empty_d = bar_full_d + 16;            // [2] workers -> MMA: accumulator drained
-  volatile uint32_t* tmem_ptr = reinterpret_cast<volatile uint32_t*>(smem + OFF_TMEM);
+  const uint32_t bar_full_b = sbase + OFF_BAR;             // [B_STAGES] bulk copy -> consumers
+  const uint32_t bar_empty_b = bar_full_b + 8 * B_STAGES;  // [B_STAGES] consumers (every thread arrives) -> producer
 
   if (threadIdx.x == 0) {
     if (sbase & 1023u) {  // SWIZZLE_128B operand tiles must be 1 KB aligned
       if (ch.status) atomicOr(ch.status, 4);
       __trap();
     }
-    for (int i = 0; i < A_SLOTS; ++i) mbar_init(bar_full_a + 8 * i, WORKER_WARPS), mbar_init(bar_empty_a + 8 * i, 1);
-    for (int i = 0; i < B_STAGES; ++i) mbar_init(bar_full_b + 8 * i, 1), mbar_init(bar_empty_b + 8 * i, 1);
-    for (int i = 0; i < 2; ++i) mbar_init(bar_full_d + 8 * i, 1), mbar_init(bar_empty_d + 8 * i, WORKER_WARPS);
+    for (int i = 0; i < B_STAGES; ++i) mbar_init(bar_full_b + 8 * i, 1), mbar_init(bar_empty_b + 8 * i, NUM_WORKERS);
     fence_barrier_init();
-  }
-  if (warp == WARP_MMA) {  // TMEM: all 512 columns (two fp32 accumulators of 256 columns)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sbase + OFF_TMEM), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   {  // per-layer column parameters -> shared memory (zero beyond n_valid)
     float* par = reinterpret_cast<float*>(smem + OFF_PAR);
@@ -405,17 +305,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
     }
     if (bad && ch.status) atomicOr(ch.status, 8);  // a magnitude bound overflowed fp32: inputs are not finite numbers of usable size
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  // Register reallocation (inside each role's branch, so that ptxas budgets the roles separately): the auxiliary warpgroup
-  // keeps 32 registers per thread, the workers (which hold a 64-value LayerNorm fragment per thread) grow to 120.
-  if (warp >= WORKER_WARPS) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(AUX_REGS));
-  if (warp == WARP_PRODUCER) {
-    // ===================================== weight producer =========================================================
-    if (lane == 0) {
+  // Register reallocation (inside each role's branch, so that ptxas budgets the roles separately)
+  if (warp >= CONSUMER_WARPS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(AUX_REGS));
+    if (warp == WARP_PRODUCER && lane == 0) {
+      // ===================================== weight producer =========================================================
       uint32_t bi = 0;
       Tracer tr;
       tr.init(ch.trace, 0, true);
@@ -441,978 +336,628 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
         }
       }
     }
-  } else if (warp == WARP_MMA) {
-    // ===================================== MMA issuer ==============================================================
-    if (lane == 0) {
-      uint32_t bi = 0, fi = 0, li = 0;
-      Tracer tr;
-      tr.init(ch.trace, 1, true);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        uint32_t prev_first = fi;
-        tr.ev(1000);
-        for (int l = 0; l < ch.n_layers; ++l, ++li) {
-          const TcLayer& L = ch.layer[l];
-          const int nk = L.K >> 6;
-          const uint32_t idesc = umma_idesc(L.N, !split);
-          const uint32_t acc = li & 1, use = li >> 1;
-          tr.ev(100 + l);
-          mbar_wait(bar_empty_d + 8 * acc, (use & 1) ^ 1, ch.status);  // epilogue of layer li-2 has drained this accumulator
-          tc_fence_after();
-          tr.ev(110 + l);
-          const uint32_t d_tmem = tmem_base + acc * 256;
-          const uint32_t first = L.reuse_a ? prev_first : fi;
-          const bool last_use = !(l + 1 < ch.n_layers && ch.layer[l + 1].reuse_a);
-          for (int kc = 0; kc < nk; ++kc) {
-            const uint32_t f = first + kc, slot = f % A_SLOTS, n = f / A_SLOTS;
-            mbar_wait(bar_full_a + 8 * slot, n & 1, ch.status);  // (already complete when the operand is re-used)
-            tc_fence_after();
-            tr.ev(200 + kc);
-            const uint32_t a_hi = sbase + OFF_A + slot * A_SLOT_BYTES, a_lo = a_hi + A_HALF_BYTES;
-            {  // hi weight panel: A_hi.B_hi (+ A_lo.B_hi)
-              const uint32_t stage = bi % B_STAGES, nb = bi / B_STAGES;
-              mbar_wait(bar_full_b + 8 * stage, nb & 1, ch.status);
-              tc_fence_after();
-              tr.ev(210 + kc);
-              const uint32_t b = sbase + OFF_B + stage * B_STAGE_BYTES;
-              if (!ABL3(ABL_MMA)) {
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) tc_mma_f16(d_tmem, umma_desc(a_hi + 32 * ks), umma_desc(b + 32 * ks), idesc, (kc | ks) != 0);
-                if (split) {
-#pragma unroll
-                  for (int ks = 0; ks < 4; ++ks) tc_mma_f16(d_tmem, umma_desc(a_lo + 32 * ks), umma_desc(b + 32 * ks), idesc, 1);
-                }
-              }
-              tc_commit(bar_empty_b + 8 * stage);
-              ++bi;
-            }
-            if (split) {  // lo weight panel: A_hi.B_lo
-              const uint32_t stage = bi % B_STAGES, nb = bi / B_STAGES;
-              tr.ev(215 + kc);
-              mbar_wait(bar_full_b + 8 * stage, nb & 1, ch.status);
-              tc_fence_after();
-              tr.ev(220 + kc);
-              const uint32_t b = sbase + OFF_B + stage * B_STAGE_BYTES;
-              if (!ABL3(ABL_MMA)) {
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) tc_mma_f16(d_tmem, umma_desc(a_hi + 32 * ks), umma_desc(b + 32 * ks), idesc, 1);
-              }
-              tc_commit(bar_empty_b + 8 * stage);
-              ++bi;
-            }
-            if (last_use) tc_commit(bar_empty_a + 8 * slot);  // one phase per use of the slot
-            tr.ev(300 + kc);
-          }
-          tc_commit(bar_full_d + 8 * acc);  // accumulator complete -> epilogue
-          if (!L.reuse_a) {
-            prev_first = fi;
-            fi += nk;
-          }
-        }
-      }
-    }
+    return;
   }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WORKER_REGS));
-    // ===================================== workers =================================================================
-    const int q = warp & 3;    // TMEM lane quadrant (a warp may only touch lanes 32 (warp % 4) ..+31)
-    const int hq = warp >> 2;  // which 16 columns of every 64-column chunk
-    const int lr = lane >> 2, lc = lane & 3;
-    int rt[4];  // my four TMEM lanes (= rows of the shared-memory operand)
-    int re[4];  // the LOGICAL tile rows they hold: four consecutive rows per thread, 32 consecutive rows per 8 lane groups
-#pragma unroll
-    for (int k = 0; k < 4; ++k) rt[k] = 32 * q + 16 * (k >> 1) + lr + 8 * (k & 1), re[k] = 32 * q + 4 * lr + k;
-    const int cofs = 16 * hq + 4 * lc;  // my first (logical) column inside a 64-column chunk; the operand position uses 2 * lc
-    const float* scl = reinterpret_cast<const float*>(smem + OFF_SCL);
-    const float a0scale = scl[2 * PAR_LAYERS];
-    // Row statistics of a LayerNorm are exchanged between the four warps of a lane quadrant through ln_x / ln_y with ONE named
-    // barrier: consecutive LayerNorms alternate between two generations of the buffers, so a warp that runs ahead into LayerNorm
-    // i+1 writes the other generation, and it cannot reach LayerNorm i+2 (the same generation again) before every warp of the
-    // quadrant has passed the barrier of i+1, i.e. has finished reading generation i.
-    float* const ln_base = reinterpret_cast<float*>(smem + OFF_LN);
-    uint32_t ln_gen = 0;
-    uint32_t fi = 0, li = 0;
-    float amax = 0.f;
-    Tracer tr;
-    tr.init(ch.trace, 5 + (hq & 1), q == 0 && lane == 0 && hq < 2);
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(WORKER_REGS));
+  // ===================================== consumers ===================================================================
+  // Warp q of warpgroup wg covers the 16 tile rows frow .. frow + 15.  A thread holds TWO CONSECUTIVE logical rows fr0, fr0 + 1
+  // (operand / accumulator rows frow + lane/4 and + 8) times, in every 32-column step u, EIGHT CONSECUTIVE features
+  // 32 u + fcofs .. + 7.  The 8 rows of a warp instruction are operand rows frow + 0..7 (+8): their low three bits differ, so
+  // the swizzled operand stores are conflict-free.
+  const int wg = warp >> 2, q = warp & 3;
+  const int lr = lane >> 2, lc = lane & 3;
+  const int frow = 64 * wg + 16 * q;
+  const int fr0 = frow + 2 * lr;
+  const int fcofs = 8 * lc;
+  const uint32_t a_rows = sbase + OFF_A + 64 * wg * 128;                         // my warpgroup's operand rows
+  const uint32_t fsa = sbase + OFF_A + (frow + lr) * 128 + 4 * lc + (lr << 4);  // store_operand_x4 of step 0 (step u: ^ (u & 1) << 6)
+  const uint32_t wbar = 1 + wg;
+  const float* scl = reinterpret_cast<const float*>(smem + OFF_SCL);
+  const float a0scale = scl[2 * PAR_LAYERS];
+  uint32_t bi = 0;
+  float amax = 0.f;
+  Tracer tr;
+  tr.init(ch.trace, 5 + wg, q == 0 && lane == 0);
 
-    // publish one finished operand chunk: my writes -> async proxy, then one arrival per warp
-    auto publish = [&](uint32_t slot) {
-      if (!ABL3(ABL_FENCE)) fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_full_a + 8 * slot);
+  auto wg_sync = [&]() GW_INLINE { asm volatile("bar.sync %0, 128;" ::"r"(wbar) : "memory"); };
+  // operand rows written by my warpgroup -> visible to its wgmma (async proxy)
+  auto publish = [&]() GW_INLINE {
+    if (!ABL3(ABL_FENCE)) fence_proxy_async();
+    wg_sync();
+  };
+  auto op_addr = [&](int u) GW_INLINE { return (fsa ^ ((uint32_t)(u & 1) << 6)) + (uint32_t)((u >> 1) % A_SLOTS) * A_SLOT_BYTES; };
+  // ---- stage 0, general path: steps [8 w, 8 w + 8) of the operand (window w of four 64-column slots) ----------------------
+  auto stage0 = [&](int tile, int w) GW_INLINE {
+    const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
+    const int nvalid = min(TILE_M, rows - i0);
+    const int r2[2] = {min(fr0, nvalid - 1), min(fr0 + 1, nvalid - 1)};
+    const int nu = min(2 * (ch.K0 >> 6), 8 * w + 8), w0 = ch.a0[0].width;
+    for (int u = 8 * w; u < nu; ++u) {
+      const int colc = 32 * u;
+      const int which = colc < w0 ? 0 : 1;
+      const RowSrc& src = ch.a0[which];
+      const int rel = which ? colc - w0 : colc;
+      float cur[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) cur[i] = 0.f;
+      if (src.kind != SRC_NONE && rel < src.width && !ABL3(ABL_LOADS)) {
+#pragma unroll
+        for (int m = 0; m < 2; ++m) {
+          load8(src_row(src, bs, i0, r2[m]), rel + fcofs, src.width, cur + 8 * m);
+          if (src.kind == SRC_GATHER_BCAST_RELU) {
+            float t[8];
+            load8(src.base2 + (size_t)(uint32_t)(i0 + r2[m]) * (size_t)src.ld2, rel + fcofs, src.width, t);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) cur[8 * m + k] = fmaxf(cur[8 * m + k] + t[k], 0.f);
+          }
+        }
+      }
+      if (a0scale != 1.f) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) cur[i] *= a0scale;
+      }
+      if (!ABL3(ABL_CONVERT)) store_operand_x4<SPLIT, true>(op_addr(u), cur, amax);
+    }
+    publish();
+  };
+
+  // ---- stage 0, lean path: NC0 + NC1 64-column chunks from one or two aligned sources, window W (chunks 4 W .. 4 W + 3) ------
+  // The rows stream from HBM (edge state) or L2 (node state): up to four steps (16 x LDG.128 per thread) are in flight before the
+  // first one is converted.  GBR: the operand is relu(gathered row + broadcast row); the two tables are kept apart until the step
+  // is converted (two steps in flight).
+  auto stage0_fast = [&](auto NC0c, auto NC1c, auto GBRc, auto Wc, int tile) GW_INLINE {
+    constexpr int NC0 = decltype(NC0c)::value, NC1 = decltype(NC1c)::value, NC = NC0 + NC1;
+    constexpr bool GBR = decltype(GBRc)::value != 0;
+    constexpr int U0 = 8 * decltype(Wc)::value, U1 = (2 * NC < U0 + 8) ? 2 * NC : U0 + 8;
+    constexpr int DEPTH = GBR ? 2 : 4;
+    const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
+    const int nvalid = min(TILE_M, rows - i0);
+    const int r2[2] = {min(fr0, nvalid - 1), min(fr0 + 1, nvalid - 1)};
+    const char* pa[2];
+    const char* pb[2] = {nullptr, nullptr};  // second source, or the broadcast table of GBR
+    row_ptrs2(ch.a0[0], bs, i0, r2, fcofs, pa);
+    if constexpr (GBR) {
+#pragma unroll
+      for (int m = 0; m < 2; ++m) pb[m] = reinterpret_cast<const char*>(ch.a0[0].base2 + (size_t)(uint32_t)(i0 + r2[m]) * (size_t)ch.a0[0].ld2 + fcofs);
+    } else if constexpr (NC1 > 0) {
+      row_ptrs2(ch.a0[1], bs, i0, r2, fcofs, pb);
+    }
+    float buf[DEPTH][16] = {};  // [row m][8 features]
+    float bufb[GBR ? DEPTH : 1][16] = {};
+    auto fetch = [&](auto uu) GW_INLINE {
+      constexpr int u = decltype(uu)::value, k = (u - U0) % DEPTH;
+      if (ABL3(ABL_LOADS)) return;
+      if constexpr (GBR) {
+        ld256(pa[0] + 128 * u, buf[k]), ld256(pa[1] + 128 * u, buf[k] + 8);
+        ld256(pb[0] + 128 * u, bufb[k]), ld256(pb[1] + 128 * u, bufb[k] + 8);
+      } else if constexpr (u < 2 * NC0) {
+        ld256(pa[0] + 128 * u, buf[k]), ld256(pa[1] + 128 * u, buf[k] + 8);
+      } else {
+        ld256(pb[0] + 128 * (u - 2 * NC0), buf[k]), ld256(pb[1] + 128 * (u - 2 * NC0), buf[k] + 8);
+      }
     };
-
-    // ---- stage 0: assemble the fp16 hi/lo operand of the first layer straight from global memory -----------------------
-    auto stage0 = [&](int tile) {
-      const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
-      const int nvalid = min(TILE_M, rows - i0);
-      int rl[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) rl[k] = min(re[k], nvalid - 1);
-      const int nk0 = ch.K0 >> 6, w0 = ch.a0[0].width;
-      int ri[4] = {0, 0, 0, 0}, ri2[4] = {0, 0, 0, 0};  // rows of the current source (and of its broadcast partner)
-      int cur_src = -1;
-      auto fetch = [&](int c, float (&o)[16]) {
-        const int colc = 64 * c;
-        const int which = colc < w0 ? 0 : 1;
-        const RowSrc& src = ch.a0[which];
-        const int rel = which ? colc - w0 : colc;
-        if (src.kind == SRC_NONE || rel >= src.width || ABL3(ABL_LOADS)) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) o[i] = 0.f;
-          return;
-        }
-        if (which != cur_src) {
-          rows_of(src, i0, rl, ri);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) ri2[k] = i0 + rl[k];
-          cur_src = which;
-        }
-        load16(src, bs, ri, rel + cofs, lc, o);
-        if (src.kind == SRC_GATHER_BCAST_RELU) {
-          float t[16];
-          load16(src.base2, src.ld2, src.width, ri2, rel + cofs, lc, t);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) o[i] = fmaxf(o[i] + t[i], 0.f);
-        }
-      };
-      float cur[16], nxt[16];
-      fetch(0, cur);
-      for (int c = 0; c < nk0; ++c) {
-        if (c + 1 < nk0) fetch(c + 1, nxt);
-        const uint32_t f = fi + c, slot = f % A_SLOTS, n = f / A_SLOTS;
-        if (n > 0) mbar_wait(bar_empty_a + 8 * slot, (n - 1) & 1, ch.status);  // the MMAs that read this slot last have completed
-        if (a0scale != 1.f) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) cur[i] *= a0scale;
-        }
-        if (!ABL3(ABL_CONVERT)) store_operand16(smem + OFF_A + slot * A_SLOT_BYTES, rt, hq, lc, cur, split, amax);
-        publish(slot);
-        tr.ev(500 + c);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) cur[i] = nxt[i];
-      }
-      fi += nk0;
-    };
-
-    // =================================== lean path (MODE 1) ================================================================
-    // One thread mapping serves stage 0 and every epilogue.  Warp (q, fh, fc) = (warp & 3, (warp >> 2) & 1, warp >> 3) covers the
-    // 16 tile rows frow = 32 q + 16 fh .. +15 and the 32 columns 32 fc .. +31 of every 64-column chunk.  A thread holds TWO
-    // CONSECUTIVE rows (logical rows fr0, fr0 + 1 <-> TMEM lanes / operand rows frow + lane/4 and + 8) times EIGHT CONSECUTIVE
-    // features fcofs .. fcofs + 7: one tcgen05.ld.16x256b.x4 under the perm32 feature order (gw_pack.cu).  Four adjacent lanes
-    // thus cover one full 128-byte line of a row, and a warp-level 256-bit access touches 8 full lines.  The L1 pipeline spends
-    // ~2 cycles per (instruction x line touched) (tools/micro/ldg_wavefront.cu: 35 B/cycle/SM with the x2 fragment's 8 rows x 64 B
-    // per LDG.128, 58 B/cycle/SM with full lines), and the rows gathered through the sorted target index coalesce further (the
-    // 8 rows of one instruction are 16 consecutive edges: ~3 distinct targets).  The 8 rows of an instruction are operand rows
-    // frow + 0..7 (+8): their low three bits differ, so the swizzled operand stores are conflict-free.
-    const int fh = hq & 1, fc = hq >> 1;
-    const int frow = 32 * q + 16 * fh;
-    const int fr0 = frow + 2 * lr;
-    const int fcofs = 32 * fc + 8 * lc;  // my first (logical) column inside a 64-column chunk
-    const uint32_t fsa = sbase + OFF_A + (frow + lr) * 128 + 4 * lc + (((4 * fc) ^ lr) << 4);  // store_operand_x4
-    const uint32_t ftm = ((uint32_t)frow << 16) + 32 * fc;                                        // my TMEM lanes / columns
-    const int fbar = 1 + 2 * q + fh;  // named barrier of the two warps (fc = 0, 1) that share my rows
-
-    // gather rows of layer 0's addends for the tile whose stage 0 ran last (resolved there, so that the index loads do
-    // not sit between two tiles); kept in shared memory, one word per thread and row: registers are the scarce resource
-    uint32_t* pre_s = reinterpret_cast<uint32_t*>(smem + OFF_PRE) + threadIdx.x;  // [4][NUM_WORKERS], one column per thread
-    const bool l0_add0 = ch.layer[0].add[0].kind != SRC_NONE, l0_add1 = ch.layer[0].add[1].kind != SRC_NONE;
-    const bool l0_g0 = src_gathered(ch.layer[0].add[0].kind), l0_g1 = src_gathered(ch.layer[0].add[1].kind);
-
-    // ---- stage 0, lean path: NC0 + NC1 64-column chunks from one or two aligned sources, fully unrolled ------------------------
-    // The rows stream from HBM (edge state) or L2 (node state): up to four chunks (8 x LDG.256 per thread) are in flight before
-    // the first one is converted, so a tile pays the memory latency once, not once per chunk.  GBR: the operand is
-    // relu(gathered row + broadcast row); the two tables are kept apart until the chunk is converted (two chunks in flight).
-    auto stage0_fast = [&](auto NC0c, auto NC1c, auto GBRc, int tile) {
-      constexpr int NC0 = decltype(NC0c)::value, NC1 = decltype(NC1c)::value, NC = NC0 + NC1;
-      constexpr bool GBR = decltype(GBRc)::value != 0;
-      constexpr int DEPTH = GBR ? 2 : 4;
-      const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
-      const int nvalid = min(TILE_M, rows - i0);
-      const int r2[2] = {min(fr0, nvalid - 1), min(fr0 + 1, nvalid - 1)};
-      // gather rows of layer 0's addends: requested first, parked in shared memory once the operand loads are under way
-      uint32_t g0[2] = {0u, 0u}, g1[2] = {0u, 0u};
-      if (l0_add0) {
-#pragma unroll
-        for (int m = 0; m < 2; ++m) g0[m] = l0_g0 ? (uint32_t)__ldg(ch.layer[0].add[0].idx + i0 + r2[m]) : (uint32_t)(i0 + r2[m]);
-      }
-      if (l0_add1) {
-#pragma unroll
-        for (int m = 0; m < 2; ++m) g1[m] = l0_g1 ? (uint32_t)__ldg(ch.layer[0].add[1].idx + i0 + r2[m]) : (uint32_t)(i0 + r2[m]);
-      }
-      const char* pa[2];
-      const char* pb[2] = {nullptr, nullptr};  // second source, or the broadcast table of GBR
-      row_ptrs2(ch.a0[0], bs, i0, r2, fcofs, pa);
+    static_for<U0, (U1 < U0 + DEPTH ? U1 : U0 + DEPTH)>([&](auto uu) GW_INLINE { fetch(uu); });
+    static_for<U0, U1>([&](auto uu) GW_INLINE {
+      constexpr int u = decltype(uu)::value, k = (u - U0) % DEPTH;
+      float(&cur)[16] = buf[k];
       if constexpr (GBR) {
 #pragma unroll
-        for (int m = 0; m < 2; ++m) pb[m] = reinterpret_cast<const char*>(ch.a0[0].base2 + (size_t)(uint32_t)(i0 + r2[m]) * (size_t)ch.a0[0].ld2 + fcofs);
-      } else if constexpr (NC1 > 0) {
-        row_ptrs2(ch.a0[1], bs, i0, r2, fcofs, pb);
+        for (int i = 0; i < 16; ++i) cur[i] = fmaxf(cur[i] + bufb[k][i], 0.f);
       }
-      float buf[DEPTH][16] = {};  // [row m][8 features]
-      float bufb[GBR ? DEPTH : 1][16] = {};
-      auto fetch = [&](auto cc) {
-        constexpr int c = decltype(cc)::value;
-        if (ABL3(ABL_LOADS)) return;
-        if constexpr (GBR) {
-          ld256(pa[0] + 256 * c, buf[c % DEPTH]), ld256(pa[1] + 256 * c, buf[c % DEPTH] + 8);
-          ld256(pb[0] + 256 * c, bufb[c % DEPTH]), ld256(pb[1] + 256 * c, bufb[c % DEPTH] + 8);
-        } else if constexpr (c < NC0) {
-          ld256(pa[0] + 256 * c, buf[c % DEPTH]), ld256(pa[1] + 256 * c, buf[c % DEPTH] + 8);
-        } else {
-          ld256(pb[0] + 256 * (c - NC0), buf[c % DEPTH]), ld256(pb[1] + 256 * (c - NC0), buf[c % DEPTH] + 8);
-        }
-      };
-      tr.ev(480);
-      static_for<0, (NC < DEPTH ? NC : DEPTH)>([&](auto cc) { fetch(cc); });
-      if (l0_add0) pre_s[0] = g0[0], pre_s[NUM_WORKERS] = g0[1];
-      if (l0_add1) pre_s[2 * NUM_WORKERS] = g1[0], pre_s[3 * NUM_WORKERS] = g1[1];
-      static_for<0, NC>([&](auto cc) {
-        constexpr int c = decltype(cc)::value;
-        const uint32_t f = fi + c, slot = f % A_SLOTS, n = f / A_SLOTS;
-        if (n > 0) mbar_wait(bar_empty_a + 8 * slot, (n - 1) & 1, ch.status);  // the MMAs that read this slot last have completed
-        tr.ev(490 + c);
-        float(&cur)[16] = buf[c % DEPTH];
-        if constexpr (GBR) {
+      if (a0scale != 1.f) {
 #pragma unroll
-          for (int i = 0; i < 16; ++i) cur[i] = fmaxf(cur[i] + bufb[c % DEPTH][i], 0.f);
-        }
-        if (a0scale != 1.f) {  // (two copies of the conversion: see layer_fast)
-#pragma unroll
-          for (int i = 0; i < 16; ++i) cur[i] *= a0scale;
-          if (!ABL3(ABL_CONVERT)) store_operand_x4<SPLIT, true>(fsa + slot * A_SLOT_BYTES, cur, amax);
-        } else {
-          if (!ABL3(ABL_CONVERT)) store_operand_x4<SPLIT, true>(fsa + slot * A_SLOT_BYTES, cur, amax);
-        }
-        publish(slot);
-        if constexpr (c + DEPTH < NC) fetch(ic<c + DEPTH>{});  // refill the buffer just consumed
-        tr.ev(500 + c);
-      });
-      fi += NC;
-    };
+        for (int i = 0; i < 16; ++i) cur[i] *= a0scale;
+      }
+      if (!ABL3(ABL_CONVERT)) store_operand_x4<SPLIT, true>(op_addr(u), cur, amax);
+      if constexpr (u + DEPTH < U1) fetch(ic<u + DEPTH>{});  // refill the buffer just consumed
+    });
+    publish();
+  };
 
-    // ---- one layer's epilogue, lean path: N = 64 NP, full-width aligned addends / residual / output ---------------------------
-    // Register budget: two accumulator fragments (the chunk in work and the next one in flight from TMEM), the prefetched
-    // addend / residual rows of the next chunk, and 4 registers of row pointers per global source.  Accumulator fragments are in
-    // fragment order (index 4 g + 2 m + e = row m, feature 2 g + e), everything read from / written to global memory in row order
-    // (index 8 m + t); FR() / PX() translate at compile time.
-    auto layer_fast = [&](auto FLc, auto NPc, int l, uint32_t acc, uint32_t use, bool waited, int tile, int ln_slot) {
-      constexpr int F = decltype(FLc)::value, NP = decltype(NPc)::value;
-      constexpr bool has_add0 = (F & F_ADD0) != 0, has_add1 = (F & F_ADD1) != 0, has_res = (F & F_RES) != 0, has_out = (F & F_OUT) != 0;
-      constexpr bool relu = (F & F_RELU) != 0, has_ln = (F & F_LN) != 0, feeds = (F & F_FEEDS) != 0, has_seg = (F & F_SEG) != 0;
-      constexpr bool has0 = has_add0 || has_res;
-      const TcLayer& L = ch.layer[l];
-      const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
-      const int nvalid = min(TILE_M, rows - i0);
-      const float wsi = scl[2 * l], osc = scl[2 * l + 1];
-      const uint32_t bias_a = sbase + OFF_PAR + 4 * fcofs + l * 1024;
-      const uint32_t g_a = sbase + OFF_LNP + 4 * fcofs + (ln_slot * 2) * 1024, b_a = g_a + 1024;
-      const uint32_t taddr = tmem_base + ftm + acc * 256;
-      const RowSrc& src0 = has_add0 ? L.add[0] : L.residual;
-      const char* p0[2] = {nullptr, nullptr};  // addend 0 or residual rows
-      const char* p1[2] = {nullptr, nullptr};  // addend 1 rows
-      float pf0[16] = {}, pf1[16] = {};
-      {
-        const int r2[2] = {min(fr0, nvalid - 1), min(fr0 + 1, nvalid - 1)};
-        if constexpr (has0) {
-          if (l == 0 && has_add0) {  // rows resolved during this tile's stage 0
-            const char* base = src_sample_base(src0, bs) + 4 * fcofs;
-            const size_t ldb = 4 * (size_t)src0.ld;
-            p0[0] = base + (size_t)pre_s[0] * ldb, p0[1] = base + (size_t)pre_s[NUM_WORKERS] * ldb;
-          } else {
-            row_ptrs2(src0, bs, i0, r2, fcofs, p0);
-          }
-        }
-        if constexpr (has_add1) {
-          if (l == 0) {
-            const char* base = src_sample_base(L.add[1], bs) + 4 * fcofs;
-            const size_t ldb = 4 * (size_t)L.add[1].ld;
-            p1[0] = base + (size_t)pre_s[2 * NUM_WORKERS] * ldb, p1[1] = base + (size_t)pre_s[3 * NUM_WORKERS] * ldb;
-          } else {
-            row_ptrs2(L.add[1], bs, i0, r2, fcofs, p1);
-          }
+  // scale + bias of the accumulator in place, steps [0, nu)
+  auto bias_in_place = [&](float (&acc)[128], int l, int nu, float wsi) GW_INLINE {
+    const uint32_t bias_a = sbase + OFF_PAR + l * 1024 + 4 * fcofs;
+    static_for<0, 8>([&](auto uu) GW_INLINE {
+      constexpr int u = decltype(uu)::value;
+      if (u < nu) {
+        const float4 bl = lds128(bias_a + 128 * u), bh = lds128(bias_a + 128 * u + 16);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) acc[16 * u + i] = fmaf(acc[16 * u + i], wsi, col8(bl, bh, i));
+      }
+    });
+  };
+  // LayerNorm statistics of my two rows over their nval real columns (two passes over the registers; the four lanes of a row
+  // combine with two shuffles): v -> v * rs[m] + sh[m]
+  auto ln_stats = [&](float (&acc)[128], int nu, int nval, float (&rs)[2], float (&sh)[2]) GW_INLINE {
+    float s[2] = {0.f, 0.f};
+    static_for<0, 8>([&](auto uu) GW_INLINE {
+      constexpr int u = decltype(uu)::value;
+      if (u < nu) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) s[(i >> 1) & 1] += acc[16 * u + i];  // (columns beyond nval are exactly zero)
+      }
+    });
+#pragma unroll
+    for (int m = 0; m < 2; ++m) s[m] += __shfl_xor_sync(0xffffffffu, s[m], 1), s[m] += __shfl_xor_sync(0xffffffffu, s[m], 2);
+    const float inv = 1.0f / (float)nval;
+    const float mean[2] = {s[0] * inv, s[1] * inv};
+    float v2[2] = {0.f, 0.f};
+    static_for<0, 8>([&](auto uu) GW_INLINE {
+      constexpr int u = decltype(uu)::value;
+      if (u < nu) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int m = (i >> 1) & 1;
+          const float d = (32 * u + fcofs + 2 * (i >> 2) + (i & 1) < nval) ? acc[16 * u + i] - mean[m] : 0.f;
+          v2[m] = fmaf(d, d, v2[m]);
         }
       }
-      const bool ld_on = !ABL3(ABL_LOADS);
-      auto ld2 = [&](const char* const(&p)[2], int off, float(&o)[16]) { ld256(p[0] + off, o), ld256(p[1] + off, o + 8); };
-      if constexpr (has0 && !has_ln) {
-        if (ld_on) ld2(p0, 0, pf0);  // (LayerNorm layers: after the statistics pass, which needs the registers)
+    });
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+      v2[m] += __shfl_xor_sync(0xffffffffu, v2[m], 1), v2[m] += __shfl_xor_sync(0xffffffffu, v2[m], 2);
+      const float rstd = 1.0f / sqrtf(v2[m] * inv + 1e-5f);
+      rs[m] = rstd, sh[m] = -mean[m] * rstd;
+    }
+  };
+
+  // ---- one layer's epilogue, lean path: N = 64 NP, full-width aligned addends / residual / output ---------------------------
+  // Accumulator fragments are in fragment order (index 4 g + 2 m + e = row m, feature 2 g + e), everything read from / written
+  // to global memory in row order (index 8 m + t); FR() / PX() translate at compile time.  The global operands of step u + 1 are
+  // in flight while step u is stored / converted.
+  auto layer_fast = [&](float (&acc)[128], auto FLc, auto NPc, int l, int tile, int ln_slot) GW_INLINE {
+    constexpr int F = decltype(FLc)::value, NP = decltype(NPc)::value, NU = 2 * NP;
+    constexpr bool has_add0 = (F & F_ADD0) != 0, has_add1 = (F & F_ADD1) != 0, has_res = (F & F_RES) != 0, has_out = (F & F_OUT) != 0;
+    constexpr bool relu = (F & F_RELU) != 0, has_ln = (F & F_LN) != 0, feeds = (F & F_FEEDS) != 0, has_seg = (F & F_SEG) != 0;
+    constexpr bool has0 = has_add0 || has_res;
+    const TcLayer& L = ch.layer[l];
+    const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
+    const int nvalid = min(TILE_M, rows - i0);
+    const float wsi = scl[2 * l], osc = scl[2 * l + 1];
+    const uint32_t g_a = sbase + OFF_LNP + 4 * fcofs + (ln_slot * 2) * 1024, b_a = g_a + 1024;
+    const RowSrc& src0 = has_add0 ? L.add[0] : L.residual;
+    const char* p0[2] = {nullptr, nullptr};  // addend 0 or residual rows
+    const char* p1[2] = {nullptr, nullptr};  // addend 1 rows
+    float pf0[16] = {}, pf1[16] = {};
+    const bool ld_on = !ABL3(ABL_LOADS);
+    auto ld2 = [&](const char* const(&p)[2], int off, float(&o)[16]) GW_INLINE { ld256(p[0] + off, o), ld256(p[1] + off, o + 8); };
+    {
+      const int r2[2] = {min(fr0, nvalid - 1), min(fr0 + 1, nvalid - 1)};
+      if constexpr (has0) row_ptrs2(src0, bs, i0, r2, fcofs, p0);
+      if constexpr (has_add1) row_ptrs2(L.add[1], bs, i0, r2, fcofs, p1);
+    }
+    if constexpr (has0) {
+      if (ld_on) ld2(p0, 0, pf0);
+    }
+    if constexpr (has_add1) {
+      if (ld_on) ld2(p1, 0, pf1);
+    }
+    // targets of my rows (fused per-target sums)
+    int d0 = 0, d1 = 0, dprev_g = 0;
+    if constexpr (has_seg) {
+      const int32_t* sd = L.seg_dst + i0;
+      d0 = (fr0 < nvalid) ? __ldg(sd + fr0) : -1;
+      d1 = (fr0 + 1 < nvalid) ? __ldg(sd + fr0 + 1) : -2;
+      dprev_g = (lr == 0 && i0 + frow > 0 && frow < nvalid) ? __ldg(sd + frow - 1) : -8;
+    }
+    bias_in_place(acc, l, NU, wsi);
+    float rs[2] = {1.f, 1.f}, sh[2] = {0.f, 0.f};  // LayerNorm as v * rs[m] + sh[m] per row
+    if constexpr (has_ln) {
+      if (!ABL3(ABL_LN)) ln_stats(acc, NU, 64 * NP, rs, sh);
+    }
+    // output rows (fp32): my two rows are ldo apart
+    char* po = nullptr;
+    const size_t ostr = 4 * (size_t)L.ldo;
+    const bool st0 = fr0 < nvalid, st1 = fr0 + 1 < nvalid;
+    if constexpr (has_out) po = reinterpret_cast<char*>(L.out + ((size_t)bs * rows + i0 + fr0) * (size_t)L.ldo + fcofs);
+    // Fused per-target sums.  Rows are sorted by target, a target's rows are a run of at most 8 consecutive rows.  The 8 lane
+    // groups of a warp hold 16 consecutive rows, two per thread.  The thread in which a run STARTS owns it: it adds to its own
+    // rows of the run the heads H (the rows before the first boundary) of the following threads the run reaches into, and
+    // stores the sum.  The heads are chained by doubling: G1(t) = H(t) + k(t) H(t+1) where k(t) = "the run passes through
+    // thread t into t+1"; the owner takes H(t+1) and G1(t+2) (two shuffles per value reach four threads = 7 rows; a third,
+    // G2(t+4), reaches the fifth thread an 8-row run can touch).  A run that reaches the next 16-row group continues there; that
+    // group's first thread leaves the continuation in the carry buffer (gw_seg_carry_kernel adds it to the run's row afterwards).
+    bool bb = false, tail_st = false, head_st = false, one_st = false, one_any = false, deep = false;
+    float mbf = 1.f, c1f = 0.f, e2f = 0.f, e4f = 0.f, kf = 0.f, k1f = 0.f;
+    char* tail_p = nullptr;
+    char* carry_p = nullptr;
+    const char* add_p = nullptr;
+    if constexpr (has_seg) {
+      int dprev = __shfl_up_sync(0xffffffffu, d1, 4);
+      if (lr == 0) dprev = dprev_g;
+      const bool ba = d0 != dprev;  // my first row starts a run
+      bb = d1 != d0;                // my second row starts a run
+      mbf = bb ? 0.f : 1.f;
+      const uint32_t nba = __shfl_down_sync(0xffffffffu, (uint32_t)ba, 4);
+      const bool c1 = lr < 7 && !nba;  // my last run continues into the next thread's rows
+      const bool k = c1 && !bb;        // ... and it entered my rows from the left or at my first row: it passes THROUGH me
+      const uint32_t k1 = __shfl_down_sync(0xffffffffu, (uint32_t)k, 4), k2 = __shfl_down_sync(0xffffffffu, (uint32_t)k, 8);
+      const uint32_t k3 = __shfl_down_sync(0xffffffffu, (uint32_t)k, 12);
+      const bool e2 = c1 && k1;         // (k(t+1) implies lane group t+2 exists)
+      const bool e4 = e2 && k2 && k3;
+      c1f = c1 ? 1.f : 0.f, e2f = e2 ? 1.f : 0.f, e4f = e4 ? 1.f : 0.f, kf = k ? 1.f : 0.f, k1f = (k && k1) ? 1.f : 0.f;
+      deep = L.seg_maxdeg > 7;  // (a run of 8 rows can reach the fifth thread; 7 rows end in the fourth)
+      carry_p = reinterpret_cast<char*>(L.seg_carry + ((((size_t)bs * tiles_per_sample + (size_t)(i0 / TILE_M)) * 8 + (size_t)(frow >> 4)) * 256 + fcofs));
+      // the run that ends with (or passes through) my second row: mine to store if it starts in my rows; the group's first
+      // thread stores the continuation of the previous group's run into the carry buffer
+      if (ba || bb) {
+        tail_st = d1 >= 0;
+        tail_p = reinterpret_cast<char*>(L.seg_out + ((size_t)bs * L.seg_rows + (size_t)(uint32_t)max(d1, 0)) * (size_t)L.seg_ld + fcofs);
+      } else if (lr == 0) {
+        tail_st = d1 >= 0;
+        tail_p = carry_p;
+      }
+      head_st = lr == 0 && !ba && bb && d0 >= 0;  // the previous group's run ends with my first row
+      one_st = ba && bb && d0 >= 0;               // my first row is a run of its own (a target with a single row)
+      one_any = __any_sync(0xffffffffu, one_st);
+      // per-target constant (a constant residual summed over the target's rows, once per weight set): the owner of a run adds it
+      if (L.seg_add && (ba || bb) && d1 >= 0)
+        add_p = reinterpret_cast<const char*>(L.seg_add + (size_t)(uint32_t)d1 * (size_t)L.seg_ld + fcofs);
+    }
+    static_for<0, NU>([&](auto uu) GW_INLINE {
+      constexpr int u = decltype(uu)::value;
+      float v[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) v[i] = acc[16 * u + i];
+      [[maybe_unused]] float sadd[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      if constexpr (has_seg) {
+        if (add_p) ld256(add_p + 128 * u, sadd);
+      }
+      if constexpr (has_add0) {
+        if (ld_on) {
+#pragma unroll
+          for (int i = 0; i < 16; ++i) v[i] += pf0[PX(i)];
+        }
       }
       if constexpr (has_add1) {
-        if (ld_on) ld2(p1, 0, pf1);
+        if (ld_on) {
+#pragma unroll
+          for (int i = 0; i < 16; ++i) v[i] += pf1[PX(i)];
+        }
       }
-      // targets of my rows (fused per-target sums): requested before the accumulator wait / the statistics pass
-      int d0 = 0, d1 = 0, dprev_g = 0;
-      if constexpr (has_seg) {
-        const int32_t* sd = L.seg_dst + i0;
-        d0 = (fr0 < nvalid) ? __ldg(sd + fr0) : -1;
-        d1 = (fr0 + 1 < nvalid) ? __ldg(sd + fr0 + 1) : -2;
-        dprev_g = (lr == 0 && i0 + frow > 0 && frow < nvalid) ? __ldg(sd + frow - 1) : -8;
+      if constexpr (relu) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
       }
-      if (!waited) {
-        tr.ev(600 + l);
-        mbar_wait(bar_full_d + 8 * acc, use & 1, ch.status);
-        tc_fence_after();
-        tr.ev(610 + l);
-      }
-      float rs[2] = {1.f, 1.f}, sh[2] = {0.f, 0.f};  // LayerNorm as v * rs[m] + sh[m] per row
       if constexpr (has_ln) {
-        if (!ABL3(ABL_LN)) {
-          // Statistics (first pass over the accumulator): each thread reduces its 8 NP values of each of its 2 rows around a
-          // pivot (the row's first value), the partial (mean, M2) pairs are merged with Chan's formula over the 4 lanes and
-          // the 2 warps that share a row: one pass, no cancellation, one barrier.
-          float pv[2] = {0.f, 0.f}, s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
-          float sv[2][16];  // chunk s+1 is fetched from TMEM while chunk s is accumulated
-          tmem_ld_16x256b_x4(taddr, sv[0]);
-          static_for<0, NP>([&](auto sc_) {
-            constexpr int s = decltype(sc_)::value;
-            float(&v)[16] = sv[s & 1];
-            tmem_wait_ld_into(v);
-            if constexpr (s + 1 < NP) tmem_ld_16x256b_x4(taddr + 64 * (s + 1), sv[(s + 1) & 1]);
-            const float4 bl = lds128(bias_a + 256 * s), bh = lds128(bias_a + 256 * s + 16);
+        const float4 gl = lds128(g_a + 128 * u), gh = lds128(g_a + 128 * u + 16);
+        const float4 el = lds128(b_a + 128 * u), eh = lds128(b_a + 128 * u + 16);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = fmaf(v[i], wsi, col8(bl, bh, i));
-            if constexpr (s == 0) pv[0] = v[0], pv[1] = v[2];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const int m = (i >> 1) & 1;
-              const float d = v[i] - pv[m];
-              s1[m] += d;
-              s2[m] = fmaf(d, d, s2[m]);
-            }
-          });
-          tr.ev(2001);
-          if constexpr (has0) {
-            if (ld_on) ld2(p0, 0, pf0);  // residual rows of chunk 0: in flight during the merge below
-          }
-          float mean[2], m2[2];
-          constexpr float inv_cnt = 1.0f / (8.0f * NP);
-#pragma unroll
-          for (int m = 0; m < 2; ++m) {
-            const float a = s1[m] * inv_cnt;
-            mean[m] = pv[m] + a;
-            m2[m] = fmaxf(s2[m] - s1[m] * a, 0.f);
-          }
-#pragma unroll
-          for (int o = 1; o <= 2; o <<= 1) {
-#pragma unroll
-            for (int m = 0; m < 2; ++m) {
-              const float mb = __shfl_xor_sync(0xffffffffu, mean[m], o), qb = __shfl_xor_sync(0xffffffffu, m2[m], o);
-              const float d = mb - mean[m];
-              mean[m] = 0.5f * (mean[m] + mb);
-              m2[m] = (m2[m] + qb) + d * d * (o == 1 ? 4.0f * NP : 8.0f * NP);
-            }
-          }
-          float* const ln_x = ln_base + (ln_gen & 1u) * (2 * WSPLIT * 128);
-          float* const ln_y = ln_x + WSPLIT * 128;
-          ++ln_gen;
-          if (lc == 0) {
-#pragma unroll
-            for (int m = 0; m < 2; ++m) ln_x[fc * 128 + frow + lr + 8 * m] = mean[m], ln_y[fc * 128 + frow + lr + 8 * m] = m2[m];
-          }
-          asm volatile("bar.sync %0, 64;" ::"r"(fbar) : "memory");  // the two warps that share these rows
-          tr.ev(2002);
-#pragma unroll
-          for (int m = 0; m < 2; ++m) {  // same order in both warps of the row
-            const float ma = ln_x[frow + lr + 8 * m], mb = ln_x[128 + frow + lr + 8 * m];
-            const float qa = ln_y[frow + lr + 8 * m], qb = ln_y[128 + frow + lr + 8 * m];
-            const float d = mb - ma;
-            const float mu = ma + 0.5f * d;
-            const float q2 = (qa + qb) + d * d * (16.0f * NP);
-            const float rstd = 1.0f / sqrtf(q2 * (1.0f / (64.0f * NP)) + 1e-5f);
-            rs[m] = rstd, sh[m] = -mu * rstd;
-          }
-          tr.ev(2003);
-        } else if constexpr (has0) {
-          if (ld_on) ld2(p0, 0, pf0);
+        for (int i = 0; i < 16; ++i) {
+          const int m = (i >> 1) & 1;
+          v[i] = fmaf(fmaf(v[i], rs[m], sh[m]), col8(gl, gh, i), col8(el, eh, i));
         }
       }
-      // output rows (fp32): my two rows are ldo apart
-      char* po = nullptr;
-      const size_t ostr = 4 * (size_t)L.ldo;
-      const bool st0 = fr0 < nvalid, st1 = fr0 + 1 < nvalid;
-      if constexpr (has_out) po = reinterpret_cast<char*>(L.out + ((size_t)bs * rows + i0 + fr0) * (size_t)L.ldo + fcofs);
-      // Fused per-target sums.  Rows are sorted by target, a target's rows are a run of at most 8 consecutive rows.  The 8 lane
-      // groups of a warp hold 16 consecutive rows, two per thread.  The thread in which a run STARTS owns it: it adds to its own
-      // rows of the run the heads H (the rows before the first boundary) of the following threads the run reaches into, and
-      // stores the sum.  The heads are chained by doubling: G1(t) = H(t) + k(t) H(t+1) where k(t) = "the run passes through
-      // thread t into t+1"; the owner takes H(t+1) and G1(t+2) (two shuffles per value reach four threads = 7 rows; a third,
-      // G2(t+4), reaches the fifth thread an 8-row run can touch).  A run that reaches the next 16-row group continues there; that
-      // group's first thread leaves the continuation in the carry buffer (gw_seg_carry_kernel adds it to the run's row afterwards).
-      bool bb = false, tail_st = false, head_st = false, one_st = false, one_any = false, deep = false;
-      float mbf = 1.f, c1f = 0.f, e2f = 0.f, e4f = 0.f, kf = 0.f, k1f = 0.f;
-      char* tail_p = nullptr;
-      char* carry_p = nullptr;
-      const char* add_p = nullptr;
-      if constexpr (has_seg) {
-        int dprev = __shfl_up_sync(0xffffffffu, d1, 4);
-        if (lr == 0) dprev = dprev_g;
-        const bool ba = d0 != dprev;  // my first row starts a run
-        bb = d1 != d0;                // my second row starts a run
-        mbf = bb ? 0.f : 1.f;
-        const uint32_t nba = __shfl_down_sync(0xffffffffu, (uint32_t)ba, 4);
-        const bool c1 = lr < 7 && !nba;  // my last run continues into the next thread's rows
-        const bool k = c1 && !bb;        // ... and it entered my rows from the left or at my first row: it passes THROUGH me
-        const uint32_t k1 = __shfl_down_sync(0xffffffffu, (uint32_t)k, 4), k2 = __shfl_down_sync(0xffffffffu, (uint32_t)k, 8);
-        const uint32_t k3 = __shfl_down_sync(0xffffffffu, (uint32_t)k, 12);
-        const bool e2 = c1 && k1;         // (k(t+1) implies lane group t+2 exists)
-        const bool e4 = e2 && k2 && k3;
-        c1f = c1 ? 1.f : 0.f, e2f = e2 ? 1.f : 0.f, e4f = e4 ? 1.f : 0.f, kf = k ? 1.f : 0.f, k1f = (k && k1) ? 1.f : 0.f;
-        deep = L.seg_maxdeg > 7;  // (a run of 8 rows can reach the fifth thread; 7 rows end in the fourth)
-        carry_p = reinterpret_cast<char*>(L.seg_carry + ((((size_t)bs * tiles_per_sample + (size_t)(i0 / TILE_M)) * 8 + (size_t)(2 * q + fh)) * 256 + fcofs));
-        // the run that ends with (or passes through) my second row: mine to store if it starts in my rows; the group's first
-        // thread stores the continuation of the previous group's run into the carry buffer
-        if (ba || bb) {
-          tail_st = d1 >= 0;
-          tail_p = reinterpret_cast<char*>(L.seg_out + ((size_t)bs * L.seg_rows + (size_t)(uint32_t)max(d1, 0)) * (size_t)L.seg_ld + fcofs);
-        } else if (lr == 0) {
-          tail_st = d1 >= 0;
-          tail_p = carry_p;
+      if constexpr (has_res) {
+        if (ld_on) {
+#pragma unroll
+          for (int i = 0; i < 16; ++i) v[i] += pf0[PX(i)];
         }
-        head_st = lr == 0 && !ba && bb && d0 >= 0;  // the previous group's run ends with my first row
-        one_st = ba && bb && d0 >= 0;               // my first row is a run of its own (a target with a single row)
-        one_any = __any_sync(0xffffffffu, one_st);
-        // per-target constant (a constant residual summed over the target's rows, once per weight set): the owner of a run adds it
-        if (L.seg_add && (ba || bb) && d1 >= 0)
-          add_p = reinterpret_cast<const char*>(L.seg_add + (size_t)(uint32_t)d1 * (size_t)L.seg_ld + fcofs);
       }
-      // The accumulator chunk s+1 is fetched from TMEM while chunk s is processed.
-      float vb[2][16] = {};
-      if constexpr (has_ln) tr.ev(2004);
-      if (!ABL3(ABL_TMEM)) tmem_ld_16x256b_x4(taddr, vb[0]);
-      static_for<0, NP>([&](auto sc_) {
-        constexpr int s = decltype(sc_)::value;
-        float(&v)[16] = vb[s & 1];
-        float sadd[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        if constexpr (has_seg) {
-          if (add_p) ld256(add_p + 256 * s, sadd);  // (requested a chunk's worth of arithmetic before it is needed)
-        }
-        tmem_wait_ld_into(v);
-        if constexpr (has_ln) tr.ev(2010 + s);
-        if constexpr (s + 1 < NP) {
-          if (!ABL3(ABL_TMEM)) tmem_ld_16x256b_x4(taddr + 64 * (s + 1), vb[(s + 1) & 1]);
-        } else {  // my last read of this accumulator
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_empty_d + 8 * acc);
-        }
-        {
-          const float4 bl = lds128(bias_a + 256 * s), bh = lds128(bias_a + 256 * s + 16);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = fmaf(v[i], wsi, col8(bl, bh, i));
-        }
-        if constexpr (has_add0) {
-          if (ld_on) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] += pf0[PX(i)];
-          }
+      if constexpr (u + 1 < NU) {  // next step's global operands: in flight while this step is stored / converted
+        if constexpr (has0) {
+          if (ld_on) ld2(p0, 128 * (u + 1), pf0);
         }
         if constexpr (has_add1) {
-          if (ld_on) {
+          if (ld_on) ld2(p1, 128 * (u + 1), pf1);
+        }
+      }
+      if constexpr (has_out) {
+        if (!ABL3(ABL_STORES)) {
+          if (st0) st256(po + 128 * u, v[FR(0, 0)], v[FR(0, 1)], v[FR(0, 2)], v[FR(0, 3)], v[FR(0, 4)], v[FR(0, 5)], v[FR(0, 6)], v[FR(0, 7)]);
+          if (st1) st256(po + ostr + 128 * u, v[FR(1, 0)], v[FR(1, 1)], v[FR(1, 2)], v[FR(1, 3)], v[FR(1, 4)], v[FR(1, 5)], v[FR(1, 6)], v[FR(1, 7)]);
+        }
+      }
+      if constexpr (has_seg) {
+        float T[8], H[8];
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] += pf1[PX(i)];
+        for (int t = 0; t < 8; ++t) {
+          const float xa = v[FR(0, t)], xb = v[FR(1, t)];
+          T[t] = fmaf(mbf, xa, xb);  // the run through my second row: both rows, or the second alone after a boundary
+          H[t] = bb ? xa : T[t];     // my rows before the first boundary: what the owner of the run that reaches me adds
+        }
+        const bool sts_on = !ABL3(ABL_STORES);
+        if (head_st && sts_on) st256(carry_p + 128 * u, H[0], H[1], H[2], H[3], H[4], H[5], H[6], H[7]);
+        if (one_any) {
+          if (one_st && sts_on) {
+            char* dp = reinterpret_cast<char*>(L.seg_out + ((size_t)bs * L.seg_rows + (size_t)(uint32_t)d0) * (size_t)L.seg_ld + fcofs);
+            float a1[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            if (L.seg_add) ld256(reinterpret_cast<const char*>(L.seg_add + (size_t)(uint32_t)d0 * (size_t)L.seg_ld + fcofs) + 128 * u, a1);
+            st256(dp + 128 * u, H[0] + a1[0], H[1] + a1[1], H[2] + a1[2], H[3] + a1[3], H[4] + a1[4], H[5] + a1[5], H[6] + a1[6], H[7] + a1[7]);
           }
         }
-        if constexpr (relu) {
 #pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
+        for (int t = 0; t < 8; ++t) {
+          const float h1 = __shfl_down_sync(0xffffffffu, H[t], 4);
+          T[t] = fmaf(c1f, h1, T[t]);
+          H[t] = fmaf(kf, h1, H[t]);  // G1
         }
-        if constexpr (has_ln) {
-          const float4 gl = lds128(g_a + 256 * s), gh = lds128(g_a + 256 * s + 16);
-          const float4 el = lds128(b_a + 256 * s), eh = lds128(b_a + 256 * s + 16);
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int m = (i >> 1) & 1;
-            v[i] = fmaf(fmaf(v[i], rs[m], sh[m]), col8(gl, gh, i), col8(el, eh, i));
-          }
-        }
-        if constexpr (has_res) {
-          if (ld_on) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] += pf0[PX(i)];
-          }
-        }
-        if constexpr (has_ln) tr.ev(2020 + s);
-        if constexpr (s + 1 < NP) {  // next chunk's global operands: in flight while this chunk is stored / converted
-          if constexpr (has0) {
-            if (ld_on) ld2(p0, 256 * (s + 1), pf0);
-          }
-          if constexpr (has_add1) {
-            if (ld_on) ld2(p1, 256 * (s + 1), pf1);
-          }
-        }
-        if constexpr (has_out) {
-          if (!ABL3(ABL_STORES)) {
-            if (st0) st256(po + 256 * s, v[FR(0, 0)], v[FR(0, 1)], v[FR(0, 2)], v[FR(0, 3)], v[FR(0, 4)], v[FR(0, 5)], v[FR(0, 6)], v[FR(0, 7)]);
-            if (st1) st256(po + ostr + 256 * s, v[FR(1, 0)], v[FR(1, 1)], v[FR(1, 2)], v[FR(1, 3)], v[FR(1, 4)], v[FR(1, 5)], v[FR(1, 6)], v[FR(1, 7)]);
-          }
-        }
-        if constexpr (has_ln) tr.ev(2030 + s);
-        if constexpr (has_seg) {
-          float T[8], H[8];
+        for (int t = 0; t < 8; ++t) T[t] = fmaf(e2f, __shfl_down_sync(0xffffffffu, H[t], 8), T[t]);
+        if (deep) {
 #pragma unroll
           for (int t = 0; t < 8; ++t) {
-            const float xa = v[FR(0, t)], xb = v[FR(1, t)];
-            T[t] = fmaf(mbf, xa, xb);  // the run through my second row: both rows, or the second alone after a boundary
-            H[t] = bb ? xa : T[t];     // my rows before the first boundary: what the owner of the run that reaches me adds
+            const float g2 = fmaf(k1f, __shfl_down_sync(0xffffffffu, H[t], 8), H[t]);  // G2
+            T[t] = fmaf(e4f, __shfl_down_sync(0xffffffffu, g2, 16), T[t]);
           }
-          const bool sts_on = !ABL3(ABL_STORES);
-          if (head_st && sts_on) st256(carry_p + 256 * s, H[0], H[1], H[2], H[3], H[4], H[5], H[6], H[7]);
-          if (one_any) {
-            if (one_st && sts_on) {
-              char* dp = reinterpret_cast<char*>(L.seg_out + ((size_t)bs * L.seg_rows + (size_t)(uint32_t)d0) * (size_t)L.seg_ld + fcofs);
-              float a1[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-              if (L.seg_add) ld256(reinterpret_cast<const char*>(L.seg_add + (size_t)(uint32_t)d0 * (size_t)L.seg_ld + fcofs) + 256 * s, a1);
-              st256(dp + 256 * s, H[0] + a1[0], H[1] + a1[1], H[2] + a1[2], H[3] + a1[3], H[4] + a1[4], H[5] + a1[5], H[6] + a1[6], H[7] + a1[7]);
-            }
-          }
-#pragma unroll
-          for (int t = 0; t < 8; ++t) {
-            const float h1 = __shfl_down_sync(0xffffffffu, H[t], 4);
-            T[t] = fmaf(c1f, h1, T[t]);
-            H[t] = fmaf(kf, h1, H[t]);  // G1
-          }
-#pragma unroll
-          for (int t = 0; t < 8; ++t) T[t] = fmaf(e2f, __shfl_down_sync(0xffffffffu, H[t], 8), T[t]);
-          if (deep) {
-#pragma unroll
-            for (int t = 0; t < 8; ++t) {
-              const float g2 = fmaf(k1f, __shfl_down_sync(0xffffffffu, H[t], 8), H[t]);  // G2
-              T[t] = fmaf(e4f, __shfl_down_sync(0xffffffffu, g2, 16), T[t]);
-            }
-          }
-          if (tail_st && sts_on)  // (sadd is zero for the threads that write a carry row or own no run)
-            st256(tail_p + 256 * s, T[0] + sadd[0], T[1] + sadd[1], T[2] + sadd[2], T[3] + sadd[3], T[4] + sadd[4], T[5] + sadd[5], T[6] + sadd[6],
-                  T[7] + sadd[7]);
         }
-        if constexpr (feeds) {
-          const uint32_t slot = (fi + s) % A_SLOTS;
-          if (osc != 1.f) {  // range scaling active (rare).  Two copies of the conversion keep this a real, warp-uniform branch:
-                             // as a short predicated block the 16 multiplies would be issued (predicated off) in every chunk
+        if (tail_st && sts_on)  // (sadd is zero for the threads that write a carry row or own no run)
+          st256(tail_p + 128 * u, T[0] + sadd[0], T[1] + sadd[1], T[2] + sadd[2], T[3] + sadd[3], T[4] + sadd[4], T[5] + sadd[5], T[6] + sadd[6],
+                T[7] + sadd[7]);
+      }
+      if constexpr (feeds) {
+        if (osc != 1.f) {
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] *= osc;
-            if (!ABL3(ABL_CONVERT)) store_operand_x4<SPLIT, false>(fsa + slot * A_SLOT_BYTES, v, amax);
-          } else {
-            if (!ABL3(ABL_CONVERT)) store_operand_x4<SPLIT, false>(fsa + slot * A_SLOT_BYTES, v, amax);
-          }
-          publish(slot);
+          for (int i = 0; i < 16; ++i) v[i] *= osc;
         }
-        tr.ev(700 + 10 * l + s);
-      });
-      if constexpr (feeds) fi += NP;
-    };
+        if (!ABL3(ABL_CONVERT)) store_operand_x4<SPLIT, false>(op_addr(u), v, amax);
+      }
+      tr.ev(700 + 10 * l + u);
+    });
+    if constexpr (feeds) publish();
+  };
 
-    // ---- the forecast's output layer on the lean path ---------------------------------------------------------------------------
-    // N is padded to 64 k columns of which n_valid (78) are real; the rows of the output and of the residual (the start features)
-    // are only 8-byte aligned: 64-bit accesses, one pair of columns at a time, warps whose 32 columns lie beyond n_valid idle.
-    // Keeping this layer in the node chain saves the hidden rows' round trip through HBM and a general-path chain per step.
-    auto layer_out_narrow = [&](auto /*instantiated in MODE 2 only*/, int l, uint32_t acc, uint32_t use, bool waited, int tile) {
-      const TcLayer& L = ch.layer[l];
-      const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
-      const int nvalid = min(TILE_M, rows - i0);
-      const int np = L.N >> 6, nval = L.n_valid;
-      const float wsi = scl[2 * l];
-      const uint32_t bias_a = sbase + OFF_PAR + 4 * fcofs + l * 1024;
-      const uint32_t taddr = tmem_base + ftm + acc * 256;
-      const bool has_res = L.residual.kind != SRC_NONE;
-      const float* rp[2] = {nullptr, nullptr};
-      if (has_res) {
-        const float* base = reinterpret_cast<const float*>(src_sample_base(L.residual, bs));
+  // ---- the forecast's output layer on the lean path ---------------------------------------------------------------------------
+  // N is padded to 64 k columns of which n_valid (78) are real; the rows of the output and of the residual (the start features)
+  // are only 8-byte aligned: 64-bit accesses, one pair of columns at a time, steps beyond n_valid idle.  Keeping this layer in the
+  // node chain saves the hidden rows' round trip through HBM and a general-path chain per step.
+  auto layer_out_narrow = [&](float (&acc)[128], int l, int tile) GW_INLINE {
+    const TcLayer& L = ch.layer[l];
+    const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
+    const int nvalid = min(TILE_M, rows - i0);
+    const int nu = L.N >> 5, nval = L.n_valid;
+    const bool has_res = L.residual.kind != SRC_NONE;
+    const float* rp[2] = {nullptr, nullptr};
+    if (has_res) {
+      const float* base = reinterpret_cast<const float*>(src_sample_base(L.residual, bs));
 #pragma unroll
-        for (int m = 0; m < 2; ++m) rp[m] = base + (size_t)(uint32_t)(i0 + min(fr0 + m, nvalid - 1)) * (size_t)L.residual.ld;
-      }
-      float* op[2];
+      for (int m = 0; m < 2; ++m) rp[m] = base + (size_t)(uint32_t)(i0 + min(fr0 + m, nvalid - 1)) * (size_t)L.residual.ld;
+    }
+    float* op[2];
 #pragma unroll
-      for (int m = 0; m < 2; ++m) op[m] = L.out + ((size_t)bs * rows + i0 + fr0 + m) * (size_t)L.ldo;
-      const bool st[2] = {fr0 < nvalid, fr0 + 1 < nvalid};
-      if (!waited) {
-        tr.ev(600 + l);
-        mbar_wait(bar_full_d + 8 * acc, use & 1, ch.status);
-        tc_fence_after();
-        tr.ev(610 + l);
-      }
-      for (int s = 0; s < np; ++s) {
-        const int c0 = 64 * s + fcofs;
-        const bool any = 64 * s + 32 * fc < nval;  // warp-uniform: my warp's 32 columns of this chunk hold real features
+    for (int m = 0; m < 2; ++m) op[m] = L.out + ((size_t)bs * rows + i0 + fr0 + m) * (size_t)L.ldo;
+    const bool st[2] = {fr0 < nvalid, fr0 + 1 < nvalid};
+    bias_in_place(acc, l, nu, scl[2 * l]);
+    static_for<0, 8>([&](auto uu) GW_INLINE {
+      constexpr int u = decltype(uu)::value;
+      const int c0 = 32 * u + fcofs;
+      if (u < nu && 32 * u < nval) {  // warp-uniform: this step holds real features
         float2 r[2][4] = {};
-        if (any && has_res && !ABL3(ABL_LOADS)) {
+        if (has_res && !ABL3(ABL_LOADS)) {
 #pragma unroll
           for (int m = 0; m < 2; ++m)
 #pragma unroll
             for (int g = 0; g < 4; ++g)
               if (c0 + 2 * g < nval) r[m][g] = __ldg(reinterpret_cast<const float2*>(rp[m] + c0 + 2 * g));
         }
-        float v[16] = {};
-        if (any && !ABL3(ABL_TMEM)) {
-          tmem_ld_16x256b_x4(taddr + 64 * s, v);
-          tmem_wait_ld();
-        }
-        if (s + 1 == np) {  // my last read of this accumulator
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_empty_d + 8 * acc);
-        }
-        if (any) {
-          const float4 bl = lds128(bias_a + 256 * s), bh = lds128(bias_a + 256 * s + 16);
+        if (!ABL3(ABL_STORES)) {
 #pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = fmaf(v[i], wsi, col8(bl, bh, i));
-          if (!ABL3(ABL_STORES)) {
+          for (int m = 0; m < 2; ++m)
 #pragma unroll
-            for (int m = 0; m < 2; ++m)
-#pragma unroll
-              for (int g = 0; g < 4; ++g)
-                if (st[m] && c0 + 2 * g < nval)  // (n_valid is even: a pair is inside or outside as a whole)
-                  *reinterpret_cast<float2*>(op[m] + c0 + 2 * g) = make_float2(v[4 * g + 2 * m] + r[m][g].x, v[4 * g + 2 * m + 1] + r[m][g].y);
-          }
+            for (int g = 0; g < 4; ++g)
+              if (st[m] && c0 + 2 * g < nval)  // (n_valid is even: a pair is inside or outside as a whole)
+                *reinterpret_cast<float2*>(op[m] + c0 + 2 * g) =
+                    make_float2(acc[16 * u + 4 * g + 2 * m] + r[m][g].x, acc[16 * u + 4 * g + 2 * m + 1] + r[m][g].y);
         }
-        tr.ev(700 + 10 * l + s);
+      }
+    });
+  };
+
+  // ---- one layer's epilogue, general path: any N (multiple of 64 in the perm32 image), n_valid real columns, sources and outputs
+  // of any width and alignment ---------------------------------------------------------------------------------------------------
+  auto layer_gen = [&](float (&acc)[128], int l, int tile, int ln_slot, bool last_layer) GW_INLINE {
+    const TcLayer& L = ch.layer[l];
+    const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
+    const int nvalid = min(TILE_M, rows - i0);
+    const int nu = L.N >> 5, nval = L.n_valid;
+    const float osc = scl[2 * l + 1];
+    const bool has_add0 = L.add[0].kind != SRC_NONE, has_add1 = L.add[1].kind != SRC_NONE;
+    const bool has_res = L.residual.kind != SRC_NONE, has_out = L.out != nullptr;
+    const bool relu = L.relu != 0, feeds = L.feeds_next != 0, has_ln = L.ln_g != nullptr;
+    const uint32_t g_a = sbase + OFF_LNP + 4 * fcofs + (ln_slot * 2) * 1024, b_a = g_a + 1024;
+    const int r2[2] = {min(fr0, nvalid - 1), min(fr0 + 1, nvalid - 1)};
+    const float* q0[2] = {nullptr, nullptr};  // addend 0 / residual rows
+    const float* q1[2] = {nullptr, nullptr};  // addend 1 rows
+    const RowSrc& src0 = has_add0 ? L.add[0] : L.residual;
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+      if (has_add0 || has_res) q0[m] = src_row(src0, bs, i0, r2[m]);
+      if (has_add1) q1[m] = src_row(L.add[1], bs, i0, r2[m]);
+    }
+    bias_in_place(acc, l, nu, scl[2 * l]);
+    float rs[2] = {1.f, 1.f}, sh[2] = {0.f, 0.f};
+    if (has_ln && !ABL3(ABL_LN)) ln_stats(acc, nu, nval, rs, sh);
+    // where the values go: this GPU's memory, or (last layer of the forecast chain on a multi-GPU job) every GPU's gather buffer at
+    // once -- NVLink multicast or one store per peer mapping
+    const int omode = last_layer ? ch.out_mode : 0;
+    const ptrdiff_t mc_delta = reinterpret_cast<const char*>(ch.out_mc) - reinterpret_cast<const char*>(L.out);
+    auto put4 = [&](float* p, float a, float b, float c, float d) GW_INLINE {
+      if (omode == 0) {
+        *reinterpret_cast<float4*>(p) = make_float4(a, b, c, d);
+      } else if (omode == 1) {
+        asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(reinterpret_cast<char*>(p) + mc_delta), "f"(a), "f"(b),
+                     "f"(c), "f"(d)
+                     : "memory");
+      } else {
+        for (int j = 0; j < ch.n_out_peers; ++j)
+          *reinterpret_cast<float4*>(reinterpret_cast<char*>(p) + (reinterpret_cast<const char*>(ch.out_peer[j]) - reinterpret_cast<const char*>(L.out))) =
+              make_float4(a, b, c, d);
       }
     };
-
-    const int n_layers = ch.n_layers;
-    bool first_tile = true;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, first_tile = false) {
-      const int bs = tile % batch, i0 = (tile / batch) * TILE_M;
-      const int nvalid = min(TILE_M, rows - i0);
-      const int next_tile = tile + gridDim.x;
-      int rl[4];
+    auto put1 = [&](float* p, float a) GW_INLINE {
+      if (omode == 0) {
+        *p = a;
+      } else if (omode == 1) {
+        asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(reinterpret_cast<char*>(p) + mc_delta), "f"(a) : "memory");
+      } else {
+        for (int j = 0; j < ch.n_out_peers; ++j)
+          *reinterpret_cast<float*>(reinterpret_cast<char*>(p) + (reinterpret_cast<const char*>(ch.out_peer[j]) - reinterpret_cast<const char*>(L.out))) = a;
+      }
+    };
+    static_for<0, 8>([&](auto uu) GW_INLINE {
+      constexpr int u = decltype(uu)::value;
+      if (u < nu) {
+        const int col = 32 * u + fcofs;
+        const bool ld_ok = !ABL3(ABL_LOADS);
+        float v[16];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) rl[k] = min(re[k], nvalid - 1);
-      int ln_slot = 0;
-      // l == -1 (first tile only): this tile's own stage 0.  Afterwards stage 0 of tile t+1 runs inside tile t's last layer.
-      for (int l = first_tile ? -1 : 0; l < n_layers; ++l) {
-        const uint32_t acc = li & 1, use = li >> 1;
-        const bool last_layer = l + 1 == n_layers;
-        if (l < 0 || last_layer) {
-          // Stage 0 of the next tile is assembled here, before this tile's last epilogue: each operand slot is refilled as soon
-          // as the last layer's MMAs have read it (empty_a), so the assembly overlaps the tail of those MMAs and the next
-          // tile's first layer then runs on the other accumulator under this tile's last epilogue.  (Placed before any
-          // per-layer state is live: the assembly needs the registers.)
-          const int t = l < 0 ? tile : next_tile;
-          if (t < num_tiles) {
-            if constexpr (MODE >= 1) {
-              if (ch.a0[1].kind != SRC_NONE) stage0_fast(ic<4>{}, ic<4>{}, ic<0>{}, t);  // node chains: [x | aggregate]
-              else if (ch.a0[0].kind == SRC_GATHER_BCAST_RELU) stage0_fast(ic<4>{}, ic<0>{}, ic<1>{}, t);  // decoder edges
-              else if (ch.K0 == 256) stage0_fast(ic<4>{}, ic<0>{}, ic<0>{}, t);          // edge chains, products of x
-              else stage0_fast(ic<2>{}, ic<0>{}, ic<0>{}, t);                            // widened feature rows (K0 = 128)
-            } else {
-              stage0(t);
-            }
-          }
-          if (l < 0) continue;
-          tr.ev(600 + l);
-          mbar_wait(bar_full_d + 8 * acc, use & 1, ch.status);
-          tc_fence_after();
-          tr.ev(610 + l);
+        for (int i = 0; i < 16; ++i) v[i] = acc[16 * u + i];
+        float t[16];
+        if (has_add0 && ld_ok) {
+          load8(q0[0], col, src0.width, t), load8(q0[1], col, src0.width, t + 8);
+#pragma unroll
+          for (int i = 0; i < 16; ++i) v[i] += t[PX(i)];
         }
-        const TcLayer& L = ch.layer[l];
-        const bool has_ln = L.ln_g != nullptr;
-        if constexpr (MODE >= 1) {
-#define GW_LF(M, NP_) layer_fast(ic<(M)>{}, ic<(NP_)>{}, l, acc, use, last_layer, tile, ln_slot)
-#define GW_LF4(M) case (M): GW_LF(M, 4); break
-#define GW_LF24(M) case (M): if (L.N == 256) GW_LF(M, 4); else GW_LF(M, 2); break
-          bool narrow_done = false;
-          if constexpr (MODE == 2) {  // (a kernel of its own: with this layer compiled in, ptxas spills scalars in EVERY chain -- measured:
-                                      //  proc_edge +11 % -- so only the chain that ends in the forecast's output layer carries it)
-            if (L.kind & F_NARROW) {
-              layer_out_narrow(ic<0>{}, l, acc, use, last_layer, tile);
-              narrow_done = true;
-            }
-          }
-          if (!narrow_done)
-          switch (L.kind) {
-            GW_LF4(F_ADD0 | F_ADD1 | F_RELU | F_FEEDS);  // edge layer 1: gathered P[src] + P[dst]
-            GW_LF4(F_ADD0 | F_RELU | F_FEEDS);           // encoder edge layer 1: broadcast constant term
-            GW_LF24(F_RELU | F_FEEDS);                   // hidden layers (N = 128: node_decoder)
-            GW_LF4(F_LN | F_RES | F_OUT);                // last layer of an edge / node MLP
-            GW_LF4(F_LN | F_RES | F_OUT | F_SEG);        // ... of the processor's edge MLP: e' rows and their per-node sums
-            GW_LF4(F_LN | F_RES | F_SEG);                // ... of the decoder's edge MLP: per-point sums only, e' is never written
-            GW_LF4(F_LN | F_SEG);                        // ... with its constant residual hoisted into a per-point constant (seg_add)
-            GW_LF4(F_LN | F_RES | F_OUT | F_FEEDS);      // ... whose rows are also the operand of the next block's P products
-            GW_LF4(F_LN | F_FEEDS);                      // LayerNorm feeding the next MLP of the same chain
-            GW_LF4(F_OUT);                               // per-node products P = x W^T
-            GW_LF24(F_RELU | F_OUT);
-            default: break;                              // (the launcher sends chains with any other layer to the general path)
-          }
-#undef GW_LF24
-#undef GW_LF4
-#undef GW_LF
-          if (has_ln) ++ln_slot;
-          ++li;
-          tr.ev(900 + l);
-          continue;
+        if (has_add1 && ld_ok) {
+          load8(q1[0], col, L.add[1].width, t), load8(q1[1], col, L.add[1].width, t + 8);
+#pragma unroll
+          for (int i = 0; i < 16; ++i) v[i] += t[PX(i)];
         }
-        const int N = L.N, nval = L.n_valid;
-        const int np = (N + 63) >> 6;
-        const float wsi = scl[2 * l], osc = scl[2 * l + 1];
-        const uint32_t bias_o = OFF_PAR + 4 * cofs + l * 1024;
-        const bool has_add0 = L.add[0].kind != SRC_NONE, has_add1 = L.add[1].kind != SRC_NONE;
-        const bool has_res = L.residual.kind != SRC_NONE, has_out = L.out != nullptr;
-        const bool relu = L.relu != 0, feeds = L.feeds_next != 0;
-        const uint32_t g_o = OFF_LNP + 4 * cofs + (ln_slot * 2) * 1024, b_o = g_o + 1024;
-        if (has_ln) ++ln_slot;
-        const uint32_t taddr = tmem_base + ((uint32_t)(32 * q) << 16) + acc * 256 + 16 * hq;
-
-        // Epilogue operands that come from global memory, prefetched one chunk ahead into pf0 / pf1:
-        //   pf0 = addend 0 (before the activation) or, on layers without addends, the residual (after LayerNorm); pf1 = addend 1
-        const RowSrc& src0 = has_add0 ? L.add[0] : L.residual;
-        const bool has0 = has_add0 || has_res;
-        int r0[4] = {0, 0, 0, 0}, r1[4] = {0, 0, 0, 0};
-        float pf0[16] = {}, pf1[16] = {};
-        auto prefetch = [&](int s) {
-          if (64 * s + 16 * hq >= N || ABL3(ABL_LOADS)) return;
-          if (has0) load16(src0, bs, r0, 64 * s + cofs, lc, pf0);
-          if (has_add1) load16(L.add[1], bs, r1, 64 * s + cofs, lc, pf1);
-        };
-        if (has0) rows_of(src0, i0, rl, r0);
-        if (has_add1) rows_of(L.add[1], i0, rl, r1);
-        prefetch(0);
-        if (!last_layer) {
-          tr.ev(600 + l);
-          mbar_wait(bar_full_d + 8 * acc, use & 1, ch.status);
-          tc_fence_after();
-          tr.ev(610 + l);
+        if (relu) {
+#pragma unroll
+          for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
         }
-
-        // LayerNorm statistics (first pass over the accumulator).  Each thread reduces its 16 columns of each of its 4 rows
-        // around a pivot (the row's first value it sees), the partial (mean, M2) pairs are merged with Chan's formula over
-        // the 4 lanes and 4 warps that share a row: one pass, no cancellation, one barrier.
-        float mean[4] = {0.f, 0.f, 0.f, 0.f}, rstd[4] = {1.f, 1.f, 1.f, 1.f};
-        if (has_ln && !ABL3(ABL_LN)) {
-          float pv[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-          int cnt = 0;
-          for (int s = 0; s < np; ++s) {
-            if (64 * s + 16 * hq >= N) break;
-            float v[16];
-            tmem_ld_16x256b_x2(taddr + 64 * s, v);
-            tmem_ld_16x256b_x2(taddr + 64 * s + (16u << 16), v + 8);
-            tmem_wait_ld();
-            const float4 b4 = *reinterpret_cast<const float4*>(smem + bias_o + 256 * s);
+        if (has_ln) {
+          const float4 gl = lds128(g_a + 128 * u), gh = lds128(g_a + 128 * u + 16);
+          const float4 el = lds128(b_a + 128 * u), eh = lds128(b_a + 128 * u + 16);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = fmaf(v[i], wsi, ((i >> 2) & 1) ? ((i & 1) ? b4.w : b4.z) : ((i & 1) ? b4.y : b4.x));
-            if (s == 0) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) pv[k] = v[8 * (k >> 1) + 2 * (k & 1)];
-            }
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const int k = 2 * (i >> 3) + ((i >> 1) & 1);
-              const float d = v[i] - pv[k];
-              s1[k] += d;
-              s2[k] = fmaf(d, d, s2[k]);
-            }
-            cnt += 4;
-          }
-          float m2[4];
-          const float fc = (float)cnt, ic = cnt > 0 ? 1.0f / fc : 0.f;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const float a = s1[k] * ic;
-            mean[k] = pv[k] + a;
-            m2[k] = fmaxf(s2[k] - s1[k] * a, 0.f);
-          }
-          float nn = fc;  // values per partial; the four lanes of a row hold equally many
-#pragma unroll
-          for (int o = 1; o <= 2; o <<= 1) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const float mb = __shfl_xor_sync(0xffffffffu, mean[k], o), qb = __shfl_xor_sync(0xffffffffu, m2[k], o);
-              const float d = mb - mean[k];
-              mean[k] = 0.5f * (mean[k] + mb);
-              m2[k] = (m2[k] + qb) + d * d * (0.5f * nn);
-            }
-            nn *= 2.f;
-          }
-          float* const ln_x = ln_base + (ln_gen & 1u) * (2 * WSPLIT * 128);
-          float* const ln_y = ln_x + WSPLIT * 128;
-          ++ln_gen;
-          if (lc == 0) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) ln_x[hq * 128 + rt[k]] = mean[k], ln_y[hq * 128 + rt[k]] = m2[k];
-          }
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + q) : "memory");  // the four warps of this lane quadrant
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            float n = 0.f, mu = 0.f, q2 = 0.f;
-#pragma unroll
-            for (int w = 0; w < WSPLIT; ++w) {  // same order in every thread of the row
-              const int cw = (N - 16 * w + 63) >> 6;  // chunks in which warp w owns columns
-              const float nw = cw > 0 ? 16.f * (float)cw : 0.f;
-              if (nw > 0.f) {
-                const float mw = ln_x[w * 128 + rt[k]], qw = ln_y[w * 128 + rt[k]];
-                const float d = mw - mu, nt = n + nw;
-                mu += d * (nw / nt);
-                q2 += qw + d * d * (n * nw / nt);
-                n = nt;
-              }
-            }
-            mean[k] = mu;
-            rstd[k] = 1.0f / sqrtf(q2 / (float)nval + 1e-5f);
+          for (int i = 0; i < 16; ++i) {
+            const int m = (i >> 1) & 1;
+            v[i] = fmaf(fmaf(v[i], rs[m], sh[m]), col8(gl, gh, i), col8(el, eh, i));
           }
         }
-
-        for (int s = 0; s < np; ++s) {
-          const bool have = 64 * s + 16 * hq < N;  // warp-uniform
-          const int col = 64 * s + cofs;
-          float v[16];
-          if (have && !ABL3(ABL_TMEM)) {
-            tmem_ld_16x256b_x2(taddr + 64 * s, v);
-            tmem_ld_16x256b_x2(taddr + 64 * s + (16u << 16), v + 8);
-            tmem_wait_ld();
-            const float4 b4 = *reinterpret_cast<const float4*>(smem + bias_o + 256 * s);
+        if (!has_add0 && has_res && ld_ok) {
+          load8(q0[0], col, src0.width, t), load8(q0[1], col, src0.width, t + 8);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = fmaf(v[i], wsi, ((i >> 2) & 1) ? ((i & 1) ? b4.w : b4.z) : ((i & 1) ? b4.y : b4.x));
-          } else {
+          for (int i = 0; i < 16; ++i) v[i] += t[PX(i)];
+        }
+        if (nval < L.N) {  // padded output columns (e.g. 78 of 128) must stay exactly zero
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] = 0.f;
-          }
-          if (s + 1 == np) {  // my last read of this accumulator
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_empty_d + 8 * acc);
-          }
-          if (have) {
-            const bool ld_ok = !ABL3(ABL_LOADS);
-            if (has_add0 && ld_ok) {
+          for (int i = 0; i < 16; ++i)
+            if (col + 2 * (i >> 2) + (i & 1) >= nval) v[i] = 0.f;
+        }
+        if (has_out && !ABL3(ABL_STORES)) {
 #pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] += pf0[i];
-            }
-            if (has_add1 && ld_ok) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] += pf1[i];
-            }
-            if (relu) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
-            }
-            if (has_ln) {
-              const float4 g4 = *reinterpret_cast<const float4*>(smem + g_o + 256 * s);
-              const float4 e4 = *reinterpret_cast<const float4*>(smem + b_o + 256 * s);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const int k = 2 * (i >> 3) + ((i >> 1) & 1);
-                const float gx = ((i >> 2) & 1) ? ((i & 1) ? g4.w : g4.z) : ((i & 1) ? g4.y : g4.x);
-                const float ex = ((i >> 2) & 1) ? ((i & 1) ? e4.w : e4.z) : ((i & 1) ? e4.y : e4.x);
-                v[i] = fmaf((v[i] - mean[k]) * rstd[k], gx, ex);
-              }
-            }
-            if (!has_add0 && has_res && ld_ok) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] += pf0[i];
-            }
-          }
-          if (s + 1 < np) prefetch(s + 1);  // in flight while this chunk is converted and stored
-          if (have) {
-            if (nval < N) {  // padded output columns (e.g. 78 of 80) must stay exactly zero
-#pragma unroll
-              for (int i = 0; i < 16; ++i)
-                if (col + 2 * ((i >> 2) & 1) + (i & 1) >= nval) v[i] = 0.f;
-            }
-            if (has_out && !ABL3(ABL_STORES)) {
-              float* ob = L.out + ((size_t)bs * rows + i0) * (size_t)L.ldo + col;
-              const bool inside = 64 * s + 16 * hq + 16 <= L.out_cols;  // warp-uniform
-              // where the values go: this GPU's memory, or (last layer of the forecast chain on a multi-GPU job) every GPU's gather
-              // buffer at once -- NVLink multicast or one store per peer mapping
-              const int omode = last_layer ? ch.out_mode : 0;
-              const ptrdiff_t mc_delta = reinterpret_cast<const char*>(ch.out_mc) - reinterpret_cast<const char*>(L.out);
-              auto put4 = [&](float* p, float a, float b, float c, float d) {
-                if (omode == 0) {
-                  *reinterpret_cast<float4*>(p) = make_float4(a, b, c, d);
-                } else if (omode == 1) {
-                  asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(reinterpret_cast<char*>(p) + mc_delta), "f"(a), "f"(b),
-                               "f"(c), "f"(d)
-                               : "memory");
-                } else {
-                  for (int j = 0; j < ch.n_out_peers; ++j)
-                    *reinterpret_cast<float4*>(reinterpret_cast<char*>(p) + (reinterpret_cast<const char*>(ch.out_peer[j]) - reinterpret_cast<const char*>(L.out))) =
-                        make_float4(a, b, c, d);
-                }
-              };
-              auto put2 = [&](float* p, float a, float b) {
-                if (omode == 0) {
-                  *reinterpret_cast<float2*>(p) = make_float2(a, b);
-                } else if (omode == 1) {
-                  asm volatile("multimem.st.relaxed.sys.global.v2.f32 [%0], {%1, %2};" ::"l"(reinterpret_cast<char*>(p) + mc_delta), "f"(a), "f"(b) : "memory");
-                } else {
-                  for (int j = 0; j < ch.n_out_peers; ++j)
-                    *reinterpret_cast<float2*>(reinterpret_cast<char*>(p) + (reinterpret_cast<const char*>(ch.out_peer[j]) - reinterpret_cast<const char*>(L.out))) =
-                        make_float2(a, b);
-                }
-              };
-              auto put1 = [&](float* p, float a) {
-                if (omode == 0) {
-                  *p = a;
-                } else if (omode == 1) {
-                  asm volatile("multimem.st.relaxed.sys.global.f32 [%0], %1;" ::"l"(reinterpret_cast<char*>(p) + mc_delta), "f"(a) : "memory");
-                } else {
-                  for (int j = 0; j < ch.n_out_peers; ++j)
-                    *reinterpret_cast<float*>(reinterpret_cast<char*>(p) + (reinterpret_cast<const char*>(ch.out_peer[j]) - reinterpret_cast<const char*>(L.out))) = a;
-                }
-              };
-              if (inside && vec4_ok(ob - col, L.ldo)) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  if (re[k] < nvalid) {
-                    const int i = 8 * (k >> 1) + 2 * (k & 1);
-                    put4(ob + (size_t)re[k] * (size_t)L.ldo, v[i], v[i + 1], v[i + 4], v[i + 5]);
-                  }
-                }
-              } else if (inside && vec2_ok(ob - col, L.ldo)) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  if (re[k] < nvalid) {
-                    float* orow = ob + (size_t)re[k] * (size_t)L.ldo;
-                    const int i = 8 * (k >> 1) + 2 * (k & 1);
-                    put2(orow, v[i], v[i + 1]);
-                    put2(orow + 2, v[i + 4], v[i + 5]);
-                  }
-                }
+          for (int m = 0; m < 2; ++m) {
+            if (fr0 + m < nvalid) {
+              float* orow = L.out + ((size_t)bs * rows + i0 + fr0 + m) * (size_t)L.ldo + col;
+              if (col + 8 <= L.out_cols && (reinterpret_cast<uintptr_t>(orow) & 15) == 0) {
+                put4(orow, v[FR(m, 0)], v[FR(m, 1)], v[FR(m, 2)], v[FR(m, 3)]);
+                put4(orow + 4, v[FR(m, 4)], v[FR(m, 5)], v[FR(m, 6)], v[FR(m, 7)]);
               } else {
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  if (re[k] < nvalid) {
-                    float* orow = ob + (size_t)re[k] * (size_t)L.ldo;
-#pragma unroll
-                    for (int j = 0; j < 2; ++j) {
-                      const int i = 8 * (k >> 1) + 4 * j + 2 * (k & 1), c = col + 2 * j;
-                      if (c < L.out_cols) put1(orow + 2 * j, v[i]);
-                      if (c + 1 < L.out_cols) put1(orow + 2 * j + 1, v[i + 1]);
-                    }
-                  }
-                }
+                for (int k = 0; k < 8; ++k)
+                  if (col + k < L.out_cols) put1(orow + k, v[FR(m, k)]);
               }
             }
           }
-          if (feeds) {
-            const uint32_t slot = (fi + s) % A_SLOTS;
-            if (osc != 1.f) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] *= osc;
-            }
-            if (!ABL3(ABL_CONVERT)) store_operand16(smem + OFF_A + slot * A_SLOT_BYTES, rt, hq, lc, v, split, amax);
-            publish(slot);
-          }
-          tr.ev(700 + 10 * l + s);
         }
-        if (feeds) fi += np;
-        ++li;
-        tr.ev(900 + l);
+        if (feeds) {
+          if (osc != 1.f) {
+#pragma unroll
+            for (int i = 0; i < 16; ++i) v[i] *= osc;
+          }
+          if (!ABL3(ABL_CONVERT)) store_operand_x4<SPLIT, false>(op_addr(u), v, amax);
+        }
       }
-    }
-    if (split && ch.status && amax > 60000.f) atomicOr(ch.status, 1);  // operand left the fp16 range: results invalid
-  }
+    });
+    if (feeds) publish();
+  };
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == WARP_MMA) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+  // One layer of the chain on the tile: its product (N, the wgmma shape, at compile time) and its epilogue.
+  auto run_layer = [&](auto Nc, int l, int tile, int ln_slot) GW_INLINE {
+    constexpr int N = decltype(Nc)::value;
+    const TcLayer& L = ch.layer[l];
+    float acc[128];  // (per layer: the first wgmma of the layer overwrites it, so nothing is live across stage 0)
+    auto mma = [&](int kc0, int kc1) GW_INLINE {
+      tr.ev(100 + kc0);
+      mma_chunks<SPLIT, N>(acc, a_rows, sbase + OFF_B, bar_full_b, bar_empty_b, bi, kc0, kc1);
+      wg_sync();  // every wgmma of my warpgroup has read its operand: the epilogue may overwrite it
+      tr.ev(110 + kc0);
+    };
+    if (l == 0) {
+      // stage 0 in windows of A_SLOTS chunks, each multiplied as soon as it is assembled
+      const int nk0 = ch.K0 >> 6;
+      for (int w = 0; 4 * w < nk0; ++w) {
+        tr.ev(480 + w);
+        if constexpr (MODE >= 1) {
+          if (ch.a0[1].kind != SRC_NONE) {  // node chains: [x | aggregate]
+            if (w == 0) stage0_fast(ic<4>{}, ic<4>{}, ic<0>{}, ic<0>{}, tile);
+            else stage0_fast(ic<4>{}, ic<4>{}, ic<0>{}, ic<1>{}, tile);
+          } else if (ch.a0[0].kind == SRC_GATHER_BCAST_RELU) {
+            stage0_fast(ic<4>{}, ic<0>{}, ic<1>{}, ic<0>{}, tile);  // decoder edges
+          } else if (ch.K0 == 256) {
+            stage0_fast(ic<4>{}, ic<0>{}, ic<0>{}, ic<0>{}, tile);  // edge chains, products of x
+          } else {
+            stage0_fast(ic<2>{}, ic<0>{}, ic<0>{}, ic<0>{}, tile);  // widened feature rows (K0 = 128)
+          }
+        } else {
+          stage0(tile, w);
+        }
+        mma(4 * w, min(nk0, 4 * w + 4));
+      }
+    } else {
+      mma(0, L.K >> 6);  // the operand the previous layer left (or, reuse_a, the one it multiplied)
+    }
+    if constexpr (MODE >= 1) {
+      if constexpr (MODE == 2) {  // (a kernel of its own: only the chain that ends in the forecast's output layer carries it)
+        if (L.kind & F_NARROW) {
+          layer_out_narrow(acc, l, tile);
+          return;
+        }
+      }
+#define GW_LF(M, NP_) case (M): layer_fast(acc, ic<(M)>{}, ic<(NP_)>{}, l, tile, ln_slot); break
+      if constexpr (N == 256) {
+        switch (L.kind) {
+          GW_LF(F_ADD0 | F_ADD1 | F_RELU | F_FEEDS, 4);  // edge layer 1: gathered P[src] + P[dst]
+          GW_LF(F_ADD0 | F_RELU | F_FEEDS, 4);           // encoder edge layer 1: broadcast constant term
+          GW_LF(F_RELU | F_FEEDS, 4);                    // hidden layers
+          GW_LF(F_LN | F_RES | F_OUT, 4);                // last layer of an edge / node MLP
+          GW_LF(F_LN | F_RES | F_OUT | F_SEG, 4);        // ... of the processor's edge MLP: e' rows and their per-node sums
+          GW_LF(F_LN | F_RES | F_SEG, 4);                // ... of the decoder's edge MLP: per-point sums only, e' is never written
+          GW_LF(F_LN | F_SEG, 4);                        // ... with its constant residual hoisted into a per-point constant (seg_add)
+          GW_LF(F_LN | F_RES | F_OUT | F_FEEDS, 4);      // ... whose rows are also the operand of the next block's P products
+          GW_LF(F_LN | F_FEEDS, 4);                      // LayerNorm feeding the next MLP of the same chain
+          GW_LF(F_OUT, 4);                               // per-node products P = x W^T
+          GW_LF(F_RELU | F_OUT, 4);
+          default: break;  // (the launcher sends chains with any other layer to the general path)
+        }
+      } else {
+        switch (L.kind) {
+          GW_LF(F_RELU | F_FEEDS, 2);  // hidden layers of the node decoder (N = 128)
+          GW_LF(F_RELU | F_OUT, 2);
+          default: break;
+        }
+      }
+#undef GW_LF
+    } else {
+      layer_gen(acc, l, tile, ln_slot, l + 1 == ch.n_layers);
+    }
+  };
+
+  const int n_layers = ch.n_layers;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int ln_slot = 0;
+    for (int l = 0; l < n_layers; ++l) {
+      const int N = ch.layer[l].N;  // (64 / 128 / 192 / 256; the lean path has 128 and 256 only)
+      if constexpr (MODE >= 1) {
+        if (N == 256) run_layer(ic<256>{}, l, tile, ln_slot);
+        else run_layer(ic<128>{}, l, tile, ln_slot);
+      } else {
+        if (N == 256) run_layer(ic<256>{}, l, tile, ln_slot);
+        else if (N == 192) run_layer(ic<192>{}, l, tile, ln_slot);
+        else if (N == 128) run_layer(ic<128>{}, l, tile, ln_slot);
+        else run_layer(ic<64>{}, l, tile, ln_slot);
+      }
+      if (ch.layer[l].ln_g) ++ln_slot;
+      tr.ev(900 + l);
+    }
   }
+  if (SPLIT && ch.status && amax > 60000.f) atomicOr(ch.status, 1);  // operand left the fp16 range: results invalid
 }
 
 }  // namespace t3
 
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 static bool aligned32(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 31) == 0; }
 static bool simple_kind(int k) { return k == SRC_STREAM || k == SRC_BCAST || k == SRC_GATHER || k == SRC_BGATHER; }
 // a source every thread may read with 8-byte loads over `need` columns
@@ -1424,7 +969,7 @@ static bool fits32(const RowSrc& s) {
   return span * (long long)s.ld * 4 + 4096 < (1ll << 32);
 }
 static bool src_fast(const RowSrc& s, int need) {
-  return simple_kind(s.kind) && s.width >= need && aligned32(s.base + s.col0) && !(s.ld & 7) && fits32(s);  // 256-bit accesses
+  return simple_kind(s.kind) && s.width >= need && aligned32(s.base + s.col0) && !(s.ld & 7) && fits32(s);  // 32-byte row segments
 }
 
 // Marks which parts of a chain take the lean full-width path (ch.fast) and the epilogue kind of every layer.
@@ -1438,7 +983,7 @@ static void tc3_mark_lean(TcChain& ch) {
       const RowSrc& s = ch.a0[a];
       if (s.kind == SRC_NONE) continue;
       const bool gbr = s.kind == SRC_GATHER_BCAST_RELU;
-      ok = ok && (simple_kind(s.kind) || gbr) && aligned32(s.base + s.col0) && !(s.ld & 7);  // 256-bit loads
+      ok = ok && (simple_kind(s.kind) || gbr) && aligned32(s.base + s.col0) && !(s.ld & 7);  // 32-byte row segments
       if (gbr) ok = ok && aligned32(s.base2) && !(s.ld2 & 7);
       wsum += s.width;
     }
@@ -1456,8 +1001,8 @@ static void tc3_mark_lean(TcChain& ch) {
     const TcLayer& L = ch.layer[l];
     // the forecast's output layer: last layer, no activation / norm / addends, n_valid (even) real columns of an N32-row image,
     // output and residual rows 8-byte aligned and not gathered
-    const bool narrow = l + 1 == ch.n_layers && L.n_valid < L.N32 && !(L.n_valid & 1) && !(L.N32 & 63) && L.N32 <= 256 && L.out && !L.relu &&
-                        !L.ln_g && !L.feeds_next && !L.seg_dst && L.add[0].kind == SRC_NONE && L.add[1].kind == SRC_NONE && L.Wp32 &&
+    const bool narrow = l + 1 == ch.n_layers && L.n_valid < L.N32 && !(L.n_valid & 1) && (L.N32 == 128 || L.N32 == 256) && L.out && !L.relu &&
+                        !L.ln_g && !L.feeds_next && !L.seg_dst && L.add[0].kind == SRC_NONE && L.add[1].kind == SRC_NONE &&
                         !(reinterpret_cast<uintptr_t>(L.out) & 7) && !(L.ldo & 1) && L.out_cols >= L.n_valid &&
                         (L.residual.kind == SRC_NONE ||
                          ((L.residual.kind == SRC_STREAM || L.residual.kind == SRC_BCAST) && L.residual.width >= L.n_valid && !(L.residual.ld & 1) &&
@@ -1474,7 +1019,6 @@ static void tc3_mark_lean(TcChain& ch) {
     if (L.out) ok = ok && aligned32(L.out) && !(L.ldo & 7) && L.out_cols >= L.N;
     if (L.seg_dst) ok = ok && L.seg_out && L.seg_carry && aligned32(L.seg_out) && aligned32(L.seg_carry) && !(L.seg_ld & 7) && L.ln_g && L.N == 256;
     if (L.seg_add) ok = ok && L.seg_dst && aligned32(L.seg_add);
-    ok = ok && L.Wp32 != nullptr;
     const int f = (L.add[0].kind != SRC_NONE ? F_ADD0 : 0) | (L.add[1].kind != SRC_NONE ? F_ADD1 : 0) | (L.relu ? F_RELU : 0) |
                   (L.ln_g ? F_LN : 0) | (L.residual.kind != SRC_NONE ? F_RES : 0) | (L.out ? F_OUT : 0) | (L.feeds_next ? F_FEEDS : 0) |
                   (L.seg_dst ? F_SEG : 0);
@@ -1549,14 +1093,12 @@ cudaError_t launch_chain_tc3(const TcChain& ch_in, cudaStream_t stream) {
   tc3_mark_lean(ch);
   if (getenv("GW_TC3_NOFAST")) ch.fast = 0;
   const int32_t all = (int32_t)(0x80000000u | ((1u << ch.n_layers) - 1u));
-  // (mode 2, per-part selection inside one kernel, measured slower than the general path: both paths' live state spills)
   int mode = ch.fast == all ? 1 : 0;
   if (ch.out_mode != 0) mode = 0;  // the multi-GPU boundary stores live in the general path's store tiers
-  if (mode == 1)
-    for (int l = 0; l < ch.n_layers; ++l) {  // the lean path's feature order (perm32) and row padding (64)
-      ch.layer[l].Wp = ch.layer[l].Wp32;
-      if (ch.layer[l].N32) ch.layer[l].N = ch.layer[l].N32;
-    }
+  for (int l = 0; l < ch.n_layers; ++l) {  // both paths run on the perm32 feature order and its row padding (64)
+    if (ch.layer[l].N32 < ch.layer[l].N || (ch.layer[l].N32 & 63) || ch.layer[l].N32 > 256) return cudaErrorInvalidValue;
+    ch.layer[l].N = ch.layer[l].N32;
+  }
   if (mode == 0)
     for (int l = 0; l < ch.n_layers; ++l)
       if (ch.layer[l].seg_dst) return cudaErrorInvalidValue;  // the fused per-target sum exists on the lean path only

@@ -104,9 +104,8 @@ class BoundaryGather:
                         self._fused.append((1, [mc - ptrs[self.rank]]))
                     elif self.world <= 8:
                         self._fused.append((2, [ptrs[r] - ptrs[self.rank] for r in range(self.world)]))
-                # "auto" takes the copy engines: measured on 2 x B200 (profiles/r02_d_*), 1 degree / batch 8 per GPU, the transfer
-                # hides completely under the next forward (12.39 ms per step = the 1-GPU step), while the in-kernel stores of the
-                # 78-wide (312-byte, 8-byte aligned) forecast rows cost the last chain +0.8 ms (peer stores) / +1.5 ms (multicast)
+                # "auto" takes the copy engines: their transfer overlaps the next forward, while in-kernel stores of the 78-wide
+                # (312-byte, 8-byte aligned) forecast rows lengthen the last chain
                 self.mode = "fused" if want in ("fused", "fused_peer") and len(self._fused) == 2 else "p2p_copy"
                 return
             except Exception as e:  # no symmetric memory on this box / build: NCCL on the side stream

@@ -60,7 +60,7 @@ class MLP(nn.Module):
         if norm_type is not None:
             assert norm_type in ["LayerNorm", "GraphNorm", "InstanceNorm", "BatchNorm", "MessageNorm"]
             if norm_type != "LayerNorm":  # only LayerNorm resolves in the reference too (getattr(nn, ...), :58)
-                raise NotImplementedError(f"norm_type={norm_type!r}: only 'LayerNorm' is supported on the B200 path")
+                raise NotImplementedError(f"norm_type={norm_type!r}: only 'LayerNorm' is supported on the CUDA path")
             layers.append(nn.LayerNorm(out_dim))
         self.model = nn.Sequential(*layers)
         self.in_dim, self.out_dim, self.hidden_dim, self.hidden_layers = in_dim, out_dim, hidden_dim, hidden_layers
@@ -95,7 +95,7 @@ class GraphProcessor(nn.Module):
                  hidden_layers_node=2, hidden_layers_edge=2, norm_type="LayerNorm", use_checkpointing=False):  # fmt: skip
         super().__init__()
         if norm_type != "LayerNorm":
-            raise NotImplementedError("the B200 message-passing kernels implement LayerNorm MLPs (the reference default)")
+            raise NotImplementedError("the CUDA message-passing kernels implement LayerNorm MLPs (the reference default)")
         self.use_checkpointing = use_checkpointing
         self.blocks = nn.ModuleList()
         for _ in range(mp_iterations):
@@ -115,7 +115,7 @@ def _params_fingerprint(named):
 
 
 def _tc_eligible(dims: dict) -> bool:
-    """The tcgen05 chains are built for the reference's default sizes: 256-wide node / edge / hidden, 2 hidden layers."""
+    """The tensor-core chains are built for the reference's default sizes: 256-wide node / edge / hidden, 2 hidden layers."""
     return (dims.get("node_dim") == 256 and dims.get("edge_dim") == 256 and dims.get("hidden_node") == 256
             and dims.get("hidden_edge") == 256 and dims.get("hidden_layers_node") == 2 and dims.get("hidden_layers_edge") == 2)  # fmt: skip
 
@@ -126,17 +126,17 @@ def _validate_precision(precision: str, dims: dict):
         raise ValueError(f"precision={precision!r}: expected one of 'auto', {sorted(_capi.PRECISIONS)}")
     if precision in ("fp32", "fp32_tc", "bf16") and not _tc_eligible(dims):
         raise ValueError(
-            f"precision={precision!r} runs the tcgen05 chains, which are built for node/edge/hidden dims of 256 and 2 hidden "
+            f"precision={precision!r} runs the tensor-core chains, which are built for node/edge/hidden dims of 256 and 2 hidden "
             "layers (the reference defaults); use precision='auto' (CUDA-core exact fp32 for other sizes) or 'fp32_simt'"
         )
 
 
 def resolve_precision(precision: str, dims: dict, device) -> str:
-    """'auto' (the default of every constructor): the fp32-faithful tcgen05 path wherever it applies -- reference default
-    sizes on an sm_100 device -- and the exact-fp32 CUDA-core path otherwise.  Explicit values are returned unchanged."""
+    """'auto' (the default of every constructor): the fp32-faithful tensor-core (wgmma) path wherever it applies -- reference
+    default sizes on an sm_90 device (H100) -- and the exact-fp32 CUDA-core path otherwise.  Explicit values are returned unchanged."""
     if precision != "auto":
         return precision
-    if _tc_eligible(dims) and torch.cuda.get_device_capability(device)[0] == 10:
+    if _tc_eligible(dims) and torch.cuda.get_device_capability(device) == (9, 0):
         return "fp32"
     return "fp32_simt"
 

@@ -33,7 +33,7 @@ from .models import MLP, GraphProcessor, Processor, _Engine, _maybe_check, _no_h
 
 @dataclass
 class RegionalForecasterConfig:
-    """regional_forecast.py:16-41 (same fields and defaults) + `precision` of the B200 path."""
+    """regional_forecast.py:16-41 (same fields and defaults) + `precision` of the CUDA path."""
 
     resolution: int = 2
     feature_dim: int = 78

@@ -1,4 +1,4 @@
-/* gw_b200.h -- C ABI of libgwb200.so: the B200 (sm_100a) encode-process-decode forward of graph_weather.
+/* gw_b200.h -- C ABI of libgwb200.so: the H100 (sm_90a) encode-process-decode forward of graph_weather.
  *
  * The reference is pure Python (SURVEY.md section 2a: no native code, no FFI), so there is no existing C interface
  * to mirror; each entry point below names the reference Python call it replaces.  A maintainer binds this library
@@ -28,8 +28,8 @@ extern "C" {
 
 /* arithmetic mode of the MLP contractions */
 #define GW_PREC_FP32_SIMT 0 /* fp32 FFMA on CUDA cores (exact fp32; any hidden size)                              */
-#define GW_PREC_FP32_TC 1   /* tcgen05 kind::f16, each fp32 operand split hi+lo (2x fp16), 3 MMAs, fp32 accumulate  */
-#define GW_PREC_BF16_TC 2   /* tcgen05 kind::f16 bf16 operands, single MMA, fp32 accumulate (configs 3/4)            */
+#define GW_PREC_FP32_TC 1   /* wgmma f16, each fp32 operand split hi+lo (2x fp16), 3 MMAs, fp32 accumulate         */
+#define GW_PREC_BF16_TC 2   /* wgmma bf16 operands, single MMA, fp32 accumulate (configs 3/4)                       */
 
 typedef struct gw_plan gw_plan; /* opaque */
 

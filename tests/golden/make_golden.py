@@ -1,6 +1,6 @@
 """Generates the golden fixtures in this directory by running the reference's OWN, UNMODIFIED source files
-(/root/reference, imported through oracle/ref_shims.py) on seeded weights and inputs.  Runs only in the build
-container (the GPU box has no /root/reference); the fixtures travel instead.
+(located by oracle/ref_shims.py, GW_REFERENCE_ROOT) on seeded weights and inputs.  Runs only where the reference sources
+are present; the fixtures travel with the repository instead.
 
     python tests/golden/make_golden.py
 
@@ -207,6 +207,24 @@ def run_regional(R, name="regional_europe_b2"):
           "mean|nudged - out|", float((out_n - out).abs().mean()))
 
 
+def run_init(R, name="reference_init_seed42"):
+    """The reference's default initialisation under torch.manual_seed(42) (30-degree grid): keys, shapes, a seeded sample of 16
+    values per tensor and the float64 sums of each tensor and of its magnitudes (tests/test_capi.py)."""
+    ll = grid(30)
+    torch.manual_seed(42)
+    ref = R.GraphWeatherForecaster(ll).state_dict()
+    rng = np.random.default_rng(0)
+    samples, sums = [], []
+    for v in ref.values():
+        v = v.detach().numpy().ravel().astype(np.float32)
+        idx = np.sort(rng.choice(v.size, min(v.size, 16), replace=False))
+        samples.append(np.pad(v[idx], (0, 16 - idx.size)))
+        sums.append([float(np.sum(v, dtype=np.float64)), float(np.sum(np.abs(v), dtype=np.float64))])
+    np.savez_compressed(os.path.join(HERE, name + ".npz"),
+                        config=json.dumps(dict(seed=42, grid_step=30, keys=list(ref.keys()), shapes=[list(v.shape) for v in ref.values()])),
+                        samples=np.array(samples, dtype=np.float32), sums=np.array(sums, dtype=np.float64))  # fmt: skip
+
+
 if __name__ == "__main__":
     torch.set_num_threads(os.cpu_count())
     R = ref_shims.load_reference()
@@ -224,3 +242,5 @@ if __name__ == "__main__":
         run_constraints(R)
     if not only or "regional" in only:
         run_regional(R)
+    if not only or "init" in only:
+        run_init(R)

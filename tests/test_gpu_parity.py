@@ -13,7 +13,7 @@ import __graft_entry__ as ge
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
-PRECISIONS = ["fp32_simt", "fp32"]  # exact-fp32 CUDA cores; tcgen05 fp16x2-split (fp32-faithful)
+PRECISIONS = ["fp32_simt", "fp32"]  # exact-fp32 CUDA cores; wgmma fp16x2-split (fp32-faithful)
 BF16_TOL = 2e-2  # bf16 operands carry 8 significand bits; through ~60 LayerNorm'd GEMM layers on O(1) outputs (measured 3e-3)
 
 
@@ -152,7 +152,7 @@ def test_full_size_properties_1deg(precision):
 
 
 def test_bf16_precision_against_oracle():
-    """precision="bf16" (BASELINE configs 3/4): one bf16 tcgen05 MMA per product, fp32 accumulation.  Its own tolerance:
+    """precision="bf16" (BASELINE configs 3/4): one bf16 wgmma per product, fp32 accumulation.  Its own tolerance:
     bf16 operands carry 8 significand bits, so through ~60 LayerNorm'd GEMM layers we accept 2e-2 max-abs (measured 2.7e-3) on O(1) outputs."""
     from graph_weather_b200 import GraphWeatherForecaster
     from oracle import restate, weights
@@ -225,14 +225,14 @@ def test_normalized_mse_loss_kernel(golden_dir):
 
 
 def test_default_constructor_runs_the_tensor_core_path(golden_dir):
-    """GraphWeatherForecaster(lat_lons)(features) with NO extra keyword (README.md:52,58) is the tcgen05 path on sm_100."""
+    """GraphWeatherForecaster(lat_lons)(features) with NO extra keyword (README.md:52,58) is the wgmma path on sm_90."""
     from graph_weather_b200 import GraphWeatherForecaster
 
     z, cfg, kw, ll, sd, x = _load_case(golden_dir, "forecaster_10deg_b2")
     model = GraphWeatherForecaster(ll).cuda().eval()
     model.load_state_dict(sd)
     out = model(x.cuda()).cpu().numpy()
-    if torch.cuda.get_device_capability(0)[0] == 10:
+    if torch.cuda.get_device_capability(0) == (9, 0):
         assert model._engine.resolved_precision == "fp32"
     assert np.abs(out - z["out"]).max() < TOL
     # sizes the chains are not built for fall to the exact CUDA-core path under the same default
@@ -273,7 +273,7 @@ def _quarter_deg():
 
 
 def test_quarter_degree_tensor_core_vs_exact_fp32():
-    """BASELINE configs[2] grid (0.25 degree ERA5, 1 038 240 points).  No CPU oracle fits (22 GB/sample), so the tcgen05 path is
+    """BASELINE configs[2] grid (0.25 degree ERA5, 1 038 240 points).  No CPU oracle fits (22 GB/sample), so the wgmma path is
     checked against the exact-fp32 CUDA-core path -- itself pinned to the reference fixtures and the oracle above -- on one
     sample (< 1e-4), and bf16 against the fp32-faithful path at its own tolerance."""
     from graph_weather_b200 import GraphWeatherForecaster
@@ -415,7 +415,7 @@ def test_assimilator_rebuilds_the_observation_graph(precision):
 @pytest.mark.parametrize("scale", [1.0e5, 3.0e-4])
 def test_raw_magnitude_inputs_are_range_scaled(scale):
     """Unnormalised inputs (geopotential ~ 1e5, pressure in Pa; the reference takes them as they are): the fp16-split operands
-    of the tcgen05 path are range-scaled from per-tensor magnitude bounds, so the result matches the oracle at 1e-4 RELATIVE to
+    of the wgmma path are range-scaled from per-tensor magnitude bounds, so the result matches the oracle at 1e-4 RELATIVE to
     the output magnitude and no status bit is raised."""
     from graph_weather_b200 import GraphWeatherForecaster
     from oracle import restate, weights

@@ -12,7 +12,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-BITS = {1: "fence", 2: "loads", 4: "convert", 8: "stores", 16: "ln", 32: "tmem", 64: "mma", 128: "weights"}
+BITS = {1: "fence", 2: "loads", 4: "convert", 8: "stores", 16: "ln", 128: "weights"}
 
 
 def build_abl(extra=()):
@@ -36,7 +36,7 @@ def name(mask):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--build-only", action="store_true")
-    ap.add_argument("--masks", default="0,1,2,4,8,16,32,64,128,255")
+    ap.add_argument("--masks", default="0,1,2,4,8,16,128,159")
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--precision", default="fp32")
     ap.add_argument("--iters", type=int, default=3)
