@@ -223,10 +223,13 @@ static int raw_bound(gw_plan* p, int slot, const float* x, long long n, cudaStre
   return 0;
 }
 
+// (the training step's phases, gw_train.inl: taped forward products, data gradients, weight gradients, per-step weight images and
+// operand bounds, and the memory-bound rest -- LayerNorm backward, segment sums, gathers, batch reductions)
 enum KernelTag { TAG_CONST = 0, TAG_ENC_GRID, TAG_ENC_MESH, TAG_PROC_P, TAG_PROC_EDGE, TAG_PROC_NODE, TAG_DEC_P, TAG_DEC_EDGE,
-                 TAG_DEC_NODE, TAG_COUNT };
+                 TAG_DEC_NODE, TAG_TRAIN_FWD, TAG_TRAIN_DGRAD, TAG_TRAIN_WGRAD, TAG_TRAIN_PACK, TAG_TRAIN_OTHER, TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"const", "enc_grid", "enc_mesh", "proc_p", "proc_edge", "proc_node", "dec_p",
-                                           "dec_edge", "dec_node"};
+                                           "dec_edge", "dec_node", "train_fwd", "train_dgrad", "train_wgrad", "train_pack",
+                                           "train_other"};
 
 static cudaEvent_t take_event(gw_plan* p) {
   if (p->ev_used == p->ev_pool.size()) {
@@ -1232,6 +1235,8 @@ int gw_plan_destroy(gw_plan* p) {
     gw::tfree_all(p->train);
     p->train->wT.release(), p->train->gbuf.release(), p->train->lat_perm_src.release(), p->train->lat_ptr_src.release();
     p->train->dec_perm_src.release(), p->train->dec_ptr_src.release(), p->train->iota.release(), p->train->sort_ws.release();
+    p->train->bslots.release(), p->train->wg_ws.release();
+    for (auto& kv : p->train->images) kv.second.img.release(), kv.second.amax.release();
     delete p->train;
     p->train = nullptr;
   }

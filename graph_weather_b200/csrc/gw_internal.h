@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <cmath>
+#include <cstring>
 #include <string>
 
 #include "gw_ops.h"
@@ -48,8 +50,33 @@ bool tc3_chain_is_lean(const TcChain& ch);  // would the launch take the lean (p
 // cp.async.bulk (perm32 feature order, gw_pack.cu); `parts` = 2 (fp16 hi, lo) or 1 (bf16).  dst must hold tc_packed_bytes(K_src, N_src, parts).
 size_t tc_packed_bytes(int K_src, int N_src, int parts);
 int tc_packed_rows(int N_src);  // rows of the packed image: N padded to 64
-cudaError_t launch_pack_weights(const float* W, int ldw, int K_src, int N_src, float wscale, int parts, void* dst, cudaStream_t stream);
+// amax_dev (optional): device max|W|; the scale is then tc_weight_scale(*amax_dev, parts), taken on the device (training images,
+// repacked every step without a host round trip) instead of `wscale`.
+cudaError_t launch_pack_weights(const float* W, int ldw, int K_src, int N_src, float wscale, int parts, void* dst, cudaStream_t stream,
+                                const float* amax_dev = nullptr);
 cudaError_t launch_absmax(const float* W, int ldw, int K_src, int N_src, float* out_max, cudaStream_t stream);
+// Power of two a weight image is stored times: fp16 hi|lo images (parts 2) bring max|W| into [2048, 4096) so the lo parts stay
+// normal (the host's pack_tc_weights uses the same rule); bf16 images are not scaled.
+__host__ __device__ inline float tc_weight_scale(float amax, int parts) {
+  if (parts != 2 || !(amax > 0.f) || !(amax < 3.0e38f)) return 1.f;
+  int e = 0;  // amax = f * 2^e, f in [0.5, 1)
+#ifdef __CUDA_ARCH__
+  e = (int)((__float_as_uint(amax) >> 23) & 0xffu) - 126;
+#else
+  uint32_t u;
+  memcpy(&u, &amax, 4);
+  e = (int)((u >> 23) & 0xffu) - 126;
+#endif
+  e = e < -100 ? -100 : e;  // (subnormal max: any scale that keeps the image finite)
+  return ldexpf(1.f, 12 - e);
+}
+
+// weight gradient on tensor cores (gw_wgrad_tc.cu): dW[o, k] += sum_r dY[r, o] A(r, k), db[o] += sum_r dY[r, o], in a fixed order
+// (per-CTA partials in `ws`, then one pass that sums them).  A: SRC_STREAM / SRC_BCAST.  split: fp16 hi/lo operands (3 MMAs per
+// product, power-of-two scaled from the operands' absmax), else bf16.  K, N <= 256.
+size_t wgrad_tc_workspace_floats(long long R, int N, int K);
+cudaError_t launch_wgrad_tc(const float* dY, int ldy, int N, const RowSrc& a, int K, int rows_per_sample, int batch, float* dW, int ldw, float* db,
+                            bool split, float* ws, size_t ws_floats, int32_t* status, cudaStream_t st);
 
 // device-side observation graph of the assimilator (gw_graph.cu)
 struct H3Tables {

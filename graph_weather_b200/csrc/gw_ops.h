@@ -97,6 +97,12 @@ struct TcLayer {
   const float* seg_add = nullptr;    // [seg_rows, seg_ld] or null: a per-target constant added to every complete sum (the sum of a
                                      // constant residual over the target's rows, hoisted out of the row loop: gw_api.cu S_dec)
   const float* seg_add_bound = nullptr;  // device float: magnitude bound of seg_add
+  // training step (gw_train.inl), general path only: the value entering LayerNorm is also stored to save_pre (same ldo / out_cols
+  // as out; GemmOp::save_pre), and the result is zeroed wherever mask(row, n) <= 0 (the ReLU's backward, applied last; GemmOp::mask)
+  float* save_pre = nullptr;
+  RowSrc mask;
+  const float* wamax = nullptr;  // device max|W| of an image packed with its scale taken on the device (launch_pack_weights with
+                                 // amax_dev): the kernel derives wscale_inv and gain from it instead of the host fields
 };
 
 struct TcChain {
@@ -109,6 +115,8 @@ struct TcChain {
   long long* trace = nullptr; // optional debug timeline: [8 roles][1024 events][2] = {clock64, code}; CTA 0 only
   int32_t fast = 0;           // gw_tc3: bit l = layer l takes the lean full-width path, bit 31 = stage 0 does (set by the launcher)
   int32_t ablate = 0;         // diagnostics build only (-DGW_ABLATE): bit mask of pipeline parts to skip, for timing attribution
+  int32_t range_fit = 0;      // 1: every fp16-split operand is scaled by a power of two into [2^14, 2^15), up as well as down (the
+                              // training step's gradients are ~1e-8: unscaled, their lo parts would be subnormal)
   // Loss-boundary gather fused into the chain that produces the forecast (multi-GPU; graph_weather_b200/dist.py): the LAST layer's
   // fp32 result rows are stored, tile by tile as they leave the accumulator, into the gather buffers of every GPU of the job --
   // out_mode 1: one multimem.st per value to the NVLink multicast alias of `out` (the switch replicates it to every GPU);

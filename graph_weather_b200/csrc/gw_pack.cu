@@ -1,4 +1,5 @@
-// gw_pack.cu -- one-off packing of nn.Linear weights into the operand images the tensor-core chain kernel (gw_tc3.cu) streams:
+// gw_pack.cu -- packing of nn.Linear weights (once per weight set; every step for the training step's W and W^T images, scale taken
+// on the device) into the operand images the tensor-core chain kernel (gw_tc3.cu) streams:
 // fp16 hi|lo (fp32-faithful mode) or bf16, K-major, SWIZZLE_128B, one contiguous panel per 64-wide K chunk, power-of-two
 // pre-scaled, output rows and K columns permuted inside every group of 32 (perm32) -- the feature order of the chain kernel's
 // wgmma accumulator fragments, see gw_tc3.cu.
@@ -26,7 +27,8 @@ size_t tc_packed_bytes(int K_src, int N_src, int parts) {
 // packed position a = 8g + 2c + e holds logical index 8c + 2g + e.
 __host__ __device__ inline int perm32_f(int a) { return (a & ~31) | (8 * ((a >> 1) & 3) + 2 * ((a >> 3) & 3) + (a & 1)); }
 __global__ void gw_pack_weights_kernel(const float* __restrict__ W, int ldw, int K_src, int N_src, int Kp, int Np,
-                                       float wscale, int parts, uint8_t* __restrict__ dst) {
+                                       float wscale, int parts, uint8_t* __restrict__ dst, const float* __restrict__ amax_dev) {
+  if (amax_dev) wscale = tc_weight_scale(*amax_dev, parts);
   const size_t total = (size_t)Np * Kp;
   for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
     const int n = (int)(e / Kp), k = (int)(e % Kp);
@@ -47,9 +49,9 @@ __global__ void gw_pack_weights_kernel(const float* __restrict__ W, int ldw, int
 }
 
 cudaError_t launch_pack_weights(const float* W, int ldw, int K_src, int N_src, float wscale, int parts, void* dst,
-                                cudaStream_t stream) {
+                                cudaStream_t stream, const float* amax_dev) {
   const int Kp = round_up(K_src, 64), Np = tc_packed_rows(N_src);
-  gw_pack_weights_kernel<<<256, 256, 0, stream>>>(W, ldw, K_src, N_src, Kp, Np, wscale, parts, static_cast<uint8_t*>(dst));
+  gw_pack_weights_kernel<<<256, 256, 0, stream>>>(W, ldw, K_src, N_src, Kp, Np, wscale, parts, static_cast<uint8_t*>(dst), amax_dev);
   count_launch();
   return cudaGetLastError();
 }

@@ -190,6 +190,13 @@ __device__ __forceinline__ float range_scale(float m) {
   const int e = (int)((__float_as_uint(m) >> 23) & 0xffu) - 127;  // floor(log2 m): m < 2^(e+1)
   return __uint_as_float((uint32_t)(127 + 14 - e) << 23);         // 2^(14-e)   (e <= 127 -> exponent field >= 14: normal)
 }
+// range_fit (training): the power of two that brings a tensor bounded by m into [2^14, 2^15), up as well as down
+__device__ __forceinline__ float fit_scale(float m) {
+  if (!(m > 0.f) || !(m < 3.0e38f)) return 1.f;
+  int e = (int)((__float_as_uint(m) >> 23) & 0xffu) - 127;  // floor(log2 m) (normals)
+  e = e < -110 ? -110 : e;
+  return __uint_as_float((uint32_t)(127 + 14 - e) << 23);   // 2^(14-e)
+}
 __device__ __forceinline__ float ldbound(const float* p) { return p ? __ldg(p) : 0.f; }
 __device__ __forceinline__ float srcbound(const RowSrc& s) {
   if (!s.bound) return 0.f;
@@ -280,13 +287,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
     float* scl = reinterpret_cast<float*>(smem + OFF_SCL);
     float m = fmaxf(srcbound(ch.a0[0]), srcbound(ch.a0[1]));
     if (ch.a0[0].kind == SRC_GATHER_BCAST_RELU) m += ldbound(ch.a0[0].bound2);
-    float sc = range_scale(m);
+    const bool fit = ch.range_fit != 0;
+    float sc = fit ? fit_scale(m) : range_scale(m);
     bool bad = !(m < 3.0e38f);
     scl[2 * PAR_LAYERS] = sc;
     for (int l = 0; l < ch.n_layers; ++l) {
       const TcLayer& L = ch.layer[l];
-      scl[2 * l] = L.wscale_inv / sc;  // (a reuse_a layer multiplies the same operand: m and sc are unchanged)
-      float mo = L.ln_g ? L.ln_bound : fmaf(m, L.gain, L.off) + srcbound(L.add[0]) + srcbound(L.add[1]);
+      // (an image scaled on the device carries its max|W|: its scale and gain follow from it)
+      const float wa = ldbound(L.wamax);
+      const float winv = L.wamax ? 1.f / tc_weight_scale(wa, ch.split ? 2 : 1) : L.wscale_inv, gain = L.wamax ? (float)L.K * wa : L.gain;
+      scl[2 * l] = winv / sc;  // (a reuse_a layer multiplies the same operand: m and sc are unchanged)
+      float mo = L.ln_g ? L.ln_bound : fmaf(m, gain, L.off) + srcbound(L.add[0]) + srcbound(L.add[1]);
       mo += srcbound(L.residual);
       bad = bad || !(mo < 3.0e38f);
       if (blockIdx.x == 0) {
@@ -299,7 +310,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
       float so = 1.f;
       if (L.feeds_next) {
         m = mo;
-        sc = so = range_scale(m);
+        sc = so = fit ? fit_scale(m) : range_scale(m);
       }
       scl[2 * l + 1] = so;
     }
@@ -754,6 +765,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
     const bool has_add0 = L.add[0].kind != SRC_NONE, has_add1 = L.add[1].kind != SRC_NONE;
     const bool has_res = L.residual.kind != SRC_NONE, has_out = L.out != nullptr;
     const bool relu = L.relu != 0, feeds = L.feeds_next != 0, has_ln = L.ln_g != nullptr;
+    const bool has_mask = L.mask.kind != SRC_NONE, has_pre = L.save_pre != nullptr;
     const uint32_t g_a = sbase + OFF_LNP + 4 * fcofs + (ln_slot * 2) * 1024, b_a = g_a + 1024;
     const int r2[2] = {min(fr0, nvalid - 1), min(fr0 + 1, nvalid - 1)};
     const float* q0[2] = {nullptr, nullptr};  // addend 0 / residual rows
@@ -764,6 +776,23 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
       if (has_add0 || has_res) q0[m] = src_row(src0, bs, i0, r2[m]);
       if (has_add1) q1[m] = src_row(L.add[1], bs, i0, r2[m]);
     }
+    // plain fp32 stores of my two rows' 8 features (out / save_pre): 128-bit where the row allows it
+    auto store8 = [&](float* base, const float (&v)[16], int col) GW_INLINE {
+#pragma unroll
+      for (int m = 0; m < 2; ++m) {
+        if (fr0 + m < nvalid) {
+          float* orow = base + ((size_t)bs * rows + i0 + fr0 + m) * (size_t)L.ldo + col;
+          if (col + 8 <= L.out_cols && (reinterpret_cast<uintptr_t>(orow) & 15) == 0) {
+            *reinterpret_cast<float4*>(orow) = make_float4(v[FR(m, 0)], v[FR(m, 1)], v[FR(m, 2)], v[FR(m, 3)]);
+            *reinterpret_cast<float4*>(orow + 4) = make_float4(v[FR(m, 4)], v[FR(m, 5)], v[FR(m, 6)], v[FR(m, 7)]);
+          } else {
+#pragma unroll
+            for (int k = 0; k < 8; ++k)
+              if (col + k < L.out_cols) orow[k] = v[FR(m, k)];
+          }
+        }
+      }
+    };
     bias_in_place(acc, l, nu, scl[2 * l]);
     float rs[2] = {1.f, 1.f}, sh[2] = {0.f, 0.f};
     if (has_ln && !ABL3(ABL_LN)) ln_stats(acc, nu, nval, rs, sh);
@@ -817,6 +846,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
 #pragma unroll
           for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.f);
         }
+        if (has_pre && !ABL3(ABL_STORES)) store8(L.save_pre, v, col);  // the value entering LayerNorm
         if (has_ln) {
           const float4 gl = lds128(g_a + 128 * u), gh = lds128(g_a + 128 * u + 16);
           const float4 el = lds128(b_a + 128 * u), eh = lds128(b_a + 128 * u + 16);
@@ -830,6 +860,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
           load8(q0[0], col, src0.width, t), load8(q0[1], col, src0.width, t + 8);
 #pragma unroll
           for (int i = 0; i < 16; ++i) v[i] += t[PX(i)];
+        }
+        if (has_mask) {  // the ReLU's backward: keep where the mask row (the taped activation) is positive
+          load8(src_row(L.mask, bs, i0, r2[0]), col, L.mask.width, t), load8(src_row(L.mask, bs, i0, r2[1]), col, L.mask.width, t + 8);
+#pragma unroll
+          for (int i = 0; i < 16; ++i) v[i] = t[PX(i)] > 0.f ? v[i] : 0.f;
         }
         if (nval < L.N) {  // padded output columns (e.g. 78 of 128) must stay exactly zero
 #pragma unroll
@@ -1012,6 +1047,10 @@ static void tc3_mark_lean(TcChain& ch) {
       ch.fast |= 1 << l;
       continue;
     }
+    if (L.save_pre || L.mask.kind != SRC_NONE) {  // (the training step's epilogue parts exist on the general path only)
+      ch.layer[l].kind = -1;
+      continue;
+    }
     bool ok = (L.N == 256 || L.N == 128) && L.n_valid == L.N;
     for (int a = 0; a < 2; ++a)
       if (L.add[a].kind != SRC_NONE) ok = ok && src_fast(L.add[a], L.N);
@@ -1084,6 +1123,8 @@ cudaError_t launch_chain_tc3(const TcChain& ch_in, cudaStream_t stream) {
         L.residual.kind != SRC_BGATHER)
       return cudaErrorInvalidValue;
     if (L.add[0].kind != SRC_NONE && L.residual.kind != SRC_NONE) return cudaErrorInvalidValue;  // they share the prefetch registers
+    if (L.mask.kind != SRC_NONE && L.mask.kind != SRC_STREAM && L.mask.kind != SRC_BCAST && L.mask.kind != SRC_GATHER && L.mask.kind != SRC_BGATHER)
+      return cudaErrorInvalidValue;
     if (l == 0 && L.K != ch.K0) return cudaErrorInvalidValue;
     if (l > 0 && !L.reuse_a && (!ch.layer[l - 1].feeds_next || ch.layer[l - 1].N != L.K)) return cudaErrorInvalidValue;
     if (L.reuse_a && (l == 0 || L.K != ch.layer[l - 1].K || ch.layer[l - 1].feeds_next || L.K > 64 * A_SLOTS)) return cudaErrorInvalidValue;  // the whole operand must still be resident

@@ -131,6 +131,22 @@ def _validate_precision(precision: str, dims: dict):
         )
 
 
+TRAIN_PRECISIONS = ("fp32_simt", "fp32", "bf16")
+
+
+def _validate_train_precision(train_precision: str, dims: dict):
+    """`train_precision` of GraphWeatherForecaster: the arithmetic of the training step (gw_train.inl).  'fp32_simt' exact fp32 on
+    CUDA cores; 'fp32' fp16 hi/lo split on tensor cores (3 MMAs per product, fp32 accumulation); 'bf16' bf16 tensor-core
+    operands (fp32 accumulation, fp32 master weights, gradients and tape)."""
+    if train_precision not in TRAIN_PRECISIONS:
+        raise ValueError(f"train_precision={train_precision!r}: expected one of {list(TRAIN_PRECISIONS)}")
+    if train_precision != "fp32_simt" and not _tc_eligible(dims):
+        raise ValueError(
+            f"train_precision={train_precision!r} runs the tensor-core chains, which are built for node/edge/hidden dims of 256 and 2 "
+            "hidden layers (the reference defaults); use train_precision='fp32_simt' for other sizes"
+        )
+
+
 def resolve_precision(precision: str, dims: dict, device) -> str:
     """'auto' (the default of every constructor): the fp32-faithful tensor-core (wgmma) path wherever it applies -- reference
     default sizes on an sm_90 device (H100) -- and the exact-fp32 CUDA-core path otherwise.  Explicit values are returned unchanged."""
@@ -572,6 +588,7 @@ class GraphWeatherForecasterConfig:
     use_checkpointing: bool = False
     constraint_type: str = "none"
     use_thermalizer: bool = False
+    train_precision: str = "fp32_simt"
 
     def build(self) -> "GraphWeatherForecaster":
         return GraphWeatherForecaster(**self.__dict__)
@@ -585,7 +602,7 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
                  hidden_dim_processor_edge: int = 256, hidden_layers_processor_node: int = 2, hidden_layers_processor_edge: int = 2,
                  hidden_dim_decoder: int = 128, hidden_layers_decoder: int = 2, norm_type: str = "LayerNorm",
                  use_checkpointing: bool = False, constraint_type: str = "none", use_thermalizer: bool = False,
-                 precision: str = "auto"):  # fmt: skip
+                 precision: str = "auto", train_precision: str = "fp32_simt"):  # fmt: skip
         super().__init__()
         if use_thermalizer:
             raise NotImplementedError("use_thermalizer=True is outside the accelerated path (stochastic layer)")
@@ -628,6 +645,8 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
                     num_blocks=num_blocks)  # fmt: skip
         self._engine = _Engine(dims, precision)
         self._engine.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
+        _validate_train_precision(train_precision, dims)
+        self.train_precision = train_precision
         if self.constraint_type != "none":  # forecast.py:162-170 (any other string fails at the first forward, as there)
             self.constraint = PhysicalConstraintLayer(model=self, grid_shape=self.grid_shape, constraint_type=constraint_type,
                                                       upsampling_factor=1)  # fmt: skip
@@ -660,9 +679,10 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
         return self.constraint.apply_rows(out, f, cell.to(torch.int32).contiguous(), self.feature_dim)
 
     def _training_engine(self):
-        """The exact-fp32 plan the training step runs on (created on first use; the inference engine stays as it is)."""
+        """The plan the training step runs on, of precision `train_precision` (created on first use; the inference engine stays
+        as it is).  A tensor-core training precision needs an sm_90 device: elsewhere the first training forward raises."""
         if getattr(self, "_train_engine", None) is None:
-            eng = _Engine(self._engine.dims, "fp32_simt")
+            eng = _Engine(self._engine.dims, self.train_precision)
             eng.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
             self.__dict__["_train_engine"] = eng
         return self._train_engine

@@ -122,11 +122,15 @@ int gw_forward(gw_plan* plan, const float* features, float* out, int32_t batch, 
 int gw_forward_strided(gw_plan* plan, const float* features, float* out, int32_t out_ld, int32_t batch, void* stream);
 
 /* Training step (SURVEY.md 8(f) row 2: "then backward"; every caller of the reference trains, train/run.py:508-543).
- * gw_train_forward is gw_forward on the exact-fp32 plan (precision GW_PREC_FP32_SIMT) that keeps the activations the backward
- * needs; gw_train_backward consumes them: grad_out [batch, n_out, out_dim] -> gradients of every parameter, copied into the
- * caller's tensors named like the parameters (`grads`: reference state_dict keys, device pointers, parameter shapes), and, if
- * grad_features is not NULL, the gradient of the input features [batch, n_in, in_dim].  One backward per forward.  LayerNorm MLPs,
- * dims <= 256.  Weight gradients are accumulated with float atomics (repeatable to ~1e-7 relative, not bit for bit). */
+ * gw_train_forward is gw_forward that keeps the activations the backward needs; gw_train_backward consumes them: grad_out
+ * [batch, n_out, out_dim] -> gradients of every parameter, copied into the caller's tensors named like the parameters (`grads`:
+ * reference state_dict keys, device pointers, parameter shapes), and, if grad_features is not NULL, the gradient of the input
+ * features [batch, n_in, in_dim].  One backward per forward.  LayerNorm MLPs, dims <= 256.  The plan's precision is the step's
+ * arithmetic: GW_PREC_FP32_SIMT exact fp32 on CUDA cores (weight gradients accumulated with float atomics: repeatable to ~1e-7
+ * relative, not bit for bit); GW_PREC_FP32_TC (fp16 hi/lo split, 3 MMAs per product) or GW_PREC_BF16_TC (bf16 operands) on wgmma
+ * tensor cores with fp32 accumulation, fp32 tape and fp32 gradients -- 256-wide dims and 2 hidden layers, sm_90a; their weight
+ * gradients of layers with more than 16 inputs are reduced in a fixed order (bit for bit repeatable).  Timing tags train_fwd,
+ * train_dgrad, train_wgrad, train_pack, train_other split a step (gw_timing_read). */
 int gw_train_forward(gw_plan* plan, const float* features, float* out, int32_t batch, void* stream);
 int gw_train_backward(gw_plan* plan, const float* grad_out, float* grad_features, const gw_param* grads, int32_t n, void* stream);
 

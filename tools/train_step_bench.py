@@ -1,8 +1,12 @@
-"""Times one training step (forward with tape + NormalizedMSELoss + backward + SGD update) of GraphWeatherForecaster on the
-exact-fp32 training path.    python tools/train_step_bench.py [--grid 1deg|10deg] [--batch B] [--steps K]"""
+"""Times one training step (forward with tape + NormalizedMSELoss + backward + SGD update) of GraphWeatherForecaster.
+    python tools/train_step_bench.py [--grid 1deg|10deg] [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16]
+Prints one JSON line: ms/step, samples/s, the device time of the step's phases (libgwb200 timing tags train_*; one extra timed
+step after the measured ones, since the per-launch events add a little host work), peak device memory, and the card name and
+power limit read in the same run."""
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 import torch
@@ -11,11 +15,26 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
+def card():
+    """Name and enforced power limit of cuda:0 (read-only query; None where nvidia-smi is unavailable)."""
+    info = {"name": torch.cuda.get_device_name(0), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", "0"], capture_output=True,
+                           text=True, timeout=30)  # fmt: skip
+        if r.returncode == 0 and r.stdout.strip():
+            name, pl = [v.strip() for v in r.stdout.strip().splitlines()[0].split(",")]
+            info["name"], info["power_limit_w"] = name, float(pl)
+    except (OSError, ValueError, subprocess.SubprocessError):
+        pass
+    return info
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--grid", default="1deg", choices=["1deg", "10deg"])
     ap.add_argument("--batch", type=int, default=2)
     ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--train-precision", default="fp32_simt", choices=["fp32_simt", "fp32", "bf16"])
     a = ap.parse_args()
     import __graft_entry__ as ge
 
@@ -25,7 +44,7 @@ def main():
     step = 1 if a.grid == "1deg" else 10
     ll = [(float(lat), float(lon)) for lat in range(-90, 90, step) for lon in range(0, 360, step)]
     torch.manual_seed(0)
-    model = GraphWeatherForecaster(ll).cuda().train()
+    model = GraphWeatherForecaster(ll, train_precision=a.train_precision).cuda().train()
     crit = NormalizedMSELoss([1.0] * 78, ll, normalize=True)
     opt = torch.optim.SGD(model.parameters(), lr=1e-3)
     x = torch.randn(a.batch, len(ll), 102, device="cuda")
@@ -50,9 +69,22 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / a.steps
+    peak = torch.cuda.max_memory_allocated()
     free, total = torch.cuda.mem_get_info()
-    print(json.dumps({"what": "training step (fwd + loss + bwd + SGD), exact fp32 CUDA cores", "grid": a.grid, "batch": a.batch, "ms_per_step": ms,
-                      "samples_per_s": a.batch / (ms * 1e-3), "losses": [float(v) for v in losses], "device_mem_used_gib": round((total - free) / 2**30, 1)}))
+    # per-phase device time of one more step (the plan's stream-ordered tape allocations are outside torch's allocator: the
+    # device-wide figure is reported too)
+    plan = model._train_engine.plan
+    plan.timing_enable(True)
+    one()
+    tags = plan.timing_read()
+    plan.timing_enable(False)
+    phases = {k: round(v[1], 3) for k, v in tags.items() if k.startswith("train_") or k == "const"}
+    plan.status()
+    print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "train_precision": a.train_precision, "grid": a.grid, "batch": a.batch,
+                      "ms_per_step": ms, "samples_per_s": a.batch / (ms * 1e-3), "phase_ms": phases,
+                      "phase_launches": {k: v[0] for k, v in tags.items() if k.startswith("train_")},
+                      "torch_peak_alloc_gib": round(peak / 2**30, 2), "device_mem_used_gib": round((total - free) / 2**30, 1),
+                      "card": card(), "losses": [float(v) for v in losses]}))  # fmt: skip
 
 
 if __name__ == "__main__":
