@@ -536,6 +536,13 @@ cudaError_t launch_transpose(const float* W, int rows, int cols, float* WT, cuda
   return cudaGetLastError();
 }
 
+// running max |x| for a magnitude bound: a NaN becomes +inf and stays (fmaxf would drop it and leave the bound finite)
+__device__ __forceinline__ float amax1(float m, float x) {
+  const float a = fabsf(x);
+  return a <= m ? m : (a == a ? a : __int_as_float(0x7f800000));
+}
+__device__ __forceinline__ float amax4(float m, float4 v) { return amax1(amax1(amax1(amax1(m, v.x), v.y), v.z), v.w); }
+
 // dst[r, 0:ld_dst] = [src[r, 0:width], 0 ...]: widens rows whose width / stride are not multiples of 64 floats (the 102
 // input features) so that the tensor-core chain can read them with aligned 128-bit loads.  The pass sees every input value,
 // so it also produces their absolute maximum (amax, may be null): the magnitude bound the chain's operand scaling starts from.
@@ -553,7 +560,7 @@ __global__ void __launch_bounds__(256) gw_pad_rows_kernel(const float* __restric
     v.y = (c + 1 < width) ? __ldg(s + 1) : 0.f;
     v.z = (c + 2 < width) ? __ldg(s + 2) : 0.f;
     v.w = (c + 3 < width) ? __ldg(s + 3) : 0.f;
-    m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
+    m = amax4(m, v);
     *reinterpret_cast<float4*>(dst + r * ld_dst + c) = v;
   }
   if (amax) {
@@ -577,12 +584,11 @@ __global__ void __launch_bounds__(256) gw_absmax_flat_kernel(const float* __rest
   const long long nv = (n - head) >> 2;
   const float4* pv = reinterpret_cast<const float4*>(p + head);
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < nv; e += (long long)gridDim.x * blockDim.x) {
-    const float4 v = __ldg(pv + e);
-    m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
+    m = amax4(m, __ldg(pv + e));
   }
   if (blockIdx.x == 0 && threadIdx.x < 8) {  // unaligned head and tail
-    for (long long e = threadIdx.x; e < head; e += 8) m = fmaxf(m, fabsf(p[e]));
-    for (long long e = head + 4 * nv + threadIdx.x; e < n; e += 8) m = fmaxf(m, fabsf(p[e]));
+    for (long long e = threadIdx.x; e < head; e += 8) m = amax1(m, p[e]);
+    for (long long e = head + 4 * nv + threadIdx.x; e < n; e += 8) m = amax1(m, p[e]);
   }
   if (!(m <= 3.0e38f)) m = __int_as_float(0x7f800000);
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));

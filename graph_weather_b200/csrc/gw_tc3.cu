@@ -1034,6 +1034,12 @@ static void tc3_mark_lean(TcChain& ch) {
   static const int kinds2[] = {F_RELU | F_FEEDS, F_RELU | F_OUT};
   for (int l = 0; l < ch.n_layers; ++l) {
     const TcLayer& L = ch.layer[l];
+    // the training step's epilogue parts (pre-LayerNorm store, ReLU mask) exist on the general path only: such a layer must not
+    // take the narrow output layer below either, whose epilogue reads neither field
+    if (L.save_pre || L.mask.kind != SRC_NONE) {
+      ch.layer[l].kind = -1;
+      continue;
+    }
     // the forecast's output layer: last layer, no activation / norm / addends, n_valid (even) real columns of an N32-row image,
     // output and residual rows 8-byte aligned and not gathered
     const bool narrow = l + 1 == ch.n_layers && L.n_valid < L.N32 && !(L.n_valid & 1) && (L.N32 == 128 || L.N32 == 256) && L.out && !L.relu &&
@@ -1045,10 +1051,6 @@ static void tc3_mark_lean(TcChain& ch) {
     if (narrow) {
       ch.layer[l].kind = F_NARROW | F_OUT | (L.residual.kind != SRC_NONE ? F_RES : 0);
       ch.fast |= 1 << l;
-      continue;
-    }
-    if (L.save_pre || L.mask.kind != SRC_NONE) {  // (the training step's epilogue parts exist on the general path only)
-      ch.layer[l].kind = -1;
       continue;
     }
     bool ok = (L.N == 256 || L.N == 128) && L.n_valid == L.N;
