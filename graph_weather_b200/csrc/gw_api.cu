@@ -515,12 +515,7 @@ static int pack_tc_weights(gw_plan* p, cudaStream_t st) {
   if (p->tc_packed.n != total) GW_TRY(p->tc_packed.alloc(total));
   size_t off = 0;
   for (size_t i = 0; i < n; ++i) {
-    float scale = 1.f;
-    if (parts == 2 && amax[i] > 0.f && std::isfinite(amax[i])) {
-      int e = 0;
-      std::frexp(amax[i], &e);           // amax = f * 2^e, f in [0.5, 1)
-      scale = std::ldexp(1.f, 12 - e);   // amax * scale in [2048, 4096)
-    }
+    const float scale = tc_weight_scale(amax[i], parts);
     void* dst = p->tc_packed.p + off;
     const size_t img = (tc_packed_bytes(reqs[i].K, reqs[i].N, parts) + 1023) / 1024 * 1024;
     GW_CUDA(launch_pack_weights(reqs[i].W, reqs[i].ldw, reqs[i].K, reqs[i].N, scale, parts, dst, st));

@@ -33,8 +33,8 @@
 //   * warp 8: weight producer (cp.async.bulk of pre-swizzled panels of up to 32 KB, two stages).  setmaxnreg gives the
 //     consumers 240 registers and the producer warpgroup 24.
 //   * operand range: every tensor carries a rigorous magnitude bound (device float); each CTA derives, per layer, the power
-//     of two that brings the next fp16-split operand under 2^15 and folds its inverse into the accumulator scale, so raw
-//     (unnormalised) inputs cannot overflow fp16.  The amax status bit stays as a guard.
+//     of two that brings the next fp16-split operand into [2^14, 2^15) and folds its inverse into the accumulator scale, so raw
+//     (unnormalised) inputs cannot overflow fp16 and small ones keep normal lo parts.  The amax status bit stays as a guard.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -184,13 +184,9 @@ __device__ __forceinline__ void store_operand_x4(uint32_t sa, const float (&v)[1
 }
 
 // ---- operand range --------------------------------------------------------------------------------------------------
-// Power of two s such that a tensor bounded by m has |s x| < 2^15 (fp16 max is 65504); 1 when m is already in range.
-__device__ __forceinline__ float range_scale(float m) {
-  if (!(m > 32768.f)) return 1.f;
-  const int e = (int)((__float_as_uint(m) >> 23) & 0xffu) - 127;  // floor(log2 m): m < 2^(e+1)
-  return __uint_as_float((uint32_t)(127 + 14 - e) << 23);         // 2^(14-e)   (e <= 127 -> exponent field >= 14: normal)
-}
-// range_fit (training): the power of two that brings a tensor bounded by m into [2^14, 2^15), up as well as down
+// The power of two s that brings a tensor bounded by m into [2^14, 2^15), up as well as down: large tensors stay under the fp16
+// maximum (65504), and small ones (gradients ~1e-8, inputs in small physical units) keep normal fp16 lo parts.  The bound is
+// rigorous, so scaling up cannot overflow.  1 when the bound is unknown (0) or not finite.
 __device__ __forceinline__ float fit_scale(float m) {
   if (!(m > 0.f) || !(m < 3.0e38f)) return 1.f;
   int e = (int)((__float_as_uint(m) >> 23) & 0xffu) - 127;  // floor(log2 m) (normals)
@@ -287,8 +283,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
     float* scl = reinterpret_cast<float*>(smem + OFF_SCL);
     float m = fmaxf(srcbound(ch.a0[0]), srcbound(ch.a0[1]));
     if (ch.a0[0].kind == SRC_GATHER_BCAST_RELU) m += ldbound(ch.a0[0].bound2);
-    const bool fit = ch.range_fit != 0;
-    float sc = fit ? fit_scale(m) : range_scale(m);
+    float sc = fit_scale(m);
     bool bad = !(m < 3.0e38f);
     scl[2 * PAR_LAYERS] = sc;
     for (int l = 0; l < ch.n_layers; ++l) {
@@ -310,7 +305,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
       float so = 1.f;
       if (L.feeds_next) {
         m = mo;
-        sc = so = fit ? fit_scale(m) : range_scale(m);
+        sc = so = fit_scale(m);
       }
       scl[2 * l + 1] = so;
     }

@@ -17,11 +17,14 @@ using namespace gw;
 
 extern "C" {
 
-struct HSrc {  // one row source: kind = gw::SrcKind (0 none, 1 stream, 2 bcast, 3 gather, 6 bgather)
+struct HSrc {  // one row source: kind = gw::SrcKind (0 none, 1 stream, 2 bcast, 3 gather, 5 relu(gather + bcast), 6 bgather)
   int32_t kind, width, ld, col0;
   const float* base;
   int32_t src_rows;
   const int32_t* idx;
+  const float* base2;  // kind 5: the broadcast table (ld2)
+  int32_t ld2;
+  const int32_t* bound_mul_i;  // h_chain: the source's bound is multiplied by this device integer (a sum of up to that many rows)
 };
 
 struct HOp {  // one training row op: out = mask(residual + LN(relu(concat(a) . W^T + bias + add)))
@@ -41,6 +44,33 @@ struct HOp {  // one training row op: out = mask(residual + LN(relu(concat(a) . 
   HSrc mask;
 };
 
+struct HLayer {  // one forward chain layer: out = residual + LN(relu(A . W^T + bias + add)), fp32 W [N, ldw] with K real inputs
+  const float* W;
+  int32_t K, N, ldw;
+  const float* bias;
+  HSrc add[2];
+  int32_t relu;
+  const float* ln_g;
+  const float* ln_b;
+  HSrc residual;
+  float* out;
+  int32_t ldo, out_cols, feeds_next, reuse_a;
+  const int32_t* seg_dst;  // fused per-target sums (gw::TcLayer::seg_*)
+  float* seg_out;
+  int32_t seg_ld, seg_rows, seg_maxdeg;
+  const float* seg_add;    // [seg_rows, seg_ld]
+  float* out_bound;        // device floats the chain sets (may be null)
+  float* seg_bound;
+};
+
+struct HChain {  // one inference chain as gw_api.cu builds it
+  int32_t rows, batch, K0, n_layers;
+  HSrc a0[2];
+  HLayer layer[6];
+  int32_t out_mode, n_out_peers;  // out_mode 2: the last layer stores through out_peer[j] instead of its own out
+  float* out_peer[3];
+};
+
 }  // extern "C"
 
 namespace {
@@ -48,6 +78,7 @@ namespace {
 RowSrc row_src(const HSrc& h) {
   RowSrc s;
   s.kind = h.kind, s.width = h.width, s.ld = h.ld, s.col0 = h.col0, s.base = h.base, s.src_rows = h.src_rows, s.idx = h.idx;
+  s.base2 = h.base2, s.ld2 = h.ld2;
   return s;
 }
 
@@ -82,6 +113,8 @@ extern "C" {
 
 int h_sizeof_src() { return (int)sizeof(HSrc); }
 int h_sizeof_op() { return (int)sizeof(HOp); }
+int h_sizeof_layer() { return (int)sizeof(HLayer); }
+int h_sizeof_chain() { return (int)sizeof(HChain); }
 
 // dW[o, k] (ld ldw) += sum_r dY[r, o] A(r, k), db[o] += sum_r dY[r, o] (db may be null), on tensor cores; workspace sized here
 int h_wgrad_tc(int split, const float* dY, int ldy, int N, const HSrc* a, int K, int rows, int batch, float* dW, int ldw, float* db, int32_t* status,
@@ -101,7 +134,7 @@ int h_wgrad_simt(const float* dY, int ldy, int N, const HSrc* a, int K, int rows
 
 // One training row op.  precision 0: fp32_simt (gw_simt.cu); 1: fp32 (fp16 hi/lo, 3 MMAs); 2: bf16.  The tensor-core precisions
 // build the one-layer chain the training step builds (gw_train.inl, train_op): weight image packed with its scale taken on the
-// device, stage-0 sources bounded by their whole tensor's absmax (fp32), K0 rounded to 64, range_fit.  *lean: whether the chain
+// device, stage-0 sources bounded by their whole tensor's absmax (fp32), K0 rounded to 64.  *lean: whether the chain
 // takes the lean path (-1 for fp32_simt).
 int h_row_op(int precision, const HOp* h, int* lean, int32_t* status, void* stream) {
   const cudaStream_t st = (cudaStream_t)stream;
@@ -131,7 +164,7 @@ int h_row_op(int precision, const HOp* h, int* lean, int32_t* status, void* stre
   TcChain ch;
   ch.rows_per_sample = op.rows_per_sample, ch.batch = op.batch;
   ch.a0[0] = op.a[0], ch.a0[1] = op.a[1];
-  ch.K0 = (op.K + 63) / 64 * 64, ch.n_layers = 1, ch.range_fit = 1, ch.split = split ? 1 : 0, ch.status = status;
+  ch.K0 = (op.K + 63) / 64 * 64, ch.n_layers = 1, ch.split = split ? 1 : 0, ch.status = status;
   if (split)
     for (int a = 0; a < 2; ++a) {
       RowSrc& s = ch.a0[a];
@@ -148,6 +181,97 @@ int h_row_op(int precision, const HOp* h, int* lean, int32_t* status, void* stre
   L.out = op.out, L.ldo = op.ldo, L.out_cols = op.N, L.save_pre = op.save_pre, L.mask = op.mask;
   if (lean) *lean = tc3_chain_is_lean(ch) ? 1 : 0;
   return (int)launch_chain_tc3(ch, st);
+}
+
+// One inference chain (precision 1: fp32, 2: bf16), prepared as gw_api.cu prepares it: every weight image packed with the host's
+// power-of-two scale (tc_weight_scale of its device absmax), gain = K max|W|, off = max|bias|, ln_bound = sqrt(N) max|gamma| +
+// max|beta|, and every source bounded by the absmax of its whole table (launch_absmax_flat).  A layer with fused per-target sums
+// gets a carry buffer (prefilled with NaN: a carry row read before it is written poisons the sum), and gw_seg_carry_kernel runs
+// after the chain, as in stage_processor / stage_decoder.  *lean: tc3_chain_is_lean.
+int h_chain(int precision, const HChain* h, int* lean, int32_t* status, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (lean) *lean = -1;
+  if ((precision != 1 && precision != 2) || h->n_layers < 1 || h->n_layers > 6 || h->n_out_peers < 0 || h->n_out_peers > 3)
+    return (int)cudaErrorInvalidValue;
+  const bool split = precision == 1;
+  const int parts = split ? 2 : 1, nl = h->n_layers;
+  Temps t(st);
+  // device maxima: per layer {W, bias, gamma, beta}, then one slot per source
+  constexpr int NSLOT = 64;
+  float* mx = nullptr;
+  H_TRY(t.get(&mx, NSLOT));
+  H_TRY(cudaMemsetAsync(mx, 0, NSLOT * sizeof(float), st));
+  int next = 24;
+  auto vmax = [&](const float* v, int n, float* slot) { return v ? launch_absmax(v, n, n, 1, slot, st) : cudaSuccess; };
+  auto bounded = [&](const HSrc& hs, RowSrc& s) -> cudaError_t {
+    s = row_src(hs);
+    if (s.kind == SRC_NONE) return cudaSuccess;
+    const bool per_sample = s.kind == SRC_STREAM || s.kind == SRC_GATHER || s.kind == SRC_GATHER_BCAST_RELU;
+    const long long table_rows = per_sample ? (long long)h->batch * s.src_rows : (s.kind == SRC_BGATHER ? s.src_rows : h->rows);
+    s.bound = mx + next++, s.bound_mul = 1.f, s.bound_mul_i = hs.bound_mul_i;
+    cudaError_t e = launch_absmax_flat(s.base, table_rows * s.ld, mx + next - 1, st);
+    if (e == cudaSuccess && s.kind == SRC_GATHER_BCAST_RELU) {
+      s.bound2 = mx + next++;
+      e = launch_absmax_flat(s.base2, (long long)h->rows * s.ld2, mx + next - 1, st);
+    }
+    return e;
+  };
+  TcChain ch;
+  ch.rows_per_sample = h->rows, ch.batch = h->batch, ch.K0 = h->K0, ch.n_layers = nl, ch.split = split ? 1 : 0, ch.status = status;
+  for (int a = 0; a < 2; ++a) H_TRY(bounded(h->a0[a], ch.a0[a]));
+  int seg_layer = -1;
+  for (int l = 0; l < nl; ++l) {
+    const HLayer& H = h->layer[l];
+    TcLayer& L = ch.layer[l];
+    H_TRY(launch_absmax(H.W, H.ldw, H.K, H.N, mx + 4 * l, st));
+    H_TRY(vmax(H.bias, H.N, mx + 4 * l + 1));
+    H_TRY(vmax(H.ln_g, H.N, mx + 4 * l + 2));
+    H_TRY(vmax(H.ln_b, H.N, mx + 4 * l + 3));
+    for (int a = 0; a < 2; ++a) H_TRY(bounded(H.add[a], L.add[a]));
+    H_TRY(bounded(H.residual, L.residual));
+    if (H.seg_add) {
+      L.seg_add_bound = mx + next++;
+      H_TRY(launch_absmax_flat(H.seg_add, (long long)H.seg_rows * H.seg_ld, mx + next - 1, st));
+    }
+    if (H.seg_dst) seg_layer = l;
+  }
+  if (next > NSLOT) return (int)cudaErrorInvalidValue;
+  float hm[24];
+  H_TRY(cudaMemcpyAsync(hm, mx, sizeof(hm), cudaMemcpyDeviceToHost, st));
+  H_TRY(cudaStreamSynchronize(st));
+  for (int l = 0; l < nl; ++l) {
+    const HLayer& H = h->layer[l];
+    TcLayer& L = ch.layer[l];
+    unsigned char* img = nullptr;
+    H_TRY(t.get(&img, tc_packed_bytes(H.K, H.N, parts)));
+    const float scale = tc_weight_scale(hm[4 * l], parts);
+    H_TRY(launch_pack_weights(H.W, H.ldw, H.K, H.N, scale, parts, img, st));
+    L.Wp = img, L.K = (H.K + 63) / 64 * 64, L.N = (H.N + 15) / 16 * 16, L.N32 = tc_packed_rows(H.N), L.n_valid = H.N;
+    L.wscale_inv = 1.f / scale, L.gain = (float)H.K * hm[4 * l], L.off = hm[4 * l + 1];
+    L.bias = H.bias, L.relu = H.relu, L.ln_g = H.ln_g, L.ln_b = H.ln_b;
+    if (H.ln_g) L.ln_bound = sqrtf((float)H.N) * hm[4 * l + 2] + hm[4 * l + 3];
+    L.out = H.out, L.ldo = H.ldo, L.out_cols = H.out_cols, L.out_bound = H.out_bound;
+    L.feeds_next = H.feeds_next, L.reuse_a = H.reuse_a;
+    L.seg_dst = H.seg_dst, L.seg_out = H.seg_out, L.seg_ld = H.seg_ld, L.seg_rows = H.seg_rows, L.seg_maxdeg = (float)H.seg_maxdeg;
+    L.seg_add = H.seg_add, L.seg_bound = H.seg_bound;
+  }
+  ch.out_mode = h->out_mode, ch.n_out_peers = h->n_out_peers;
+  for (int j = 0; j < h->n_out_peers; ++j) ch.out_peer[j] = h->out_peer[j];
+  float* carry = nullptr;
+  const int tiles = (h->rows + 127) / 128;
+  if (seg_layer >= 0) {
+    const size_t n = (size_t)h->batch * tiles * 8 * 256;
+    H_TRY(t.get(&carry, n));
+    H_TRY(cudaMemsetAsync(carry, 0xff, n * sizeof(float), st));
+    ch.layer[seg_layer].seg_carry = carry;
+  }
+  if (lean) *lean = tc3_chain_is_lean(ch) ? 1 : 0;
+  H_TRY(launch_chain_tc3(ch, st));
+  if (seg_layer >= 0) {
+    const HLayer& H = h->layer[seg_layer];
+    H_TRY(launch_seg_carry(carry, H.seg_dst, h->rows, H.seg_rows, h->batch, H.seg_out, H.seg_ld, st));
+  }
+  return 0;
 }
 
 int h_ln_bwd(const float* dy, int ld_dy, const float* z, int ld_z, int N, const float* gamma, long long R, float* dz, int ld_dz, float* dgamma,

@@ -49,7 +49,8 @@ WGRAD_LONG_EPS_F = 6e-5
 # ---- the harness ------------------------------------------------------------------------------------------------------------
 class HSrc(ctypes.Structure):
     _fields_ = [("kind", ctypes.c_int32), ("width", ctypes.c_int32), ("ld", ctypes.c_int32), ("col0", ctypes.c_int32),
-                ("base", ctypes.c_void_p), ("src_rows", ctypes.c_int32), ("idx", ctypes.c_void_p)]
+                ("base", ctypes.c_void_p), ("src_rows", ctypes.c_int32), ("idx", ctypes.c_void_p), ("base2", ctypes.c_void_p),
+                ("ld2", ctypes.c_int32), ("bound_mul_i", ctypes.c_void_p)]
 
 
 class HOp(ctypes.Structure):
@@ -59,10 +60,27 @@ class HOp(ctypes.Structure):
                 ("save_pre", ctypes.c_void_p), ("mask", HSrc)]
 
 
+class HLayer(ctypes.Structure):  # one forward chain layer (tests/test_gpu_chains.py)
+    _fields_ = [("W", ctypes.c_void_p), ("K", ctypes.c_int32), ("N", ctypes.c_int32), ("ldw", ctypes.c_int32), ("bias", ctypes.c_void_p),
+                ("add", HSrc * 2), ("relu", ctypes.c_int32), ("ln_g", ctypes.c_void_p), ("ln_b", ctypes.c_void_p), ("residual", HSrc),
+                ("out", ctypes.c_void_p), ("ldo", ctypes.c_int32), ("out_cols", ctypes.c_int32), ("feeds_next", ctypes.c_int32),
+                ("reuse_a", ctypes.c_int32), ("seg_dst", ctypes.c_void_p), ("seg_out", ctypes.c_void_p), ("seg_ld", ctypes.c_int32),
+                ("seg_rows", ctypes.c_int32), ("seg_maxdeg", ctypes.c_int32), ("seg_add", ctypes.c_void_p), ("out_bound", ctypes.c_void_p),
+                ("seg_bound", ctypes.c_void_p)]
+
+
+class HChain(ctypes.Structure):
+    _fields_ = [("rows", ctypes.c_int32), ("batch", ctypes.c_int32), ("K0", ctypes.c_int32), ("n_layers", ctypes.c_int32), ("a0", HSrc * 2),
+                ("layer", HLayer * 6), ("out_mode", ctypes.c_int32), ("n_out_peers", ctypes.c_int32), ("out_peer", ctypes.c_void_p * 3)]
+
+
 _vp, _i32, _i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong
 _SIGNATURES = {
     "h_sizeof_src": [],
     "h_sizeof_op": [],
+    "h_sizeof_layer": [],
+    "h_sizeof_chain": [],
+    "h_chain": [_i32, ctypes.POINTER(HChain), ctypes.POINTER(ctypes.c_int), _vp, _vp],
     "h_wgrad_tc": [_i32, _vp, _i32, _i32, ctypes.POINTER(HSrc), _i32, _i32, _i32, _vp, _i32, _vp, _vp, _vp],
     "h_wgrad_simt": [_vp, _i32, _i32, ctypes.POINTER(HSrc), _i32, _i32, _i32, _vp, _i32, _vp, _vp],
     "h_row_op": [_i32, ctypes.POINTER(HOp), ctypes.POINTER(ctypes.c_int), _vp, _vp],
@@ -95,6 +113,8 @@ def test_harness_builds_and_links(tmp_path):
     lib = _compile_harness(tmp_path)
     assert lib.h_sizeof_src() == ctypes.sizeof(HSrc)
     assert lib.h_sizeof_op() == ctypes.sizeof(HOp)
+    assert lib.h_sizeof_layer() == ctypes.sizeof(HLayer)
+    assert lib.h_sizeof_chain() == ctypes.sizeof(HChain)
 
 
 HK = None  # the harness library of the GPU tests (fixture `hk`)

@@ -412,18 +412,19 @@ def test_assimilator_rebuilds_the_observation_graph(precision):
         assert float((out - ref).abs().max()) < TOL, trial
 
 
-@pytest.mark.parametrize("scale", [1.0e5, 3.0e-4])
-def test_raw_magnitude_inputs_are_range_scaled(scale):
+@pytest.mark.parametrize("scale,cols", [(1.0e5, (5, 40)), (3.0e-4, (5, 40)), (1.0e-5, (0, 102))], ids=["100000.0", "0.0003", "whole1e-05"])
+def test_raw_magnitude_inputs_are_range_scaled(scale, cols):
     """Unnormalised inputs (geopotential ~ 1e5, pressure in Pa; the reference takes them as they are): the fp16-split operands
     of the wgmma path are range-scaled from per-tensor magnitude bounds, so the result matches the oracle at 1e-4 RELATIVE to
-    the output magnitude and no status bit is raised."""
+    the output magnitude and no status bit is raised.  whole1e-05: every feature is small (inputs in kg/kg or metres of
+    precipitation), so the operands must be scaled UP for their fp16 lo parts to stay normal."""
     from graph_weather_b200 import GraphWeatherForecaster
     from oracle import restate, weights
 
     ll = _grid(10)
     sd = weights.make_state_dict(weights.forecaster_shapes(), 15)
     x = weights.make_features(2, len(ll), 102, 15)
-    x[..., 5:40] *= scale  # a block of raw-magnitude channels beside O(1) ones (some of them among the 78 residual features)
+    x[..., cols[0]:cols[1]] *= scale  # a block of raw-magnitude channels beside O(1) ones (some of them among the 78 residual features)
     model = GraphWeatherForecaster(ll).cuda().eval()
     model.load_state_dict(sd)
     out = model(x.cuda()).cpu()
@@ -436,6 +437,8 @@ def test_raw_magnitude_inputs_are_range_scaled(scale):
           f"on O(1) channels {float((out - ref)[..., 40:].abs().max()):.3e}")
     assert float(excess.max()) <= 0.0
     assert float((out - ref)[..., 40:].abs().max()) < 1e-4  # channels whose inputs are O(1): plain 1e-4
+    if cols == (0, 102):  # every input small: every output is O(1) or smaller, plain 1e-4 everywhere
+        assert float((out - ref).abs().max()) < TOL
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
