@@ -27,6 +27,7 @@ cudaError_t launch_wgrad(const float* dY, int ldy, int N, const RowSrc& a, int K
                          cudaStream_t st);
 cudaError_t launch_ln_bwd(const float* dy, int ld_dy, const float* z, int ld_z, int N, const float* gamma, long long R, float* dz, int ld_dz,
                           float* dgamma, float* dbeta, cudaStream_t st);
+constexpr int LN_BWD_MAX_N = 1024;  // widest row launch_ln_bwd takes (rows of more than 256 columns run on a kernel of their own)
 cudaError_t launch_batch_reduce(const float* in, int ld_in, long long rows, int width, int batch, float* out, int ld_out, bool accumulate,
                                 cudaStream_t st);
 cudaError_t launch_gather_rows(const float* in, int ld_in, int src_rows, const int32_t* idx, long long rows, int width, int batch, float* out,
@@ -46,6 +47,13 @@ cudaError_t launch_segsum(const float* base, int ld, int width, const int32_t* p
 // wgmma chain kernel (gw_tc3.cu)
 cudaError_t launch_chain_tc3(const TcChain& ch, cudaStream_t stream);
 bool tc3_chain_is_lean(const TcChain& ch);  // would the launch take the lean (perm32, 256-bit access) path?
+// A one-layer chain computes at most TC_COL_BLOCK output columns.  Wider training row ops (the encoder's data gradient into the
+// features, the decoder's output layer) run as column blocks: tc_column_block turns the layer of `ch`, which describes all its
+// outputs, into the chain of columns n0 .. n0 + nb - 1 (bias, addends, residual, mask, pre-LayerNorm store and output shifted
+// by n0 columns; stage-0 sources and their bounds shared).  The caller sets the block's weight image (W rows n0 .. n0 + nb - 1).
+// A layer with a LayerNorm cannot be split: cudaErrorInvalidValue.
+constexpr int TC_COL_BLOCK = 256;
+cudaError_t tc_column_block(const TcChain& ch, int n0, int nb, TcChain* out);
 // Packs W[n, k] (n < N_src rows of stride ldw, k < K_src) into the GMMA operand image the chain kernel streams with
 // cp.async.bulk (perm32 feature order, gw_pack.cu); `parts` = 2 (fp16 hi, lo) or 1 (bf16).  dst must hold tc_packed_bytes(K_src, N_src, parts).
 size_t tc_packed_bytes(int K_src, int N_src, int parts);
@@ -73,7 +81,8 @@ __host__ __device__ inline float tc_weight_scale(float amax, int parts) {
 
 // weight gradient on tensor cores (gw_wgrad_tc.cu): dW[o, k] += sum_r dY[r, o] A(r, k), db[o] += sum_r dY[r, o], in a fixed order
 // (per-CTA partials in `ws`, then one pass that sums them).  A: SRC_STREAM / SRC_BCAST.  split: fp16 hi/lo operands (3 MMAs per
-// product, power-of-two scaled from the operands' absmax), else bf16.  K, N <= 256.
+// product, power-of-two scaled from the operands' absmax), else bf16.  Any N (128-row output blocks); K > 256 runs as blocks of
+// 256 columns of A, one after the other through the same workspace.
 size_t wgrad_tc_workspace_floats(long long R, int N, int K);
 cudaError_t launch_wgrad_tc(const float* dY, int ldy, int N, const RowSrc& a, int K, int rows_per_sample, int batch, float* dW, int ldw, float* db,
                             bool split, float* ws, size_t ws_floats, int32_t* status, cudaStream_t st);

@@ -310,7 +310,8 @@ cudaError_t launch_segsum_chunked(const float* base, int ld, const int32_t* ptr,
 
 // ---- backward primitives (exact fp32; gw_train.inl) -------------------------------------------------------------------------
 // dW[n, k] += sum_r dY[r, n] * A[r, k]   (and db[n] += sum_r dY[r, n]) over R = rows_per_sample * batch rows, A assembled from a row
-// source like the forward kernel does.  Tile: all N <= 256 output rows x 32 k-columns per CTA column (blockIdx.y), the rows are
+// source like the forward kernel does (N > 256: one launch per block of 256 outputs).  Tile: all N <= 256 output rows x 32
+// k-columns per CTA column (blockIdx.y), the rows are
 // cut into gridDim.x slabs; every CTA accumulates its slab in registers (8 n x 4 k per thread) and adds it to dW with float
 // atomics (summation order across slabs is not fixed: gradients repeat to ~1e-7 relative, not bit for bit).
 constexpr int WG_KT = 32, WG_RT = 16;
@@ -379,10 +380,12 @@ cudaError_t launch_wgrad(const float* dY, int ldy, int N, const RowSrc& a, int K
                          cudaStream_t st) {
   const long long R = (long long)rows_per_sample * batch;
   if (R <= 0 || N <= 0 || K <= 0) return cudaSuccess;
-  if (N > 256) return cudaErrorInvalidValue;
   const int slabs = (int)std::min<long long>(296, (R + 255) / 256);
-  gw_wgrad_kernel<<<dim3(slabs, (K + WG_KT - 1) / WG_KT), 256, 0, st>>>(dY, ldy, N, a, K, rows_per_sample, batch, dW, ldw, db);
-  count_launch();
+  for (int o0 = 0; o0 < N; o0 += 256) {  // output blocks of 256 (the Ys tile), each a launch over all rows
+    gw_wgrad_kernel<<<dim3(slabs, (K + WG_KT - 1) / WG_KT), 256, 0, st>>>(dY + o0, ldy, std::min(256, N - o0), a, K, rows_per_sample, batch,
+                                                                           dW + (size_t)o0 * ldw, ldw, db ? db + o0 : nullptr);
+    count_launch();
+  }
   return cudaGetLastError();
 }
 
@@ -448,11 +451,92 @@ __global__ void __launch_bounds__(256) gw_ln_bwd_kernel(const float* __restrict_
     atomicAdd(dgamma + c, g), atomicAdd(dbeta + c, b);
   }
 }
+// The same for rows of 256 < N <= 32 J columns (LN_BWD_MAX_N = 1024: the 1024-wide models of train/run.py:491-501): one warp per
+// row with J values per lane (column lane + 32 j).  The per-CTA dgamma / dbeta partials of the 8 warps meet in one [8][1024]
+// shared array, dgamma first, then dbeta (two [8][1024] arrays would not fit in 48 KB of static shared memory).
+template <int J>
+__global__ void __launch_bounds__(256) gw_ln_bwd_wide_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z, int N,
+                                                             const float* __restrict__ gamma, long long R, float* __restrict__ dz, int ld_dz,
+                                                             float* __restrict__ dgamma, float* __restrict__ dbeta) {
+  __shared__ float sp[8][LN_BWD_MAX_N];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  float ag[J], ab[J];
+#pragma unroll
+  for (int j = 0; j < J; ++j) ag[j] = ab[j] = 0.f;
+  for (long long r = (long long)blockIdx.x * 8 + w; r < R; r += (long long)gridDim.x * 8) {
+    float zv[J], dv[J];
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const int c = lane + 32 * j;
+      zv[j] = c < N ? __ldg(z + r * ld_z + c) : 0.f;
+      dv[j] = c < N ? __ldg(dy + r * ld_dy + c) : 0.f;
+      s += zv[j];
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    const float mean = s / (float)N;
+    float q = 0.f;
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const float d = (lane + 32 * j < N) ? zv[j] - mean : 0.f;
+      q += d * d;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+    const float rstd = 1.0f / sqrtf(q / (float)N + 1e-5f);
+    float m1 = 0.f, m2 = 0.f;
+#pragma unroll
+    for (int j = 0; j < J; ++j) {  // zv <- zh, dv <- g = dy * gamma (after the dgamma / dbeta terms have used dy)
+      const int c = lane + 32 * j;
+      const bool ok = c < N;
+      zv[j] = ok ? (zv[j] - mean) * rstd : 0.f;
+      ag[j] += dv[j] * zv[j], ab[j] += dv[j];
+      dv[j] = ok ? dv[j] * __ldg(gamma + c) : 0.f;
+      m1 += dv[j], m2 += dv[j] * zv[j];
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m1 += __shfl_xor_sync(0xffffffffu, m1, o), m2 += __shfl_xor_sync(0xffffffffu, m2, o);
+    m1 /= (float)N, m2 /= (float)N;
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const int c = lane + 32 * j;
+      if (c < N) dz[r * ld_dz + c] = rstd * (dv[j] - m1 - zv[j] * m2);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < J; ++j)
+    if (lane + 32 * j < N) sp[w][lane + 32 * j] = ag[j];
+  __syncthreads();
+  for (int c = threadIdx.x; c < N; c += 256) {
+    float g = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) g += sp[k][c];
+    atomicAdd(dgamma + c, g);
+  }
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < J; ++j)
+    if (lane + 32 * j < N) sp[w][lane + 32 * j] = ab[j];
+  __syncthreads();
+  for (int c = threadIdx.x; c < N; c += 256) {
+    float b = 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) b += sp[k][c];
+    atomicAdd(dbeta + c, b);
+  }
+}
 cudaError_t launch_ln_bwd(const float* dy, int ld_dy, const float* z, int ld_z, int N, const float* gamma, long long R, float* dz, int ld_dz,
                           float* dgamma, float* dbeta, cudaStream_t st) {
   if (R <= 0) return cudaSuccess;
-  if (N > 256) return cudaErrorInvalidValue;
-  gw_ln_bwd_kernel<<<(unsigned)std::min<long long>(GRID_SMS * 8, (R + 7) / 8), 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, dgamma, dbeta);
+  if (N > LN_BWD_MAX_N) return cudaErrorInvalidValue;
+  const unsigned grid = (unsigned)std::min<long long>(GRID_SMS * 8, (R + 7) / 8);
+  if (N <= 256)
+    gw_ln_bwd_kernel<<<grid, 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, dgamma, dbeta);
+  else if (N <= 512)
+    gw_ln_bwd_wide_kernel<16><<<grid, 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, dgamma, dbeta);
+  else
+    gw_ln_bwd_wide_kernel<32><<<grid, 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, dgamma, dbeta);
   count_launch();
   return cudaGetLastError();
 }

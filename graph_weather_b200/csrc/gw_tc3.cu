@@ -41,6 +41,7 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "gw_internal.h"
@@ -1076,6 +1077,27 @@ bool tc3_chain_is_lean(const TcChain& ch_in) {
   if (getenv("GW_TC3_NOFAST")) return false;
   const int32_t all = (int32_t)(0x80000000u | ((1u << ch.n_layers) - 1u));
   return ch.fast == all && ch.out_mode == 0;
+}
+cudaError_t tc_column_block(const TcChain& ch, int n0, int nb, TcChain* out) {
+  const TcLayer& L = ch.layer[0];
+  if (ch.n_layers != 1 || n0 < 0 || nb <= 0 || nb > TC_COL_BLOCK || n0 + nb > L.n_valid) return cudaErrorInvalidValue;
+  if (L.ln_g && (n0 != 0 || nb != L.n_valid)) return cudaErrorInvalidValue;  // a LayerNorm row must stay in one chain
+  if (L.feeds_next || L.seg_dst || ch.out_mode != 0) return cudaErrorInvalidValue;
+  auto shift = [&](RowSrc s) {  // the source's columns n0 .. n0 + nb - 1
+    if (s.kind != SRC_NONE) s.col0 += n0, s.width = std::max(0, std::min(s.width - n0, nb));
+    return s;
+  };
+  *out = ch;
+  TcLayer& B = out->layer[0];
+  B.Wp = nullptr, B.wamax = nullptr;
+  B.N = (nb + 15) / 16 * 16, B.N32 = tc_packed_rows(nb), B.n_valid = nb;
+  if (L.bias) B.bias = L.bias + n0;
+  for (int a = 0; a < 2; ++a) B.add[a] = shift(L.add[a]);
+  B.residual = shift(L.residual), B.mask = shift(L.mask);
+  if (L.out) B.out = L.out + n0;
+  if (L.save_pre) B.save_pre = L.save_pre + n0;
+  B.out_cols = std::max(0, std::min(L.out_cols - n0, nb));
+  return cudaSuccess;
 }
 cudaError_t launch_chain_tc3(const TcChain& ch_in, cudaStream_t stream) {
   TcChain ch = ch_in;

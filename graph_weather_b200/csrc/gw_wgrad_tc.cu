@@ -7,7 +7,8 @@
 //
 // Layout of the work (one CTA = 2 consumer warpgroups = 256 threads, 1 CTA per SM):
 //   * output block: 128 rows o (warpgroup w owns 64 w .. 64 w + 63, a 64 x NW fp32 accumulator in registers, NW = K rounded up
-//     to 64 <= 256) x all K columns; gridDim.y = ceil(N / 128) blocks of o, gridDim.x = row ranges.
+//     to 64 <= 256) x all K columns; gridDim.y = ceil(N / 128) blocks of o, gridDim.x = row ranges.  A wider K (the encoder's
+//     621 input features) runs as blocks of 256 columns, each a launch of its own over all rows, one after the other.
 //   * per 64-row chunk r0 .. r0 + 63 the threads read dY[r, o] and A(r, k) (coalesced along o / k), split them to fp16 hi/lo (or
 //     round to bf16) and store them TRANSPOSED into two K-major SWIZZLE_128B images [o][r] and [k][r] -- the layout of the chain
 //     kernel's operands (gw_tc3.cu), so the same GMMA descriptors apply: D[o, k] += Y^T[o, r] . (A^T[k, r])^T.  A thread loads 8
@@ -21,6 +22,8 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <algorithm>
 
 #include "gw_internal.h"
 #include "gw_ops.h"
@@ -237,25 +240,30 @@ static int splits_for(long long R, int gy) {
 
 }  // namespace wgt
 
+namespace wgt {
+// K > KB runs as blocks of KB columns of A (one kernel + sum pass each, in order, through the same partials)
+constexpr int KB = 256;
+}  // namespace wgt
+
 size_t wgrad_tc_workspace_floats(long long R, int N, int K) {
   const int S = wgt::splits_for(R, (N + wgt::OB - 1) / wgt::OB);
-  return (size_t)S * N * K + (size_t)S * N + 2;
+  return (size_t)S * N * std::min(K, wgt::KB) + (size_t)S * N + 2;
 }
 
 cudaError_t launch_wgrad_tc(const float* dY, int ldy, int N, const RowSrc& a, int K, int rows_per_sample, int batch, float* dW, int ldw, float* db,
                             bool split, float* ws, size_t ws_floats, int32_t* status, cudaStream_t st) {
   using namespace wgt;
-  if (N <= 0 || N > 256 || K <= 0 || K > 256 || rows_per_sample <= 0 || batch <= 0) return cudaErrorInvalidValue;
+  if (N <= 0 || K <= 0 || rows_per_sample <= 0 || batch <= 0) return cudaErrorInvalidValue;
   if (a.kind != SRC_STREAM && a.kind != SRC_BCAST) return cudaErrorInvalidValue;
   const long long R = (long long)rows_per_sample * batch;
   const int gy = (N + OB - 1) / OB;
   const int S = splits_for(R, gy);
   if (ws_floats < wgrad_tc_workspace_floats(R, N, K)) return cudaErrorInvalidValue;
   Args g;
-  g.dY = dY, g.ldy = ldy, g.N = N, g.K = K, g.a = a, g.rows = rows_per_sample, g.batch = batch, g.R = R;
+  g.dY = dY, g.ldy = ldy, g.N = N, g.a = a, g.rows = rows_per_sample, g.batch = batch, g.R = R;
   const long long chunks = (R + RC - 1) / RC;
   g.rows_per_cta = (int)(((chunks + S - 1) / S) * RC);
-  g.part = ws, g.part_b = ws + (size_t)S * N * K;
+  g.part = ws, g.part_b = ws + (size_t)S * N * std::min(K, KB);
   float* amax = g.part_b + (size_t)S * N;
   g.amax = amax, g.status = status;
   cudaError_t e;
@@ -265,25 +273,30 @@ cudaError_t launch_wgrad_tc(const float* dY, int ldy, int N, const RowSrc& a, in
     const long long arows = a.kind == SRC_BCAST ? rows_per_sample : (long long)batch * a.src_rows;
     if ((e = launch_absmax_flat(a.base, arows * a.ld, amax + 1, st)) != cudaSuccess) return e;
   }
-  const int nw = (K + 63) / 64;  // 1..4
   const dim3 grid(S, gy);
-#define GW_WG(SPLIT_, NW_)                                                                                            \
-  do {                                                                                                                \
-    e = cudaFuncSetAttribute(gw_wgrad_tc_kernel<SPLIT_, NW_>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); \
-    if (e != cudaSuccess) return e;                                                                                   \
-    gw_wgrad_tc_kernel<SPLIT_, NW_><<<grid, THREADS, SMEM_BYTES, st>>>(g);                                            \
-  } while (0)
-  if (split) {
-    if (nw == 1) GW_WG(true, 64); else if (nw == 2) GW_WG(true, 128); else if (nw == 3) GW_WG(true, 192); else GW_WG(true, 256);
-  } else {
-    if (nw == 1) GW_WG(false, 64); else if (nw == 2) GW_WG(false, 128); else if (nw == 3) GW_WG(false, 192); else GW_WG(false, 256);
-  }
+  for (int k0 = 0; k0 < K; k0 += KB) {  // dW[:, k0 .. k0 + kb) from A's columns k0 .. (the bias gradient with the first block)
+    const int kb = std::min(KB, K - k0);
+    g.K = kb, g.a = a, g.a.col0 = a.col0 + k0;
+    const int nw = (kb + 63) / 64;  // 1..4
+#define GW_WG(SPLIT_, NW_)                                                                                              \
+    do {                                                                                                                \
+      e = cudaFuncSetAttribute(gw_wgrad_tc_kernel<SPLIT_, NW_>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES); \
+      if (e != cudaSuccess) return e;                                                                                   \
+      gw_wgrad_tc_kernel<SPLIT_, NW_><<<grid, THREADS, SMEM_BYTES, st>>>(g);                                            \
+    } while (0)
+    if (split) {
+      if (nw == 1) GW_WG(true, 64); else if (nw == 2) GW_WG(true, 128); else if (nw == 3) GW_WG(true, 192); else GW_WG(true, 256);
+    } else {
+      if (nw == 1) GW_WG(false, 64); else if (nw == 2) GW_WG(false, 128); else if (nw == 3) GW_WG(false, 192); else GW_WG(false, 256);
+    }
 #undef GW_WG
-  count_launch();
-  if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  gw_wgrad_sum_kernel<<<4 * GRID_SMS, 256, 0, st>>>(g.part, g.part_b, S, N, K, dW, ldw, db);
-  count_launch();
-  return cudaGetLastError();
+    count_launch();
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    gw_wgrad_sum_kernel<<<4 * GRID_SMS, 256, 0, st>>>(g.part, g.part_b, S, N, kb, dW + k0, ldw, k0 == 0 ? db : nullptr);
+    count_launch();
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 }  // namespace gw

@@ -1,5 +1,10 @@
 """Times one training step (forward with tape + NormalizedMSELoss + backward + SGD update) of GraphWeatherForecaster.
-    python tools/train_step_bench.py [--grid 1deg|10deg] [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16]
+    python tools/train_step_bench.py [--grid 1deg|2deg|10deg] [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16]
+                                     [--feature-dim F] [--aux-dim A] [--num-blocks NB] [--width W]
+The model defaults to the README's 78 + 24 features, 9 blocks, 256-wide.  The reference's ERA5 training scripts:
+    train/run_fulll.py  --feature-dim 597 --aux-dim 24 --num-blocks 6 (1-degree grid)
+    train/run.py        --feature-dim 605 --aux-dim 40 --num-blocks 6 --width 1024 --grid 2deg
+(--width sets the node / edge / hidden / decoder widths together.)
 Prints one JSON line: ms/step, samples/s, the device time of the step's phases (libgwb200 timing tags train_*; one extra timed
 step after the measured ones, since the per-launch events add a little host work), peak device memory, and the card name and
 power limit read in the same run."""
@@ -31,24 +36,33 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--grid", default="1deg", choices=["1deg", "10deg"])
+    ap.add_argument("--grid", default="1deg", choices=["1deg", "2deg", "10deg"])
     ap.add_argument("--batch", type=int, default=2)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--train-precision", default="fp32_simt", choices=["fp32_simt", "fp32", "bf16"])
+    ap.add_argument("--feature-dim", type=int, default=78)
+    ap.add_argument("--aux-dim", type=int, default=24)
+    ap.add_argument("--num-blocks", type=int, default=9)
+    ap.add_argument("--width", type=int, default=None, help="node / edge / hidden / decoder width (default: the model's 256 / 128)")
     a = ap.parse_args()
     import __graft_entry__ as ge
 
     ge.build()
     from graph_weather_b200 import GraphWeatherForecaster, NormalizedMSELoss
 
-    step = 1 if a.grid == "1deg" else 10
+    step = {"1deg": 1, "2deg": 2, "10deg": 10}[a.grid]
     ll = [(float(lat), float(lon)) for lat in range(-90, 90, step) for lon in range(0, 360, step)]
     torch.manual_seed(0)
-    model = GraphWeatherForecaster(ll, train_precision=a.train_precision).cuda().train()
-    crit = NormalizedMSELoss([1.0] * 78, ll, normalize=True)
+    dims = dict(feature_dim=a.feature_dim, aux_dim=a.aux_dim, num_blocks=a.num_blocks)
+    if a.width is not None:
+        dims.update(node_dim=a.width, edge_dim=a.width, hidden_dim_processor_node=a.width, hidden_dim_processor_edge=a.width,
+                    hidden_dim_decoder=a.width)  # fmt: skip
+    model = GraphWeatherForecaster(ll, train_precision=a.train_precision, **dims).cuda().train()
+    F = a.feature_dim
+    crit = NormalizedMSELoss([1.0] * F, ll, normalize=True)
     opt = torch.optim.SGD(model.parameters(), lr=1e-3)
-    x = torch.randn(a.batch, len(ll), 102, device="cuda")
-    y = torch.randn(a.batch, len(ll), 78, device="cuda")
+    x = torch.randn(a.batch, len(ll), F + a.aux_dim, device="cuda")
+    y = torch.randn(a.batch, len(ll), F, device="cuda")
     losses = []
 
     def one():
@@ -81,6 +95,7 @@ def main():
     phases = {k: round(v[1], 3) for k, v in tags.items() if k.startswith("train_") or k == "const"}
     plan.status()
     print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "train_precision": a.train_precision, "grid": a.grid, "batch": a.batch,
+                      "dims": dims, "n_params": sum(q.numel() for q in model.parameters()),
                       "ms_per_step": ms, "samples_per_s": a.batch / (ms * 1e-3), "phase_ms": phases,
                       "phase_launches": {k: v[0] for k, v in tags.items() if k.startswith("train_")},
                       "torch_peak_alloc_gib": round(peak / 2**30, 2), "device_mem_used_gib": round((total - free) / 2**30, 1),
