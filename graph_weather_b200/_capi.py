@@ -303,7 +303,8 @@ class Plan:
         if v.value:
             raise RuntimeError(f"libgwb200 device status {v.value}: " + ("an operand left the fp16 range despite range scaling in precision 'fp32' (use 'fp32_simt'); " if v.value & 1 else "")
                                + ("pipeline timeout; " if v.value & 2 else "") + ("shared memory misaligned; " if v.value & 4 else "")
-                               + ("a magnitude bound is not finite: the inputs contain inf / nan or overflow fp32" if v.value & 8 else ""))
+                               + ("a magnitude bound is not finite: the inputs contain inf / nan or overflow fp32; " if v.value & 8 else "")
+                               + ("an observation could not be located on the mesh (non-finite coordinates)" if v.value & 16 else ""))
         return 0
 
     def peek(self) -> int:

@@ -1,7 +1,8 @@
 // gw_kernel_harness.cu -- test-only shim over the internal launchers of libgwb200.so (tests/test_gpu_kernels.py).
 //
 // Host code only: flat extern "C" wrappers that the kernel tests call through ctypes, so that every CUDA primitive of the
-// training step can be run on its own and compared with a float64 reference.  The row sources cross the boundary as the
+// training step, the forward's CUDA-core row ops and helpers, and the device-built graphs (tests/test_gpu_forward_simt.py,
+// tests/test_gpu_graph_kernels.py) can be run on its own and compared with a float64 or host reference.  The row sources cross the boundary as the
 // harness's own POD (HSrc / HOp below), never as gw::RowSrc / gw::TcChain, so the tests do not depend on their layout.  Every
 // wrapper enqueues on the caller's stream and returns the CUDA error code (cudaErrorInvalidValue from a launcher that does not
 // take a shape is passed through unchanged).  Built by the test into a temporary directory and linked against the package's
@@ -17,7 +18,7 @@ using namespace gw;
 
 extern "C" {
 
-struct HSrc {  // one row source: kind = gw::SrcKind (0 none, 1 stream, 2 bcast, 3 gather, 5 relu(gather + bcast), 6 bgather)
+struct HSrc {  // one row source: kind = gw::SrcKind (0 none, 1 stream, 2 bcast, 3 gather, 4 segsum, 5 relu(gather + bcast), 6 bgather)
   int32_t kind, width, ld, col0;
   const float* base;
   int32_t src_rows;
@@ -25,6 +26,8 @@ struct HSrc {  // one row source: kind = gw::SrcKind (0 none, 1 stream, 2 bcast,
   const float* base2;  // kind 5: the broadcast table (ld2)
   int32_t ld2;
   const int32_t* bound_mul_i;  // h_chain: the source's bound is multiplied by this device integer (a sum of up to that many rows)
+  const int32_t* ptr;          // kind 4: CSR [rows + 1] over the summed table's rows
+  const int32_t* perm;         // kind 4: optional row permutation (null: rows in CSR order)
 };
 
 struct HOp {  // one training row op: out = mask(residual + LN(relu(concat(a) . W^T + bias + add)))
@@ -78,7 +81,7 @@ namespace {
 RowSrc row_src(const HSrc& h) {
   RowSrc s;
   s.kind = h.kind, s.width = h.width, s.ld = h.ld, s.col0 = h.col0, s.base = h.base, s.src_rows = h.src_rows, s.idx = h.idx;
-  s.base2 = h.base2, s.ld2 = h.ld2;
+  s.base2 = h.base2, s.ld2 = h.ld2, s.ptr = h.ptr, s.perm = h.perm;
   return s;
 }
 
@@ -312,6 +315,47 @@ int h_gather_rows(const float* in, int ld_in, int src_rows, const int32_t* idx, 
 
 int h_transpose(const float* W, int rows, int cols, float* WT, void* stream) {
   return (int)launch_transpose(W, rows, cols, WT, (cudaStream_t)stream);
+}
+
+// ---- the forward's small helpers (gw_simt.cu) and the device-built graphs (gw_graph.cu) ---------------------------------------
+// dst[r, :] = [src[r, 0:width], 0 ...] over ld_dst columns; *amax = max(*amax, max |src|) (amax may be null)
+int h_pad_rows(const float* src, int ld_src, int width, float* dst, int ld_dst, long long rows, float* amax, void* stream) {
+  return (int)launch_pad_rows(src, ld_src, width, dst, ld_dst, rows, amax, (cudaStream_t)stream);
+}
+
+// *amax = max(*amax, max |p[0..n)|)
+int h_absmax_flat(const float* p, long long n, float* amax, void* stream) { return (int)launch_absmax_flat(p, n, amax, (cudaStream_t)stream); }
+
+// dst[j] = i for ptr[i] <= j < ptr[i + 1] (dst may be null); stats = {max(stats[0], longest segment), min(stats[1], shortest)}
+int h_csr_expand(const int32_t* ptr, int n, int32_t* dst, int* stats, void* stream) {
+  return (int)launch_csr_expand(ptr, n, dst, stats, (cudaStream_t)stream);
+}
+
+// perm = the row ids ordered by src (ties in row order), ptr[s] = first position of slot s (s = 0 .. n_slots); workspace sized here
+int h_sort_csr(const int32_t* src, int n, int n_slots, int32_t* perm, int32_t* ptr, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  Temps t(st);
+  const size_t nb = sort_csr_workspace_bytes(n);
+  unsigned char* ws = nullptr;
+  H_TRY(t.get(&ws, nb));
+  return (int)launch_sort_csr(src, n, n_slots, perm, ptr, ws, nb, st);
+}
+
+// The observation graph of n points llh [n, 3] (lat deg, lon deg, height): the arrays of h3lite.device_tables(res) as device
+// pointers (gw_plan_set_h3_tables), cell_slot = H - 1 - rank; slot [n], perm [n], ptr [n_slots + 1], attr [n, 3]; workspace sized here
+int h_obs_graph(int res, int n_cells, int lat_n, const double* frames, const int32_t* cell_of, const int32_t* cell_slot, const double* cell_lat,
+                const double* cell_lng, double scale, double rot_cos, double rot_sin, const float* llh, int n, int n_slots, int32_t* slot,
+                int32_t* perm, int32_t* ptr, float* attr, int32_t* status, void* stream) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  H3Tables tab;
+  tab.res = res, tab.n_cells = n_cells, tab.lat_n = lat_n;
+  tab.frames = frames, tab.cell_of = cell_of, tab.cell_slot = cell_slot, tab.cell_lat = cell_lat, tab.cell_lng = cell_lng;
+  tab.scale = scale, tab.cr = rot_cos, tab.sr = rot_sin;
+  Temps t(st);
+  const size_t nb = obs_graph_workspace_bytes(n);
+  unsigned char* ws = nullptr;
+  H_TRY(t.get(&ws, nb));
+  return (int)launch_obs_graph(tab, llh, n, n_slots, slot, perm, ptr, attr, ws, nb, status, st);
 }
 
 }  // extern "C"

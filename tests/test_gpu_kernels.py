@@ -26,7 +26,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HARNESS = os.path.join(ROOT, "tests", "kernels", "gw_kernel_harness.cu")
 PKG = os.path.join(ROOT, "graph_weather_b200")
 
-NONE, STREAM, BCAST, GATHER, BGATHER = 0, 1, 2, 3, 6
+NONE, STREAM, BCAST, GATHER, SEGSUM, GBR, BGATHER = 0, 1, 2, 3, 4, 5, 6  # gw::SrcKind (GBR: relu(gather + broadcast))
 SIMT, FP32, BF16 = 0, 1, 2
 PREC_NAME = {SIMT: "fp32_simt", FP32: "fp32", BF16: "bf16"}
 
@@ -50,7 +50,7 @@ WGRAD_LONG_EPS_F = 6e-5
 class HSrc(ctypes.Structure):
     _fields_ = [("kind", ctypes.c_int32), ("width", ctypes.c_int32), ("ld", ctypes.c_int32), ("col0", ctypes.c_int32),
                 ("base", ctypes.c_void_p), ("src_rows", ctypes.c_int32), ("idx", ctypes.c_void_p), ("base2", ctypes.c_void_p),
-                ("ld2", ctypes.c_int32), ("bound_mul_i", ctypes.c_void_p)]
+                ("ld2", ctypes.c_int32), ("bound_mul_i", ctypes.c_void_p), ("ptr", ctypes.c_void_p), ("perm", ctypes.c_void_p)]
 
 
 class HOp(ctypes.Structure):
@@ -90,6 +90,12 @@ _SIGNATURES = {
     "h_batch_reduce": [_vp, _i32, _i64, _i32, _i32, _vp, _i32, _i32, _vp],
     "h_gather_rows": [_vp, _i32, _i32, _vp, _i64, _i32, _i32, _vp, _i32, _i32, _vp],
     "h_transpose": [_vp, _i32, _i32, _vp, _vp],
+    "h_pad_rows": [_vp, _i32, _i32, _vp, _i32, _i64, _vp, _vp],
+    "h_absmax_flat": [_vp, _i64, _vp, _vp],
+    "h_csr_expand": [_vp, _i32, _vp, _vp, _vp],
+    "h_sort_csr": [_vp, _i32, _i32, _vp, _vp, _vp],
+    "h_obs_graph": [_i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, ctypes.c_double, _vp, _i32, _i32, _vp, _vp,
+                    _vp, _vp, _vp, _vp],
 }
 
 
@@ -188,18 +194,37 @@ FLOAT = [pytest.param(dict(exact=False, mag=1.0), id="normal"), pytest.param(dic
 
 
 class Src:
-    """A row source over a 2-d fp32 tensor t [*, ld]; rows64() assembles the [batch * rows, width] float64 rows it stands for."""
+    """A row source over a 2-d fp32 tensor t [*, ld]; rows64() assembles the [batch * rows, width] float64 rows it stands for.
+    SEGSUM: the sum of t's rows over CSR segment i (ptr, optional perm); GBR: relu(t[b, idx[i]] + t2[i]) (t2 [rows, ld2])."""
 
-    def __init__(self, kind, t, width, col0=0, src_rows=0, idx=None):
+    def __init__(self, kind, t, width, col0=0, src_rows=0, idx=None, ptr=None, perm=None, t2=None):
         self.kind, self.t, self.width, self.ld, self.col0, self.src_rows, self.idx = kind, t, width, t.shape[1], col0, src_rows, idx
+        self.ptr, self.perm, self.t2 = ptr, perm, t2
 
     def h(self):
-        return HSrc(self.kind, self.width, self.ld, self.col0, self.t.data_ptr(), self.src_rows, self.idx.data_ptr() if self.idx is not None else None)
+        def a(x):
+            return x.data_ptr() if x is not None else None
 
-    def rows64(self, rows, batch):
+        return HSrc(self.kind, self.width, self.ld, self.col0, self.t.data_ptr(), self.src_rows, a(self.idx), a(self.t2),
+                    self.t2.shape[1] if self.t2 is not None else 0, None, a(self.ptr), a(self.perm))  # fmt: skip
+
+    def rows64(self, rows, batch, absolute=False):
+        """absolute: the rows of |values| a sum runs over (SEGSUM: the sum of |rows|), for the magnitude term of eps_el."""
         t = self.t[:, self.col0:self.col0 + self.width].double()
         b = torch.arange(batch, device="cuda")[:, None]
         i = torch.arange(rows, device="cuda")[None, :]
+        if self.kind == SEGSUM:  # float64 sum over each segment, rows in perm order when perm is set
+            t = t.abs() if absolute else t
+            ptr = self.ptr.long()
+            seg = torch.repeat_interleave(torch.arange(rows, device="cuda"), ptr[1:] - ptr[:-1])
+            e = self.perm.long() if self.perm is not None else torch.arange(int(ptr[-1]), device="cuda")
+            out = torch.zeros(batch, rows, self.width, dtype=torch.float64, device="cuda")
+            for s in range(batch):
+                out[s].index_add_(0, seg, t[s * self.src_rows + e])
+            return out.reshape(batch * rows, self.width)
+        if self.kind == GBR:
+            g = t[(b * self.src_rows + self.idx.long()[None, :]).reshape(-1)]
+            return torch.relu(g + self.t2[:, :self.width].double()[i.expand(batch, rows).reshape(-1)])
         if self.kind == STREAM:
             r = b * self.src_rows + i
         elif self.kind == BCAST:
@@ -277,7 +302,7 @@ class RowOp:
         A = torch.cat([s.rows64(self.rows, self.batch) for s in self.a], dim=1)
         W = self.W[:, self.wcol:self.wcol + self.K].double()
         y = A @ W.T
-        c = A.abs() @ W.abs().T
+        c = torch.cat([s.rows64(self.rows, self.batch, absolute=True) for s in self.a], dim=1).abs() @ W.abs().T
         if self.bias is not None:
             y = y + self.bias.double()
         for s in self.add:
