@@ -69,6 +69,8 @@ _SIGNATURES = {
     "gw_forward_strided": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _vp]),
     "gw_constraint_workspace_bytes": (_i64, [_i64, _i32]),
     "gw_constraint_apply": (ctypes.c_int, [_i32, _vp, _vp, _i32, _i32, _vp, _vp, _i64, _i64, _i32, ctypes.c_float, _vp, _vp]),
+    "gw_constraint_backward_workspace_bytes": (_i64, [_i64, _i64, _i32]),
+    "gw_constraint_backward": (ctypes.c_int, [_i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _i32, ctypes.c_float, _vp, _vp]),
     "gw_normalized_mse_loss_grad": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _vp, ctypes.c_float, _vp, _vp]),
     "gw_train_forward": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp]),
     "gw_train_backward": (ctypes.c_int, [_vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),

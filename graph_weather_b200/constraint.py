@@ -4,6 +4,8 @@ GraphWeatherForecaster (forecast.py:178-213) for the CUDA path.
 The reference moves every tensor through Python loops over the nodes (`graph_to_grid` / `grid_to_graph`, O(N) Python per
 call) and a handful of eager ops.  Here the mapping is two precomputed index vectors and the constraint itself is
 `gw_constraint_apply` (csrc/gw_constraint.cu): column means + one element-wise pass on the device, no layout copies.
+The backward (training, and any call on tensors that require grad) is `gw_constraint_backward`: column sums of the upstream
+gradient, then one pass that sums each row's nodes through the CSR of the row index.
 Only `upsampling_factor == 1` exists in the reference's forecaster (forecast.py:166) and only that is built."""
 
 from __future__ import annotations
@@ -83,18 +85,28 @@ class PhysicalConstraintLayer(nn.Module):
             raise NotImplementedError("upsampling_factor != 1: GraphWeatherForecaster only ever uses 1 (forecast.py:166)")
         self._ws = {}
 
-    def apply_rows(self, hr: torch.Tensor, lr: torch.Tensor, src: torch.Tensor, lr_channels: int) -> torch.Tensor:
-        """hr [B, N, C] rows, lr [B, N, >= lr_channels] rows (any row stride), src [N] int32 -> constrained rows [B, N, C]."""
+    def _prepare(self, hr: torch.Tensor, lr: torch.Tensor):
+        """The float32 rows the kernels read: hr contiguous, lr with unit column stride and rows of one stride."""
         if self.constraint_type not in CONSTRAINT_TYPES:
             raise ValueError(f"Unknown constraint type: {self.constraint_type}")
         if not hr.is_cuda:
             raise RuntimeError("graph_weather_b200.PhysicalConstraintLayer runs on CUDA tensors only (no CPU fallback)")
-        lib = _capi.load()
-        B, N, C = hr.shape
+        N = hr.shape[1]
         hr = hr.detach().to(torch.float32).contiguous()
         lr = lr.detach().to(torch.float32)
         if lr.stride(-1) != 1 or lr.stride(0) != N * lr.stride(1):
             lr = lr.contiguous()
+        return hr, lr
+
+    def apply_rows(self, hr: torch.Tensor, lr: torch.Tensor, src: torch.Tensor, lr_channels: int) -> torch.Tensor:
+        """hr [B, N, C] rows, lr [B, N, >= lr_channels] rows (any row stride), src [N] int32 -> constrained rows [B, N, C].
+        No autograd: `constrain_rows` is the differentiable form."""
+        hr, lr = self._prepare(hr, lr)
+        return self._launch_apply(hr, lr, src, lr_channels)
+
+    def _launch_apply(self, hr, lr, src, lr_channels):
+        lib = _capi.load()
+        B, N, C = hr.shape
         out = torch.empty_like(hr)
         key = (str(hr.device), B, C)
         if key not in self._ws:
@@ -106,6 +118,27 @@ class PhysicalConstraintLayer(nn.Module):
                 int(lr_channels), ctypes.c_void_p(src.data_ptr()), ctypes.c_void_p(out.data_ptr()), B, N, C, float(self.exp_factor),
                 ctypes.c_void_p(self._ws[key].data_ptr()), ctypes.c_void_p(st)))  # fmt: skip
         return out
+
+    def _backward(self, dy, hr, lr, src, need_lr):
+        """gw_constraint_backward: d loss / d out [B, N, C] -> (d_hr [B, N, C], d_lr [B, N, C] or None)."""
+        lib = _capi.load()
+        B, N, C = hr.shape
+        dy = dy.to(torch.float32).contiguous()
+        d_hr = torch.empty_like(hr)
+        d_lr = torch.empty_like(hr) if need_lr else None
+        ws = torch.empty(int(lib.gw_constraint_backward_workspace_bytes(B, N, C)), dtype=torch.uint8, device=hr.device)
+        with torch.cuda.device(hr.device):
+            st = torch.cuda.current_stream().cuda_stream
+            _capi._check(lib.gw_constraint_backward(
+                CONSTRAINT_TYPES[self.constraint_type], ctypes.c_void_p(dy.data_ptr()), ctypes.c_void_p(hr.data_ptr()),
+                ctypes.c_void_p(lr.data_ptr()), int(lr.stride(1)), int(lr.shape[-1]), ctypes.c_void_p(src.data_ptr()),
+                ctypes.c_void_p(d_hr.data_ptr()), ctypes.c_void_p(d_lr.data_ptr() if d_lr is not None else None), B, N, C,
+                float(self.exp_factor), ctypes.c_void_p(ws.data_ptr()), ctypes.c_void_p(st)))  # fmt: skip
+        return d_hr, d_lr
+
+    def constrain_rows(self, hr: torch.Tensor, lr: torch.Tensor, src: torch.Tensor) -> torch.Tensor:
+        """apply_rows with lr_channels = lr.shape[-1], differentiable in hr and lr (gw_constraint_backward)."""
+        return _ConstraintFn.apply(self, hr, lr, src)
 
     def forward(self, hr_graph: torch.Tensor, lr_graph: torch.Tensor) -> torch.Tensor:
         m: GridMapping = self.model._grid_mapping
@@ -124,4 +157,26 @@ class PhysicalConstraintLayer(nn.Module):
             lr = lr_graph.reshape(lr_graph.shape[0], lr_graph.shape[1], H * W).permute(0, 2, 1).contiguous()
         else:
             raise ValueError("Input tensor must be either 3D (graph) or 4D (grid).")
+        if torch.is_grad_enabled() and (hr.requires_grad or lr.requires_grad):
+            return self.constrain_rows(hr, lr, src.contiguous())
         return self.apply_rows(hr, lr, src.contiguous(), lr.shape[-1])
+
+
+class _ConstraintFn(torch.autograd.Function):
+    """autograd node of PhysicalConstraintLayer on rows: forward = gw_constraint_apply, backward = gw_constraint_backward (the
+    gradients of hr and of lr, the latter only when lr requires it).  Reshapes and permutes around it are torch's."""
+
+    @staticmethod
+    def forward(ctx, layer, hr, lr, src):
+        hr32, lr32 = layer._prepare(hr, lr)
+        out = layer._launch_apply(hr32, lr32, src, lr32.shape[-1])
+        ctx.layer, ctx.dtypes = layer, (hr.dtype, lr.dtype)
+        ctx.save_for_backward(hr32, lr32, src)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        hr32, lr32, src = ctx.saved_tensors
+        d_hr, d_lr = ctx.layer._backward(grad_out, hr32, lr32, src, ctx.needs_input_grad[2])
+        return (None, d_hr.to(ctx.dtypes[0]) if ctx.needs_input_grad[1] else None,
+                d_lr.to(ctx.dtypes[1]) if d_lr is not None else None, None)  # fmt: skip

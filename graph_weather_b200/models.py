@@ -595,7 +595,10 @@ class GraphWeatherForecasterConfig:
 
 
 class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
-    """GraphWeatherForecaster(lat_lons)(features): forecast.py:61-247 (constraint_type='none', no thermalizer)."""
+    """GraphWeatherForecaster(lat_lons)(features): forecast.py:61-247, the main weather prediction model, optionally with physical
+    constraints (constraint_type 'additive' | 'multiplicative' | 'softmax', upsampling factor 1); no thermalizer.  Inference and
+    training (train mode with autograd on: `loss.backward()` runs the CUDA backward of the network and of the constraint layer)
+    run on the device."""
 
     def __init__(self, lat_lons: list, resolution: int = 2, feature_dim: int = 78, aux_dim: int = 24, output_dim: Optional[int] = None,
                  node_dim: int = 256, edge_dim: int = 256, num_blocks: int = 9, hidden_dim_processor_node: int = 256,
@@ -672,11 +675,14 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
     def _constrain(self, out, f):
         """forecast.py:231-246: the decoder output, read as a row-major H x W grid, is corrected against the input's first
         feature_dim channels.  `rearrange(x, "b (h w) c -> b c h w")` only re-labels rows here: no layout pass exists."""
+        return self.constraint.apply_rows(out, f, self._constraint_cell(out), self.feature_dim)
+
+    def _constraint_cell(self, out):
         H, W = self.grid_shape
         if out.shape[1] != H * W:
             raise RuntimeError(f"Shape mismatch, can't divide axis of length {out.shape[1]} in chunks of {W}")  # einops' failure
         cell, _ = self._grid_mapping.tensors(out.device)
-        return self.constraint.apply_rows(out, f, cell.to(torch.int32).contiguous(), self.feature_dim)
+        return cell.to(torch.int32).contiguous()
 
     def _training_engine(self):
         """The plan the training step runs on, of precision `train_precision` (created on first use; the inference engine stays
@@ -696,10 +702,14 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
             # train mode with autograd on, like every training caller of the reference (train/run.py:508-543): the forward keeps
             # its activations and `loss.backward()` runs the CUDA backward.  Inference (`model.eval()` or `torch.no_grad()`) takes
             # the tensor-core path below.
-            if self.constraint_type != "none":
-                raise NotImplementedError("training with a constraint layer is not built (inference only)")
             params = [q for _, q in self.named_parameters()]
-            return _ForecastTrainFn.apply(self, features, *params)
+            out = _ForecastTrainFn.apply(self, features, *params)
+            if self.constraint_type != "none":
+                # forecast.py:235-246 under autograd: the layer's backward adds the gradient of its `lr` input (the first
+                # feature_dim features) to the residual and encoder paths of features.grad
+                cell = self._constraint_cell(out)
+                out = self.constraint.constrain_rows(out, features[..., : self.feature_dim], cell)
+            return out
         B = features.shape[0]
         plan = self._engine.ensure(features.device, B, self._named())
         f = features.detach().to(torch.float32).contiguous()

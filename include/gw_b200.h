@@ -219,6 +219,17 @@ int gw_normalized_mse_loss_sum(const float* pred, const float* target, const flo
 int64_t gw_constraint_workspace_bytes(int64_t batch, int32_t channels);
 int gw_constraint_apply(int32_t type, const float* hr, const float* lr, int32_t lr_ld, int32_t lr_channels, const int32_t* src,
                         float* out, int64_t batch, int64_t n_nodes, int32_t channels, float exp_factor, void* workspace, void* stream);
+/* Backward of gw_constraint_apply (the reference trains through the layer: forecast.py:231-246 lies inside the forward that
+ * loss.backward() walks).  dy [batch, n_nodes, channels] = d loss / d out; hr, lr, lr_ld, src, exp_factor: the forward's inputs.
+ *   d_hr [batch, n_nodes, channels]  gradient of hr;  d_lr [batch, n_nodes, channels] (contiguous; NULL: not computed) gradient of
+ *   lr's first `channels` columns.  Rows no node reads get 0; a row read by several nodes sums their terms in ascending node order.
+ * lr_channels must equal channels.  Additive / multiplicative: column sums in double, fixed order (the multiplicative means are
+ * recomputed by the forward's kernels, bit for bit); softmax: torch's autograd of constraint_layer.py:172-187 op by op in fp32.
+ * No atomics: repeated calls give identical bits.  workspace: gw_constraint_backward_workspace_bytes(batch, n_nodes, channels). */
+int64_t gw_constraint_backward_workspace_bytes(int64_t batch, int64_t n_nodes, int32_t channels);
+int gw_constraint_backward(int32_t type, const float* dy, const float* hr, const float* lr, int32_t lr_ld, int32_t lr_channels, const int32_t* src,
+                           float* d_hr, float* d_lr, int64_t batch, int64_t n_nodes, int32_t channels, float exp_factor, void* workspace,
+                           void* stream);
 
 /* Backward of the loss sum: grad_pred[b, n, f] = (*scale_dev) * scale * node_weight[n] * 2 (pred - target) * inv_variance[f] / n_features.
  * scale_dev (device float, may be NULL = 1) carries the upstream gradient; scale is a host factor (1 / global row count). */

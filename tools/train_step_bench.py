@@ -1,13 +1,15 @@
 """Times one training step (forward with tape + NormalizedMSELoss + backward + SGD update) of GraphWeatherForecaster.
     python tools/train_step_bench.py [--grid 1deg|2deg|10deg] [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16]
                                      [--feature-dim F] [--aux-dim A] [--num-blocks NB] [--width W]
+                                     [--constraint-type none|additive|multiplicative|softmax]
 The model defaults to the README's 78 + 24 features, 9 blocks, 256-wide.  The reference's ERA5 training scripts:
     train/run_fulll.py  --feature-dim 597 --aux-dim 24 --num-blocks 6 (1-degree grid)
     train/run.py        --feature-dim 605 --aux-dim 40 --num-blocks 6 --width 1024 --grid 2deg
 (--width sets the node / edge / hidden / decoder widths together.)
 Prints one JSON line: ms/step, samples/s, the device time of the step's phases (libgwb200 timing tags train_*; one extra timed
 step after the measured ones, since the per-launch events add a little host work), peak device memory, and the card name and
-power limit read in the same run."""
+power limit read in the same run.  With --constraint-type the step includes PhysicalConstraintLayer; the constraint backward
+(gw_constraint_backward, no timing tag of the plan) is also timed on its own with CUDA events around it, on the step's shapes."""
 import argparse
 import json
 import os
@@ -34,6 +36,30 @@ def card():
     return info
 
 
+def constraint_backward_time(model, x, F, reps=20):
+    """Device time of one gw_constraint_backward on the step's shapes (d_hr and d_lr; CSR build included), CUDA events around
+    `reps` calls, and the bytes it must move at least: the passes over B x N x F floats each type makes."""
+    layer = model.constraint
+    B, N = x.shape[0], x.shape[1]
+    g = torch.Generator(device="cuda").manual_seed(2)
+    hr32, lr32 = layer._prepare(torch.randn(B, N, F, device="cuda", generator=g), x[..., :F])
+    dy = torch.randn(B, N, F, device="cuda", generator=g)
+    src = model._constraint_cell(hr32)
+    layer._backward(dy, hr32, lr32, src, True)
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        layer._backward(dy, hr32, lr32, src, True)
+    e1.record()
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1) / reps
+    # additive: dy (sums) + dy (rows) + d_hr + d_lr; multiplicative: + hr, lr (means) + hr (sums); softmax: dy, hr, lr, d_hr, d_lr
+    passes = {"additive": 4, "multiplicative": 7, "softmax": 5}[layer.constraint_type]
+    nbytes = passes * B * N * F * 4
+    return {"ms": round(ms, 4), "min_bytes": nbytes, "achieved_gb_s": round(nbytes / (ms * 1e-3) / 1e9, 1)}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--grid", default="1deg", choices=["1deg", "2deg", "10deg"])
@@ -44,6 +70,7 @@ def main():
     ap.add_argument("--aux-dim", type=int, default=24)
     ap.add_argument("--num-blocks", type=int, default=9)
     ap.add_argument("--width", type=int, default=None, help="node / edge / hidden / decoder width (default: the model's 256 / 128)")
+    ap.add_argument("--constraint-type", default="none", choices=["none", "additive", "multiplicative", "softmax"])
     a = ap.parse_args()
     import __graft_entry__ as ge
 
@@ -57,7 +84,7 @@ def main():
     if a.width is not None:
         dims.update(node_dim=a.width, edge_dim=a.width, hidden_dim_processor_node=a.width, hidden_dim_processor_edge=a.width,
                     hidden_dim_decoder=a.width)  # fmt: skip
-    model = GraphWeatherForecaster(ll, train_precision=a.train_precision, **dims).cuda().train()
+    model = GraphWeatherForecaster(ll, train_precision=a.train_precision, constraint_type=a.constraint_type, **dims).cuda().train()
     F = a.feature_dim
     crit = NormalizedMSELoss([1.0] * F, ll, normalize=True)
     opt = torch.optim.SGD(model.parameters(), lr=1e-3)
@@ -94,8 +121,10 @@ def main():
     plan.timing_enable(False)
     phases = {k: round(v[1], 3) for k, v in tags.items() if k.startswith("train_") or k == "const"}
     plan.status()
+    cbwd = constraint_backward_time(model, x, F) if a.constraint_type != "none" else None
     print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "train_precision": a.train_precision, "grid": a.grid, "batch": a.batch,
-                      "dims": dims, "n_params": sum(q.numel() for q in model.parameters()),
+                      "dims": dims, "constraint_type": a.constraint_type, "constraint_backward": cbwd,
+                      "n_params": sum(q.numel() for q in model.parameters()),
                       "ms_per_step": ms, "samples_per_s": a.batch / (ms * 1e-3), "phase_ms": phases,
                       "phase_launches": {k: v[0] for k, v in tags.items() if k.startswith("train_")},
                       "torch_peak_alloc_gib": round(peak / 2**30, 2), "device_mem_used_gib": round((total - free) / 2**30, 1),
