@@ -41,6 +41,7 @@ _SIGNATURES = {
     "gw_abi_version": (ctypes.c_int, []),
     "gw_last_error": (ctypes.c_char_p, []),
     "gw_plan_create": (ctypes.c_int, [ctypes.POINTER(GwDims), ctypes.POINTER(_vp)]),
+    "gw_plan_create_train": (ctypes.c_int, [ctypes.POINTER(GwDims), ctypes.POINTER(_vp)]),
     "gw_plan_destroy": (ctypes.c_int, [_vp]),
     "gw_plan_device_bytes": (_i64, [_vp]),
     "gw_plan_set_encoder_graph": (ctypes.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp]),
@@ -74,6 +75,7 @@ _SIGNATURES = {
     "gw_normalized_mse_loss_grad": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _vp, ctypes.c_float, _vp, _vp]),
     "gw_train_forward": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp]),
     "gw_train_backward": (ctypes.c_int, [_vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
+    "gw_train_peak_bytes": (_i64, [_vp]),
     "gw_launch_count": (_i64, []),
     "gw_launch_count_reset": (None, []),
 }
@@ -137,9 +139,10 @@ def launch_count_reset() -> None:
 
 
 class Plan:
-    """Owns one gw_plan on one CUDA device."""
+    """Owns one gw_plan on one CUDA device.  train_only: a training-only plan (gw_plan_create_train), whose training step is the
+    bounded-memory one and which runs no inference forward."""
 
-    def __init__(self, device, **dims):
+    def __init__(self, device, train_only: bool = False, **dims):
         self.lib = load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -147,9 +150,11 @@ class Plan:
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.dims = GwDims(**dims)
+        self.train_only = bool(train_only)
         self.handle = _vp()
+        create = self.lib.gw_plan_create_train if self.train_only else self.lib.gw_plan_create
         with torch.cuda.device(self.device):
-            _check(self.lib.gw_plan_create(ctypes.byref(self.dims), ctypes.byref(self.handle)))
+            _check(create(ctypes.byref(self.dims), ctypes.byref(self.handle)))
         self._keep = []
 
     def close(self):
@@ -165,6 +170,10 @@ class Plan:
 
     def device_bytes(self) -> int:
         return int(self.lib.gw_plan_device_bytes(self.handle))
+
+    def train_peak_bytes(self) -> int:
+        """High-water mark of the training step's working allocations over the last train_forward + train_backward."""
+        return int(self.lib.gw_train_peak_bytes(self.handle))
 
     def _dev(self, arr, dtype):
         t = torch.as_tensor(arr).to(dtype=dtype).contiguous().to(self.device)

@@ -100,6 +100,8 @@ struct TrainState;
 
 struct gw_plan {
   gw::TrainState* train = nullptr;  // training step state (gw_train.inl), created on first use
+  bool train_only = false;          // gw_plan_create_train: graphs, weights and the bounded-memory (chunked) training step only
+  int train_chunk_pts = 0;          // GW_B200_TRAIN_CHUNK: points per chunk of that step (0: from the shapes, gw_train.inl)
   gw_dims d;
   int device = 0;
   int n_in_cur = 0;
@@ -1081,9 +1083,11 @@ static int encoder_degree(gw_plan* p, cudaStream_t st) {
 #include "gw_train.inl"
 namespace gw {
 
-enum { NEED_ENC = 1, NEED_PROC = 2, NEED_DEC = 4 };
+enum { NEED_ENC = 1, NEED_PROC = 2, NEED_DEC = 4, NEED_INFER = 8 };
 static int check_ready(gw_plan* p, int batch, int need) {
   GW_CHECK(p != nullptr, "null plan");
+  if (need & NEED_INFER)
+    GW_CHECK(!p->train_only, "this plan was made by gw_plan_create_train: it holds no inference scratch (use a gw_plan_create plan to run forwards)");
   if (need & NEED_ENC) GW_CHECK(p->have_enc && p->have_lat && p->w_enc, "encoder stage needs the encoder + latent graphs and encoder.* weights");
   if (need & NEED_PROC) GW_CHECK(p->w_proc, "processor stage needs processor.* weights");
   if (need & NEED_DEC) GW_CHECK(p->have_dec && p->w_dec, "decoder stage needs the decoder graph and decoder.* weights");
@@ -1104,7 +1108,46 @@ const char* gw_last_error(void) { return gw::g_err.c_str(); }
 int64_t gw_launch_count(void) { return gw::g_launches; }
 void gw_launch_count_reset(void) { gw::g_launches = 0; }
 
-int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) {
+// inference scratch and weight constants of a plan (gw_plan_create; a training-only plan holds none of it)
+static int alloc_inference_scratch(gw_plan* p, size_t chunk) {
+  const gw_dims& d = p->d;
+  const bool tc = d.precision != GW_PREC_FP32_SIMT;
+  const size_t Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, Hn = d.hidden_node;
+  const size_t max_hid = std::max({Dn, De, He, Hn, (size_t)d.hidden_dec, (size_t)d.out_dim});
+  const size_t max_rows = std::max({(size_t)d.n_in, (size_t)d.n_out, (size_t)d.n_mesh, (size_t)d.n_lat_edges, (size_t)d.n_dec_edges});
+  const size_t n_io = std::max((size_t)d.n_in, (size_t)d.n_out);
+  const size_t dec_tiles = ((size_t)d.n_dec_edges + 127) / 128, lat_tiles = ((size_t)d.n_lat_edges + 127) / 128;
+  const size_t B = d.max_batch;
+  int rc = 0;
+  rc |= p->e_enc.alloc((size_t)d.n_in * De) | p->xm0.alloc((size_t)d.n_mesh * Dn) | p->C1_enc.alloc((size_t)d.n_in * He);
+  rc |= p->e_lat.alloc((size_t)d.n_lat_edges * De) | p->e_dec.alloc((size_t)d.n_dec_edges * De);
+  rc |= p->E1_dec.alloc((size_t)d.n_dec_edges * He) | p->tmpP.alloc((size_t)d.n_mesh * He);
+  if (tc && d.n_out > 0 && d.n_dec_edges > 0) rc |= p->S_dec.alloc((size_t)d.n_out * De);
+  {  // hidden-activation ping-pong of run_mlp: every stage on the CUDA-core path, the one-off constant precompute
+     // (one sample's worth of rows) on the tensor-core path
+    size_t pp = (tc ? 1 : chunk) * max_rows * max_hid;
+    if (!tc && B * std::max((size_t)d.n_lat_edges, (size_t)d.n_mesh) > chunk * max_rows) pp = B * max_rows * max_hid;
+    rc |= p->bufA.alloc(pp) | p->bufB.alloc(pp);
+  }
+  rc |= p->rows_n.alloc(chunk * n_io * Dn);
+  rc |= p->rows_e.alloc(chunk * (tc ? (size_t)d.n_in : std::max((size_t)d.n_in, (size_t)d.n_dec_edges)) * De);
+  rc |= p->xbuf0.alloc(B * d.n_mesh * Dn) | p->xbuf1.alloc(B * d.n_mesh * Dn);
+  rc |= p->ebuf0.alloc(B * d.n_lat_edges * De) | p->ebuf1.alloc(B * d.n_lat_edges * De);
+  rc |= p->P.alloc(B * d.n_mesh * 2 * He);
+  rc |= p->agg_mesh.alloc(B * d.n_mesh * De);
+  if (tc && d.n_in > 0) {
+    p->enc_max_chunks = gw::seg_chunk_bound(d.n_mesh, d.n_in);
+    rc |= p->enc_chunk_seg.alloc(p->enc_max_chunks) | p->enc_chunk_j0.alloc(p->enc_max_chunks) | p->enc_seg_chunk0.alloc(d.n_mesh + 1);
+    rc |= p->enc_partial.alloc(chunk * (size_t)p->enc_max_chunks * 256);
+  }
+  if (tc) {
+    rc |= p->agg_grid.alloc(chunk * d.n_out * De);
+    rc |= p->seg_carry.alloc(std::max(chunk * dec_tiles, B * (lat_tiles + 1)) * 2048);  // [samples][tiles][8 row groups][256]
+  }
+  return rc;
+}
+
+static int plan_create(const gw_dims* dims, gw_plan** out_plan, bool train_only) {
   GW_CHECK(dims && out_plan, "null argument");
   const gw_dims& d = *dims;
   GW_CHECK(d.n_in >= 0 && d.n_out >= 0 && d.n_mesh > 0 && d.n_lat_edges >= 0 && d.n_dec_edges >= 0,
@@ -1133,6 +1176,7 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) {
   }
   gw_plan* p = new gw_plan();
   p->d = d;
+  p->train_only = train_only;
   // every failure after this point releases the plan and whatever it already holds
 #define GW_CUDA_P(expr)                                                          \
   do {                                                                           \
@@ -1153,7 +1197,7 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) {
   // the SM, so its per-sample scratch is three lat/lon-sized row buffers; the CUDA-core path also needs e' and the ping-pong.
   const bool tc = d.precision != GW_PREC_FP32_SIMT;
   const size_t n_io = std::max((size_t)d.n_in, (size_t)d.n_out);
-  const size_t dec_tiles = ((size_t)d.n_dec_edges + 127) / 128, lat_tiles = ((size_t)d.n_lat_edges + 127) / 128;
+  const size_t dec_tiles = ((size_t)d.n_dec_edges + 127) / 128;
   const size_t per_sample = tc ? (n_io * Dn + (size_t)d.n_in * De + (size_t)d.n_out * De + dec_tiles * 2048) * sizeof(float)
                                : (2 * max_rows * max_hid + std::max((size_t)d.n_in, (size_t)d.n_dec_edges) * De + n_io * Dn) * sizeof(float);
   size_t chunk = std::max<size_t>(1, std::min<size_t>(d.max_batch, (24ull << 30) / std::max<size_t>(per_sample, 1)));
@@ -1163,7 +1207,10 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) {
   }
   p->chunk = (int)chunk;
   p->fuse_seg = tc && !getenv("GW_TC3_NOSEG");  // diagnostics: GW_TC3_NOSEG=1 keeps the separate segment-sum kernels
-  const size_t B = d.max_batch;
+  if (const char* pts = getenv("GW_B200_TRAIN_CHUNK")) {  // test knob: many chunks of the bounded-memory training step on small grids
+    const long v = atol(pts);
+    if (v >= 1) p->train_chunk_pts = (int)std::min<long>(v, 1l << 30);
+  }
   int rc = 0;
   rc |= p->enc_mesh.alloc(d.n_in) | p->enc_perm.alloc(d.n_in) | p->enc_ptr.alloc(d.n_mesh + 1);
   rc |= p->enc_attr.alloc((size_t)d.n_in * d.enc_edge_attr_dim);
@@ -1172,31 +1219,7 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) {
   rc |= p->dec_src.alloc(d.n_dec_edges) | p->dec_ptr.alloc(d.n_out + 1) | p->dec_attr.alloc((size_t)d.n_dec_edges * 2);
   rc |= p->dec_dst.alloc(d.n_dec_edges) | p->deg_stats.alloc(2) | p->enc_deg.alloc(2) | p->bounds.alloc(gw::SL_COUNT);
   rc |= p->zeros_h3.alloc((size_t)d.n_mesh * d.in_dim);
-  rc |= p->e_enc.alloc((size_t)d.n_in * De) | p->xm0.alloc((size_t)d.n_mesh * Dn) | p->C1_enc.alloc((size_t)d.n_in * He);
-  rc |= p->e_lat.alloc((size_t)d.n_lat_edges * De) | p->e_dec.alloc((size_t)d.n_dec_edges * De);
-  rc |= p->E1_dec.alloc((size_t)d.n_dec_edges * He) | p->tmpP.alloc((size_t)d.n_mesh * He);
-  if (tc && d.n_out > 0 && d.n_dec_edges > 0) rc |= p->S_dec.alloc((size_t)d.n_out * De);
-  {  // hidden-activation ping-pong of run_mlp: every stage on the CUDA-core path, the one-off constant precompute
-     // (one sample's worth of rows) on the tensor-core path
-    size_t pp = (tc ? 1 : chunk) * max_rows * max_hid;
-    if (!tc && B * std::max((size_t)d.n_lat_edges, (size_t)d.n_mesh) > chunk * max_rows) pp = B * max_rows * max_hid;
-    rc |= p->bufA.alloc(pp) | p->bufB.alloc(pp);
-  }
-  rc |= p->rows_n.alloc(chunk * n_io * Dn);
-  rc |= p->rows_e.alloc(chunk * (tc ? (size_t)d.n_in : std::max((size_t)d.n_in, (size_t)d.n_dec_edges)) * De);
-  rc |= p->xbuf0.alloc(B * d.n_mesh * Dn) | p->xbuf1.alloc(B * d.n_mesh * Dn);
-  rc |= p->ebuf0.alloc(B * d.n_lat_edges * De) | p->ebuf1.alloc(B * d.n_lat_edges * De);
-  rc |= p->P.alloc(B * d.n_mesh * 2 * He);
-  rc |= p->agg_mesh.alloc(B * d.n_mesh * De);
-  if (tc && d.n_in > 0) {
-    p->enc_max_chunks = gw::seg_chunk_bound(d.n_mesh, d.n_in);
-    rc |= p->enc_chunk_seg.alloc(p->enc_max_chunks) | p->enc_chunk_j0.alloc(p->enc_max_chunks) | p->enc_seg_chunk0.alloc(d.n_mesh + 1);
-    rc |= p->enc_partial.alloc(chunk * (size_t)p->enc_max_chunks * 256);
-  }
-  if (tc) {
-    rc |= p->agg_grid.alloc(chunk * d.n_out * De);
-    rc |= p->seg_carry.alloc(std::max(chunk * dec_tiles, B * (lat_tiles + 1)) * 2048);  // [samples][tiles][8 row groups][256]
-  }
+  if (!train_only) rc |= alloc_inference_scratch(p, chunk);
   if (rc) {
     std::string keep = gw::g_err;
     gw_plan_destroy(p);
@@ -1214,6 +1237,9 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) {
   return 0;
 }
 
+int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) { return plan_create(dims, out_plan, false); }
+int gw_plan_create_train(const gw_dims* dims, gw_plan** out_plan) { return plan_create(dims, out_plan, true); }
+
 int gw_plan_destroy(gw_plan* p) {
   if (!p) return 0;
   for (DevBuf<int32_t>* b : {&p->enc_mesh, &p->enc_perm, &p->enc_ptr, &p->lat_src, &p->lat_dst, &p->lat_ptr, &p->dec_src, &p->dec_ptr})
@@ -1230,6 +1256,7 @@ int gw_plan_destroy(gw_plan* p) {
     gw::tfree_all(p->train);
     p->train->wT.release(), p->train->gbuf.release(), p->train->lat_perm_src.release(), p->train->lat_ptr_src.release();
     p->train->dec_perm_src.release(), p->train->dec_ptr_src.release(), p->train->iota.release(), p->train->sort_ws.release();
+    p->train->enc_slot_sorted.release(), p->train->dec_cperm.release(), p->train->dec_cptr.release();
     p->train->bslots.release(), p->train->wg_ws.release();
     for (auto& kv : p->train->images) kv.second.img.release(), kv.second.amax.release();
     delete p->train;
@@ -1267,7 +1294,7 @@ int gw_plan_set_encoder_graph(gw_plan* p, int32_t n_in, const int32_t* enc_mesh,
   p->n_in_cur = n_in;
   p->have_enc = true;
   GW_TRY(gw::encoder_degree(p, st));
-  if (p->w_enc) GW_TRY(gw::precompute_encoder_constants(p, st));  // per-call graphs (assimilator_encoder.py:118)
+  if (p->w_enc && !p->train_only) GW_TRY(gw::precompute_encoder_constants(p, st));  // per-call graphs (assimilator_encoder.py:118)
   return 0;
 }
 
@@ -1311,7 +1338,7 @@ int gw_plan_build_obs_graph(gw_plan* p, const float* lat_lon_heights, int32_t n_
   p->n_in_cur = n_obs;
   p->have_enc = true;
   GW_TRY(gw::encoder_degree(p, st));
-  if (p->w_enc) GW_TRY(gw::precompute_encoder_constants(p, st));  // per-call graphs (assimilator_encoder.py:118)
+  if (p->w_enc && !p->train_only) GW_TRY(gw::precompute_encoder_constants(p, st));  // per-call graphs (assimilator_encoder.py:118)
   return 0;
 }
 
@@ -1363,19 +1390,20 @@ int gw_plan_set_weights(gw_plan* p, const gw_param* params, int32_t n, void* str
     off += (cnt + 63) / 64 * 64;
   }
   GW_TRY(gw::bind_all(p));
+  if (p->train_only) return 0;  // (the training step packs its own weight images and computes the constants it needs)
   if (gw::is_tc(p)) GW_TRY(gw::pack_tc_weights(p, st));
   GW_TRY(gw::precompute_constants(p, st));
   return 0;
 }
 
 int gw_encoder_forward(gw_plan* p, const float* features, float* x_out, int32_t batch, void* stream) {
-  GW_TRY(gw::check_ready(p, batch, gw::NEED_ENC));
+  GW_TRY(gw::check_ready(p, batch, gw::NEED_ENC | gw::NEED_INFER));
   GW_CHECK(features && x_out, "null argument");
   return gw::stage_encoder(p, features, x_out, gw::sl(p, gw::SL_XOUT), batch, (cudaStream_t)stream);
 }
 
 int gw_processor_forward(gw_plan* p, const float* x_in, float* x_out, int32_t batch, void* stream) {
-  GW_TRY(gw::check_ready(p, batch, gw::NEED_PROC));
+  GW_TRY(gw::check_ready(p, batch, gw::NEED_PROC | gw::NEED_INFER));
   GW_CHECK(x_in && x_out, "null argument");
   GW_CHECK(p->have_lat && p->w_enc, "gw_processor_forward uses the plan's latent graph and encoded latent edges; "
                                     "use gw_processor_forward_graph for caller-supplied graphs");
@@ -1386,7 +1414,7 @@ int gw_processor_forward(gw_plan* p, const float* x_in, float* x_out, int32_t ba
 
 int gw_processor_forward_graph(gw_plan* p, const float* x_in, float* x_out, const float* edge_attr, int32_t n_nodes,
                                int32_t n_edges, const int32_t* src, const int32_t* dst, const int32_t* ptr, void* stream) {
-  GW_TRY(gw::check_ready(p, 1, gw::NEED_PROC));
+  GW_TRY(gw::check_ready(p, 1, gw::NEED_PROC | gw::NEED_INFER));
   GW_CHECK(x_in && x_out && edge_attr && src && dst && ptr, "null argument");
   GW_CHECK(n_nodes >= 1 && (size_t)n_nodes <= (size_t)p->d.max_batch * p->d.n_mesh, "n_nodes exceeds max_batch*n_mesh");
   GW_CHECK(n_edges >= 1 && (size_t)n_edges <= (size_t)p->d.max_batch * p->d.n_lat_edges, "n_edges exceeds max_batch*n_lat_edges");
@@ -1401,7 +1429,7 @@ int gw_processor_forward_graph(gw_plan* p, const float* x_in, float* x_out, cons
 }
 
 int gw_decoder_forward(gw_plan* p, const float* x_in, const float* start, int32_t start_ld, float* out, int32_t batch, void* stream) {
-  GW_TRY(gw::check_ready(p, batch, gw::NEED_DEC));
+  GW_TRY(gw::check_ready(p, batch, gw::NEED_DEC | gw::NEED_INFER));
   GW_CHECK(x_in && out, "null argument");
   GW_CHECK(p->d.residual_dim == 0 || (start && start_ld >= p->d.residual_dim), "start features required (decoder.py:93)");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1414,7 +1442,7 @@ int gw_forward(gw_plan* p, const float* features, float* out, int32_t batch, voi
 }
 
 int gw_forward_strided(gw_plan* p, const float* features, float* out, int32_t out_ld, int32_t batch, void* stream) {
-  GW_TRY(gw::check_ready(p, batch, gw::NEED_ENC | gw::NEED_PROC | gw::NEED_DEC));
+  GW_TRY(gw::check_ready(p, batch, gw::NEED_ENC | gw::NEED_PROC | gw::NEED_DEC | gw::NEED_INFER));
   GW_CHECK(features && out, "null argument");
   GW_CHECK(out_ld >= p->d.out_dim, "out_ld must be at least out_dim");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1449,6 +1477,8 @@ int gw_train_backward(gw_plan* p, const float* grad_out, float* grad_features, c
   return 0;
 }
 
+int64_t gw_train_peak_bytes(const gw_plan* p) { return (p && p->train) ? (int64_t)p->train->peak_bytes : 0; }
+
 int gw_plan_set_output_peers(gw_plan* p, int32_t mode, int32_t n, const int64_t* deltas_bytes) {
   GW_CHECK(p != nullptr, "null plan");
   GW_CHECK(mode == 0 || (mode == 1 && n == 1 && deltas_bytes) || (mode == 2 && n >= 1 && n <= 8 && deltas_bytes), "bad mode / count");
@@ -1459,6 +1489,7 @@ int gw_plan_set_output_peers(gw_plan* p, int32_t mode, int32_t n, const int64_t*
 
 int gw_latent_edge_features(gw_plan* p, float* edge_attr_out, void* stream) {
   GW_CHECK(p && edge_attr_out, "null argument");
+  GW_CHECK(!p->train_only, "this plan was made by gw_plan_create_train: it holds no encoded latent edges");
   GW_CHECK(p->w_enc && p->have_lat, "needs the latent graph and encoder.* weights");
   GW_CUDA(cudaMemcpyAsync(edge_attr_out, p->e_lat.p, p->e_lat.bytes(), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return 0;

@@ -30,8 +30,12 @@ cudaError_t launch_ln_bwd(const float* dy, int ld_dy, const float* z, int ld_z, 
 constexpr int LN_BWD_MAX_N = 1024;  // widest row launch_ln_bwd takes (rows of more than 256 columns run on a kernel of their own)
 cudaError_t launch_batch_reduce(const float* in, int ld_in, long long rows, int width, int batch, float* out, int ld_out, bool accumulate,
                                 cudaStream_t st);
+// idx_base: `in` holds the targets idx_base .. idx_base + src_rows - 1 only (a chunk of the training step's grid-sized stages)
 cudaError_t launch_gather_rows(const float* in, int ld_in, int src_rows, const int32_t* idx, long long rows, int width, int batch, float* out,
-                               int ld_out, bool accumulate, cudaStream_t st);
+                               int ld_out, bool accumulate, cudaStream_t st, int idx_base = 0);
+// rows through a permutation, per sample: gather (out row j = in row idx[j] of other_rows) or scatter (out row idx[j] of other_rows = in row j)
+cudaError_t launch_permute_rows(const float* in, int ld_in, const int32_t* idx, long long rows, int other_rows, int width, int batch, float* out,
+                                int ld_out, bool scatter, cudaStream_t st);
 cudaError_t launch_strided_add(const float* src, int ld_src, float* dst, int ld_dst, long long rows, int width, cudaStream_t st);
 cudaError_t launch_transpose(const float* W, int rows, int cols, float* WT, cudaStream_t st);
 int seg_chunk_bound(int n_seg, int n_rows);
@@ -41,8 +45,10 @@ cudaError_t launch_segsum_chunked(const float* base, int ld, const int32_t* ptr,
                                   float* out, int ldo, cudaStream_t st);
 cudaError_t launch_seg_carry(const float* carry, const int32_t* seg_dst, int rows, int seg_rows, int batch, float* out, int ldo,
                              cudaStream_t stream);
+// ptr_base: subtracted from every ptr entry (a CSR slice over a range of rows that starts at row ptr_base of the full table);
+// accumulate: out += the segment sums (a per-segment sum split over row ranges, added in the order of the calls)
 cudaError_t launch_segsum(const float* base, int ld, int width, const int32_t* ptr, const int32_t* perm, int src_rows,
-                          int rows, int batch, float* out, int ldo, cudaStream_t stream);
+                          int rows, int batch, float* out, int ldo, cudaStream_t stream, int ptr_base = 0, bool accumulate = false);
 
 // wgmma chain kernel (gw_tc3.cu)
 cudaError_t launch_chain_tc3(const TcChain& ch, cudaStream_t stream);

@@ -181,9 +181,10 @@ __global__ void __launch_bounds__(NT) gw_rowop_f32_kernel(const GemmOp op) {
 // encoder's lat/lon -> mesh aggregation, whose segments are very skewed (a polar cell collects thousands of points).
 __global__ void __launch_bounds__(64) gw_segsum_kernel(const float* __restrict__ base, int ld, int width,
                                                        const int32_t* __restrict__ ptr, const int32_t* __restrict__ perm,
-                                                       int src_rows, int rows, float* __restrict__ out, int ldo) {
+                                                       int src_rows, int rows, float* __restrict__ out, int ldo, int ptr_base,
+                                                       int accumulate) {
   const int i = blockIdx.x, b = blockIdx.y;
-  const int j0 = __ldg(ptr + i), j1 = __ldg(ptr + i + 1);
+  const int j0 = __ldg(ptr + i) - ptr_base, j1 = __ldg(ptr + i + 1) - ptr_base;
   for (int c = threadIdx.x * 4; c < width; c += 256) {
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int j = j0; j < j1; ++j) {
@@ -191,15 +192,20 @@ __global__ void __launch_bounds__(64) gw_segsum_kernel(const float* __restrict__
       const float4 t = __ldg(reinterpret_cast<const float4*>(base + ((size_t)b * src_rows + e) * ld + c));
       acc.x += t.x, acc.y += t.y, acc.z += t.z, acc.w += t.w;
     }
-    *reinterpret_cast<float4*>(out + ((size_t)b * rows + i) * ldo + c) = acc;
+    float4* o = reinterpret_cast<float4*>(out + ((size_t)b * rows + i) * ldo + c);
+    if (accumulate) {  // the segment's sum is added to what an earlier call left (a sum split over row ranges)
+      const float4 t = *o;
+      acc.x = t.x + acc.x, acc.y = t.y + acc.y, acc.z = t.z + acc.z, acc.w = t.w + acc.w;
+    }
+    *o = acc;
   }
 }
 
 cudaError_t launch_segsum(const float* base, int ld, int width, const int32_t* ptr, const int32_t* perm, int src_rows,
-                          int rows, int batch, float* out, int ldo, cudaStream_t stream) {
+                          int rows, int batch, float* out, int ldo, cudaStream_t stream, int ptr_base, bool accumulate) {
   if (rows <= 0 || batch <= 0) return cudaSuccess;
   if ((width & 3) || (ld & 3) || (ldo & 3)) return cudaErrorInvalidValue;
-  gw_segsum_kernel<<<dim3(rows, batch), 64, 0, stream>>>(base, ld, width, ptr, perm, src_rows, rows, out, ldo);
+  gw_segsum_kernel<<<dim3(rows, batch), 64, 0, stream>>>(base, ld, width, ptr, perm, src_rows, rows, out, ldo, ptr_base, accumulate ? 1 : 0);
   count_launch();
   return cudaGetLastError();
 }
@@ -560,16 +566,17 @@ cudaError_t launch_batch_reduce(const float* in, int ld_in, long long rows, int 
   count_launch();
   return cudaGetLastError();
 }
-// out[(b * rows + j), c] (+)= in[(b * src_rows + idx[j]), c]   (gradient of a per-target sum: every row receives its target's gradient)
+// out[(b * rows + j), c] (+)= in[(b * src_rows + idx[j] - idx_base), c]   (gradient of a per-target sum: every row receives its target's
+// gradient; idx_base: the first target of a table that holds a range of targets)
 __global__ void gw_gather_rows_kernel(const float* __restrict__ in, int ld_in, int src_rows, const int32_t* __restrict__ idx, long long rows, int width,
-                                      int batch, float* __restrict__ out, int ld_out, int accumulate) {
+                                      int batch, float* __restrict__ out, int ld_out, int accumulate, int idx_base) {
   const long long total = rows * batch * (width >> 2);
   const int q = width >> 2;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     const long long rj = e / q;
     const int c = (int)(e - rj * q) * 4;
     const long long b = rj / rows, j = rj - b * rows;
-    const float4 v = __ldg(reinterpret_cast<const float4*>(in + (b * src_rows + __ldg(idx + j)) * ld_in + c));
+    const float4 v = __ldg(reinterpret_cast<const float4*>(in + (b * src_rows + (__ldg(idx + j) - idx_base)) * ld_in + c));
     float4* o = reinterpret_cast<float4*>(out + rj * ld_out + c);
     if (accumulate) {
       float4 t = *o;
@@ -581,10 +588,34 @@ __global__ void gw_gather_rows_kernel(const float* __restrict__ in, int ld_in, i
   }
 }
 cudaError_t launch_gather_rows(const float* in, int ld_in, int src_rows, const int32_t* idx, long long rows, int width, int batch, float* out,
-                               int ld_out, bool accumulate, cudaStream_t st) {
+                               int ld_out, bool accumulate, cudaStream_t st, int idx_base) {
   if (rows <= 0 || batch <= 0) return cudaSuccess;
   if ((width & 3) || (ld_in & 3) || (ld_out & 3)) return cudaErrorInvalidValue;
-  gw_gather_rows_kernel<<<GRID_SMS * 8, 256, 0, st>>>(in, ld_in, src_rows, idx, rows, width, batch, out, ld_out, accumulate ? 1 : 0);
+  gw_gather_rows_kernel<<<GRID_SMS * 8, 256, 0, st>>>(in, ld_in, src_rows, idx, rows, width, batch, out, ld_out, accumulate ? 1 : 0, idx_base);
+  count_launch();
+  return cudaGetLastError();
+}
+// scatter = 0: out[(b * rows + j), c] = in[(b * other_rows + idx[j]), c]     (rows of a caller tensor picked through a permutation)
+// scatter = 1: out[(b * other_rows + idx[j]), c] = in[(b * rows + j), c]     (and written back through it)
+// Any width and stride (the 102 or 621 input features): one float per thread, 64-bit offsets throughout.
+__global__ void gw_permute_rows_kernel(const float* __restrict__ in, int ld_in, const int32_t* __restrict__ idx, long long rows, int other_rows,
+                                       int width, int batch, float* __restrict__ out, int ld_out, int scatter) {
+  const long long total = rows * batch * width;
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const long long rj = e / width;
+    const int c = (int)(e - rj * width);
+    const long long b = rj / rows, j = rj - b * rows;
+    const long long far = b * other_rows + __ldg(idx + j);
+    if (scatter)
+      out[far * ld_out + c] = __ldg(in + rj * ld_in + c);
+    else
+      out[rj * ld_out + c] = __ldg(in + far * ld_in + c);
+  }
+}
+cudaError_t launch_permute_rows(const float* in, int ld_in, const int32_t* idx, long long rows, int other_rows, int width, int batch, float* out,
+                                int ld_out, bool scatter, cudaStream_t st) {
+  if (rows <= 0 || batch <= 0 || width <= 0) return cudaSuccess;
+  gw_permute_rows_kernel<<<GRID_SMS * 8, 256, 0, st>>>(in, ld_in, idx, rows, other_rows, width, batch, out, ld_out, scatter ? 1 : 0);
   count_launch();
   return cudaGetLastError();
 }

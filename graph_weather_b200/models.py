@@ -161,10 +161,11 @@ class _Engine:
     """Creates the plan lazily on the device of the first input, uploads graphs once and weights whenever a parameter
     changed (in-place optimiser steps and load_state_dict bump tensor versions; .to() changes data pointers)."""
 
-    def __init__(self, dims: dict, precision: str):
+    def __init__(self, dims: dict, precision: str, train_only: bool = False):
         _validate_precision(precision, dims)
         self.dims = dict(dims)
         self.precision = precision
+        self.train_only = train_only  # training-only plans (gw_plan_create_train): the bounded-memory training step
         self.resolved_precision: Optional[str] = None
         self.plan: Optional[_capi.Plan] = None
         self.graph_uploaders = []  # callables(plan)
@@ -178,7 +179,7 @@ class _Engine:
         d["max_batch"] = int(max_batch)
         self.resolved_precision = resolve_precision(self.precision, self.dims, device)
         d["precision"] = _capi.PRECISIONS[self.resolved_precision]
-        self.plan = _capi.Plan(device, **d)
+        self.plan = _capi.Plan(device, train_only=self.train_only, **d)
         self.generation += 1
         for up in self.graph_uploaders:
             up(self.plan)
@@ -277,7 +278,7 @@ class Encoder(nn.Module):
                  hidden_layers_processor_edge=2, mlp_norm_type="LayerNorm", use_checkpointing: bool = False,
                  efficient_batching: bool = False, precision: str = "auto"):  # fmt: skip
         super().__init__()
-        self.use_checkpointing = use_checkpointing  # accepted for API parity; forward-only path keeps no activations
+        self.use_checkpointing = use_checkpointing  # accepted for API parity; GraphWeatherForecaster(use_checkpointing=True) selects its bounded-memory training step
         self.efficient_batching = efficient_batching
         self.output_dim = output_dim
         self.num_latlons = len(lat_lons)
@@ -614,6 +615,7 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
         self.feature_dim = feature_dim
         self.constraint_type = constraint_type
         self.use_thermalizer = use_thermalizer
+        self.use_checkpointing = use_checkpointing
         if output_dim is None:
             output_dim = self.feature_dim
         self.output_dim = output_dim
@@ -686,9 +688,12 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
 
     def _training_engine(self):
         """The plan the training step runs on, of precision `train_precision` (created on first use; the inference engine stays
-        as it is).  A tensor-core training precision needs an sm_90 device: elsewhere the first training forward raises."""
+        as it is).  A tensor-core training precision needs an sm_90 device: elsewhere the first training forward raises.
+        use_checkpointing=True (forecast.py:81): a training-only plan, whose step keeps only the mesh-sized activations and
+        recomputes the grid-sized stages chunk by chunk in the backward -- its working memory does not grow with the grid beyond
+        one chunk (the 0.25 degree grid trains on one 80 GB card); the taped step (the default) is faster where it fits."""
         if getattr(self, "_train_engine", None) is None:
-            eng = _Engine(self._engine.dims, self.train_precision)
+            eng = _Engine(self._engine.dims, self.train_precision, train_only=bool(self.use_checkpointing))
             eng.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
             self.__dict__["_train_engine"] = eng
         return self._train_engine

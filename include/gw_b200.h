@@ -69,6 +69,16 @@ const char* gw_last_error(void);
  * (forecast.py:129-170, analysis.py:96-134).  Allocates scratch for dims->max_batch samples on the current device. */
 int gw_plan_create(const gw_dims* dims, gw_plan** out_plan);
 int gw_plan_destroy(gw_plan* plan);
+/* A plan for training only (GraphWeatherForecaster(use_checkpointing=True)): graphs, weights and the training state, none of
+ * the inference scratch, packed inference weights or weight constants.  gw_plan_set_weights on it binds the weights only;
+ * gw_forward, gw_forward_strided, the stage entry points and gw_latent_edge_features on it fail.  Its training step is the
+ * bounded-memory one: gw_train_forward keeps only the mesh-sized activations and the output, and gw_train_backward recomputes
+ * the grid-sized stages (the encoder's lat/lon side, the decoder) chunk by chunk with the forward's own ops, releasing each
+ * chunk's temporaries before the next.  Its peak working memory grows with the grid by at most one chunk.  Chunks hold a fixed
+ * working-set budget divided by the batch, chosen from the shapes alone (never from free device memory): encoder chunks are whole
+ * mesh slots, decoder chunks runs of consecutive points.  The forward equals the taped step's bit for bit in GW_PREC_FP32_SIMT and
+ * GW_PREC_BF16_TC (GW_PREC_FP32_TC scales each chunk's operands from the chunk); gradients equal it up to fp32 summation order. */
+int gw_plan_create_train(const gw_dims* dims, gw_plan** out_plan);
 /* bytes of device memory the plan holds (scratch + packed weights + constants) */
 int64_t gw_plan_device_bytes(const gw_plan* plan);
 
@@ -133,6 +143,9 @@ int gw_forward_strided(gw_plan* plan, const float* features, float* out, int32_t
  * train_dgrad, train_wgrad, train_pack, train_other split a step (gw_timing_read). */
 int gw_train_forward(gw_plan* plan, const float* features, float* out, int32_t batch, void* stream);
 int gw_train_backward(gw_plan* plan, const float* grad_out, float* grad_features, const gw_param* grads, int32_t n, void* stream);
+/* High-water mark, in bytes, of the training step's stream-ordered working allocations over the last gw_train_forward and the
+ * gw_train_backward after it (0 before the first step).  It depends on the shapes only, unlike device-wide figures on a shared card. */
+int64_t gw_train_peak_bytes(const gw_plan* plan);
 
 /* Multi-GPU loss boundary fused into the forecast's last chain (SURVEY.md 8(e): the one gather of the outputs).  After this call
  * every gw_forward / gw_forward_strided / gw_decoder_forward stores its `out` rows, as the tiles leave the tensor cores, into

@@ -1,14 +1,19 @@
 """Times one training step (forward with tape + NormalizedMSELoss + backward + SGD update) of GraphWeatherForecaster.
-    python tools/train_step_bench.py [--grid 1deg|2deg|10deg] [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16]
+    python tools/train_step_bench.py [--grid 0.25deg|1deg|2deg|10deg] [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16]
                                      [--feature-dim F] [--aux-dim A] [--num-blocks NB] [--width W]
-                                     [--constraint-type none|additive|multiplicative|softmax]
+                                     [--constraint-type none|additive|multiplicative|softmax] [--use-checkpointing] [--fit-batch]
 The model defaults to the README's 78 + 24 features, 9 blocks, 256-wide.  The reference's ERA5 training scripts:
     train/run_fulll.py  --feature-dim 597 --aux-dim 24 --num-blocks 6 (1-degree grid)
     train/run.py        --feature-dim 605 --aux-dim 40 --num-blocks 6 --width 1024 --grid 2deg
 (--width sets the node / edge / hidden / decoder widths together.)
 Prints one JSON line: ms/step, samples/s, the device time of the step's phases (libgwb200 timing tags train_*; one extra timed
 step after the measured ones, since the per-launch events add a little host work), peak device memory, and the card name and
-power limit read in the same run.  With --constraint-type the step includes PhysicalConstraintLayer; the constraint backward
+power limit read in the same run.  --use-checkpointing runs the bounded-memory step (a training-only plan; 0.25deg is the 721 x 1440
+grid bench.py uses).  Every run reports train_peak_bytes (the step's working allocations, gw_train_peak_bytes) and the plan's
+device_bytes.  --fit-batch: the largest batch whose step should fit on the card, from the device bytes the step needs at
+batches 1 and 2 (train_peak_bytes + plan bytes + torch's reserved peak, each linear in the batch), confirmed by one run at that
+batch in a fresh process.
+With --constraint-type the step includes PhysicalConstraintLayer; the constraint backward
 (gw_constraint_backward, no timing tag of the plan) is also timed on its own with CUDA events around it, on the step's shapes."""
 import argparse
 import json
@@ -62,7 +67,7 @@ def constraint_backward_time(model, x, F, reps=20):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--grid", default="1deg", choices=["1deg", "2deg", "10deg"])
+    ap.add_argument("--grid", default="1deg", choices=["0.25deg", "1deg", "2deg", "10deg"])
     ap.add_argument("--batch", type=int, default=2)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--train-precision", default="fp32_simt", choices=["fp32_simt", "fp32", "bf16"])
@@ -71,46 +76,76 @@ def main():
     ap.add_argument("--num-blocks", type=int, default=9)
     ap.add_argument("--width", type=int, default=None, help="node / edge / hidden / decoder width (default: the model's 256 / 128)")
     ap.add_argument("--constraint-type", default="none", choices=["none", "additive", "multiplicative", "softmax"])
+    ap.add_argument("--use-checkpointing", action="store_true", help="the bounded-memory training step (training-only plan)")
+    ap.add_argument("--fit-batch", action="store_true", help="report the largest batch that should fit, confirmed by one run")
     a = ap.parse_args()
     import __graft_entry__ as ge
 
     ge.build()
     from graph_weather_b200 import GraphWeatherForecaster, NormalizedMSELoss
 
-    step = {"1deg": 1, "2deg": 2, "10deg": 10}[a.grid]
-    ll = [(float(lat), float(lon)) for lat in range(-90, 90, step) for lon in range(0, 360, step)]
+    if a.grid == "0.25deg":
+        import numpy as np
+
+        ll = [(float(lat), float(lon)) for lat in np.linspace(-90.0, 90.0, 721) for lon in np.arange(0.0, 360.0, 0.25)]
+    else:
+        step = {"1deg": 1, "2deg": 2, "10deg": 10}[a.grid]
+        ll = [(float(lat), float(lon)) for lat in range(-90, 90, step) for lon in range(0, 360, step)]
     torch.manual_seed(0)
     dims = dict(feature_dim=a.feature_dim, aux_dim=a.aux_dim, num_blocks=a.num_blocks)
     if a.width is not None:
         dims.update(node_dim=a.width, edge_dim=a.width, hidden_dim_processor_node=a.width, hidden_dim_processor_edge=a.width,
                     hidden_dim_decoder=a.width)  # fmt: skip
-    model = GraphWeatherForecaster(ll, train_precision=a.train_precision, constraint_type=a.constraint_type, **dims).cuda().train()
+    model = GraphWeatherForecaster(ll, train_precision=a.train_precision, constraint_type=a.constraint_type, use_checkpointing=a.use_checkpointing,
+                                   **dims).cuda().train()  # fmt: skip
     F = a.feature_dim
     crit = NormalizedMSELoss([1.0] * F, ll, normalize=True)
     opt = torch.optim.SGD(model.parameters(), lr=1e-3)
-    x = torch.randn(a.batch, len(ll), F + a.aux_dim, device="cuda")
-    y = torch.randn(a.batch, len(ll), F, device="cuda")
-    losses = []
 
-    def one():
-        opt.zero_grad(set_to_none=True)
-        loss = crit(model(x), y)
-        loss.backward()
-        opt.step()
-        return loss
+    def measure(batch, steps):
+        """(ms/step, losses, torch peak bytes, train_peak_bytes, plan device_bytes, step function, inputs) of `steps` timed steps."""
+        x = torch.randn(batch, len(ll), F + a.aux_dim, device="cuda")
+        y = torch.randn(batch, len(ll), F, device="cuda")
 
-    for _ in range(2):
-        one()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.reset_peak_memory_stats()
-    e0.record()
-    for _ in range(a.steps):
-        losses.append(one())
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / a.steps
-    peak = torch.cuda.max_memory_allocated()
+        def one():
+            opt.zero_grad(set_to_none=True)
+            loss = crit(model(x), y)
+            loss.backward()
+            opt.step()
+            return loss
+
+        for _ in range(2):
+            one()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.reset_peak_memory_stats()
+        losses = []
+        e0.record()
+        for _ in range(steps):
+            losses.append(one())
+        e1.record()
+        torch.cuda.synchronize()
+        plan = model._train_engine.plan
+        return e0.elapsed_time(e1) / steps, losses, torch.cuda.max_memory_allocated(), plan.train_peak_bytes(), plan.device_bytes(), one, x
+
+    if a.fit_batch:
+        need = {}
+        for b in (1, 2):
+            _, _, _, trp, pb, _, _ = measure(b, 1)
+            need[b] = torch.cuda.max_memory_reserved() + trp + pb
+        per = need[2] - need[1]
+        total = torch.cuda.mem_get_info()[1]
+        # a tenth of the card for the CUDA context and the allocators' slack (the stream-ordered pool holds more than its live bytes)
+        bfit = max(1, int((0.9 * total - (need[1] - per)) // per))
+        # the confirming run is a fresh process: this one's allocators still cache the blocks of batches 1 and 2
+        argv = [v for v in sys.argv[1:] if v != "--fit-batch"] + ["--batch", str(bfit)]
+        r = subprocess.run([sys.executable, os.path.abspath(__file__), *argv], capture_output=True, text=True)
+        lines = [v for v in r.stdout.splitlines() if v.startswith("{")]
+        res = json.loads(lines[-1]) if r.returncode == 0 and lines else {"failed": r.stderr[-2000:]}
+        res["fit_batch"] = {"need_bytes_b1": need[1], "need_bytes_b2": need[2], "card_bytes": total, "batch": bfit}
+        print(json.dumps(res))
+        return
+    ms, losses, peak, train_peak, plan_bytes, one, x = measure(a.batch, a.steps)
     free, total = torch.cuda.mem_get_info()
     # per-phase device time of one more step (the plan's stream-ordered tape allocations are outside torch's allocator: the
     # device-wide figure is reported too)
@@ -123,6 +158,8 @@ def main():
     plan.status()
     cbwd = constraint_backward_time(model, x, F) if a.constraint_type != "none" else None
     print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "train_precision": a.train_precision, "grid": a.grid, "batch": a.batch,
+                      "use_checkpointing": a.use_checkpointing, "train_peak_gib": round(train_peak / 2**30, 3),
+                      "plan_device_gib": round(plan_bytes / 2**30, 3),
                       "dims": dims, "constraint_type": a.constraint_type, "constraint_backward": cbwd,
                       "n_params": sum(q.numel() for q in model.parameters()),
                       "ms_per_step": ms, "samples_per_s": a.batch / (ms * 1e-3), "phase_ms": phases,
