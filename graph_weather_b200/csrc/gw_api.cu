@@ -62,7 +62,7 @@ struct Mlp {  // views into the plan-owned weight buffer; Linear l: W[l] [out_l,
   const float* ln_b = nullptr;
   // magnitudes (filled by pack_tc_weights; tensor-core chains only): max |b[l]|, and the bound of the LayerNorm'd row
   std::vector<float> bmax;
-  float ln_bound = 0.f;  // sqrt(out) * max|gamma| + max|beta|
+  float ln_bound = 0.f;  // tc_ln_bound of the LayerNorm
 };
 
 template <class T>
@@ -133,8 +133,7 @@ struct gw_plan {
   DevBuf<float> P;            // [max_batch*n_mesh, 2*He]       per-node layer-1 products [W1s x | W1d x]
   size_t total_bytes = 0;
   // tensor-core path: packed weight images (GMMA operand layout) and their descriptors
-  struct TcW { const void* p = nullptr; int K = 0, N = 0, N32 = 0, n_valid = 0; float winv = 1.f; float gain = 0.f; };  // gain = K * max|W|: |A.W^T| <= gain * max|A|
-  struct TcMlp { TcW w0, w0b, w0c, w1, w2; };  // w0*: slices of the first Linear as each chain needs them
+  struct TcMlp { TcWeights w0, w0b, w0c, w1, w2; };  // w0*: slices of the first Linear as each chain needs them
   DevBuf<unsigned char> tc_packed;
   DevBuf<float> tc_absmax;
   long long* trace_buf = nullptr;   // debug: device buffer [8][1024][2] handed to the next chain launched under trace_tag
@@ -299,7 +298,7 @@ static int run_chain(gw_plan* p, TcChain& ch, cudaStream_t st) {
 static bool is_tc(const gw_plan* p) { return p->d.precision != GW_PREC_FP32_SIMT; }
 
 // layer = Linear `w` (+ bias b[l] of MLP m when l >= 0) (+ ReLU); magnitudes for the operand-range ladder travel along
-static TcLayer tc_layer(const gw_plan::TcW& w, const Mlp* m, int l, bool relu, bool feeds) {
+static TcLayer tc_layer(const TcWeights& w, const Mlp* m, int l, bool relu, bool feeds) {
   TcLayer L;
   L.Wp = w.p, L.K = w.K, L.N = w.N, L.N32 = w.N32, L.n_valid = w.n_valid, L.wscale_inv = w.winv;
   L.bias = (m && l >= 0) ? m->b[l] : nullptr, L.relu = relu ? 1 : 0, L.feeds_next = feeds ? 1 : 0;
@@ -442,9 +441,9 @@ static int pack_tc_weights(gw_plan* p, cudaStream_t st) {
   const gw_dims& d = p->d;
   const int Dn = d.node_dim, De = d.edge_dim;
   const int parts = (d.precision == GW_PREC_FP32_TC) ? 2 : 1;
-  struct Req { const float* W; int ldw, K, N; gw_plan::TcW* out; };
+  struct Req { const float* W; int ldw, K, N; TcWeights* out; };
   std::vector<Req> reqs;
-  auto want = [&](const float* W, int ldw, int K, int N, gw_plan::TcW* out) { reqs.push_back({W, ldw, K, N, out}); };
+  auto want = [&](const float* W, int ldw, int K, int N, TcWeights* out) { reqs.push_back({W, ldw, K, N, out}); };
   auto tail = [&](const Mlp& m, gw_plan::TcMlp& t) {
     want(m.W[1], m.in[1], m.in[1], m.out[1], &t.w1);
     want(m.W[2], m.in[2], m.in[2], m.out[2], &t.w2);
@@ -509,26 +508,16 @@ static int pack_tc_weights(gw_plan* p, cudaStream_t st) {
   GW_CUDA(cudaStreamSynchronize(st));
   for (size_t i = 0; i < nv; ++i) {
     const VReq& r = vreqs[i];
-    const float a = amax[n + i];
-    if (r.what == 0) r.m->bmax[r.l] = a;
-    else if (r.what == 1) r.m->ln_bound += std::sqrt((float)r.n) * a;
-    else r.m->ln_bound += a;
+    if (r.what == 0) r.m->bmax[r.l] = amax[n + i];
+    else if (r.what == 1) r.m->ln_bound = tc_ln_bound(r.n, amax[n + i], amax[n + i + 1]);  // (beta's entry follows gamma's)
   }
   if (p->tc_packed.n != total) GW_TRY(p->tc_packed.alloc(total));
   size_t off = 0;
   for (size_t i = 0; i < n; ++i) {
-    const float scale = tc_weight_scale(amax[i], parts);
-    void* dst = p->tc_packed.p + off;
-    const size_t img = (tc_packed_bytes(reqs[i].K, reqs[i].N, parts) + 1023) / 1024 * 1024;
-    GW_CUDA(launch_pack_weights(reqs[i].W, reqs[i].ldw, reqs[i].K, reqs[i].N, scale, parts, dst, st));
-    reqs[i].out->p = dst;
-    reqs[i].out->K = (reqs[i].K + 63) / 64 * 64;
-    reqs[i].out->N = (reqs[i].N + 15) / 16 * 16;  // the layer's output width as the chain checks see it
-    reqs[i].out->N32 = tc_packed_rows(reqs[i].N);   // rows of the packed image
-    reqs[i].out->n_valid = reqs[i].N;
-    reqs[i].out->winv = 1.f / scale;
-    reqs[i].out->gain = (float)reqs[i].K * amax[i];
-    off += img;
+    const Req& r = reqs[i];
+    *r.out = tc_weights(p->tc_packed.p + off, r.K, r.N, amax[i], parts);
+    GW_CUDA(launch_pack_weights(r.W, r.ldw, r.K, r.N, 1.f / r.out->winv, parts, p->tc_packed.p + off, st));
+    off += (tc_packed_bytes(r.K, r.N, parts) + 1023) / 1024 * 1024;
   }
   return 0;
 }

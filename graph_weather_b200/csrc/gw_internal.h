@@ -60,6 +60,15 @@ bool tc3_chain_is_lean(const TcChain& ch);  // would the launch take the lean (p
 // A layer with a LayerNorm cannot be split: cudaErrorInvalidValue.
 constexpr int TC_COL_BLOCK = 256;
 cudaError_t tc_column_block(const TcChain& ch, int n0, int nb, TcChain* out);
+// The one-layer chain of a training row op (gw_train.inl, train_op): stage 0 = op.a with K0 = K rounded to 64, layer 0 = the op's
+// bias, addends, ReLU, LayerNorm, residual, output, pre-LayerNorm store and mask over all N columns -- the `ch` tc_column_block
+// cuts into the blocks that run.  It sets no operand bounds, weight image, split or status.  cudaErrorInvalidValue for an op no
+// chain runs: an add[2] addend, no a[0], or a LayerNorm wider than TC_COL_BLOCK.
+cudaError_t tc_row_op_chain(const GemmOp& op, TcChain* ch);
+// fp32-mode bound of a training row op's stage-0 source s: *amax (zeroed by the caller) takes the absmax of the whole tensor s
+// reads (batch x src_rows rows of a stream, rows_per_sample rows of a broadcast), and s is bounded by it.  Sources of another
+// kind: cudaErrorInvalidValue.
+cudaError_t launch_operand_bound(RowSrc& s, int rows_per_sample, int batch, float* amax, cudaStream_t st);
 // Packs W[n, k] (n < N_src rows of stride ldw, k < K_src) into the GMMA operand image the chain kernel streams with
 // cp.async.bulk (perm32 feature order, gw_pack.cu); `parts` = 2 (fp16 hi, lo) or 1 (bf16).  dst must hold tc_packed_bytes(K_src, N_src, parts).
 size_t tc_packed_bytes(int K_src, int N_src, int parts);
@@ -69,6 +78,20 @@ int tc_packed_rows(int N_src);  // rows of the packed image: N padded to 64
 cudaError_t launch_pack_weights(const float* W, int ldw, int K_src, int N_src, float wscale, int parts, void* dst, cudaStream_t stream,
                                 const float* amax_dev = nullptr);
 cudaError_t launch_absmax(const float* W, int ldw, int K_src, int N_src, float* out_max, cudaStream_t stream);
+// The training step's image of W, scale taken on the device: *wamax = max|W| (reset first), then the pack.  A chain layer given
+// this image takes wamax as its TcLayer::wamax.
+cudaError_t launch_pack_image(const float* W, int ldw, int K_src, int N_src, int parts, void* img, float* wamax, cudaStream_t stream);
+// A weight image packed with a scale the host chose from max|W| (the inference plans' images, gw_api.cu): what its chain layer
+// needs to know of it.  Pack it with wscale = 1 / winv (a power of two: exact).
+struct TcWeights {
+  const void* p = nullptr;
+  int K = 0, N = 0, N32 = 0, n_valid = 0;  // TcLayer::K (K_src rounded to 64), N (N_src rounded to 16), N32, n_valid (N_src)
+  float winv = 1.f;                        // TcLayer::wscale_inv
+  float gain = 0.f;                        // K_src * max|W|: |A.W^T| <= gain * max|A|
+};
+TcWeights tc_weights(const void* img, int K_src, int N_src, float wamax, int parts);
+// bound of a LayerNorm'd row of N columns: sqrt(N) max|gamma| + max|beta|
+float tc_ln_bound(int N, float gamma_amax, float beta_amax);
 // Power of two a weight image is stored times: fp16 hi|lo images (parts 2) bring max|W| into [2048, 4096) so the lo parts stay
 // normal (the host's pack_tc_weights uses the same rule); bf16 images are not scaled.
 __host__ __device__ inline float tc_weight_scale(float amax, int parts) {

@@ -115,8 +115,6 @@ struct TcChain {
   long long* trace = nullptr; // optional debug timeline: [8 roles][1024 events][2] = {clock64, code}; CTA 0 only
   int32_t fast = 0;           // gw_tc3: bit l = layer l takes the lean full-width path, bit 31 = stage 0 does (set by the launcher)
   int32_t ablate = 0;         // diagnostics build only (-DGW_ABLATE): bit mask of pipeline parts to skip, for timing attribution
-  int32_t range_fit = 0;      // ignored: every chain scales its fp16-split operands into [2^14, 2^15), up as well as down (gw_tc3.cu,
-                              // fit_scale).  Kept so that callers written when this selected that rule (1) still compile.
   // Loss-boundary gather fused into the chain that produces the forecast (multi-GPU; graph_weather_b200/dist.py): the LAST layer's
   // fp32 result rows are stored, tile by tile as they leave the accumulator, into the gather buffers of every GPU of the job --
   // out_mode 1: one multimem.st per value to the NVLink multicast alias of `out` (the switch replicates it to every GPU);

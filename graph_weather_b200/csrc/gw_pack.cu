@@ -71,4 +71,18 @@ cudaError_t launch_absmax(const float* W, int ldw, int K_src, int N_src, float* 
   return cudaGetLastError();
 }
 
+cudaError_t launch_pack_image(const float* W, int ldw, int K_src, int N_src, int parts, void* img, float* wamax, cudaStream_t stream) {
+  cudaError_t e = cudaMemsetAsync(wamax, 0, sizeof(float), stream);
+  if (e == cudaSuccess) e = launch_absmax(W, ldw, K_src, N_src, wamax, stream);
+  if (e == cudaSuccess) e = launch_pack_weights(W, ldw, K_src, N_src, 1.f, parts, img, stream, wamax);
+  return e;
+}
+
+TcWeights tc_weights(const void* img, int K_src, int N_src, float wamax, int parts) {
+  TcWeights w;
+  w.p = img, w.K = round_up(K_src, 64), w.N = round_up(N_src, 16), w.N32 = tc_packed_rows(N_src), w.n_valid = N_src;
+  w.winv = 1.f / tc_weight_scale(wamax, parts), w.gain = (float)K_src * wamax;
+  return w;
+}
+
 }  // namespace gw

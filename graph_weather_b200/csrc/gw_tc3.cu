@@ -1099,6 +1099,27 @@ cudaError_t tc_column_block(const TcChain& ch, int n0, int nb, TcChain* out) {
   B.out_cols = std::max(0, std::min(L.out_cols - n0, nb));
   return cudaSuccess;
 }
+cudaError_t tc_row_op_chain(const GemmOp& op, TcChain* ch) {
+  if (op.add[2].kind != SRC_NONE || op.a[0].kind == SRC_NONE || (op.ln_gamma && op.N > TC_COL_BLOCK)) return cudaErrorInvalidValue;
+  *ch = TcChain();
+  ch->rows_per_sample = op.rows_per_sample, ch->batch = op.batch;
+  ch->a0[0] = op.a[0], ch->a0[1] = op.a[1];
+  ch->K0 = (op.K + 63) / 64 * 64, ch->n_layers = 1;
+  TcLayer& L = ch->layer[0];
+  L.K = ch->K0, L.N = op.N, L.n_valid = op.N;
+  L.bias = op.bias, L.add[0] = op.add[0], L.add[1] = op.add[1], L.relu = op.relu;
+  L.ln_g = op.ln_gamma, L.ln_b = op.ln_beta, L.residual = op.residual;
+  L.out = op.out, L.ldo = op.ldo, L.out_cols = op.N, L.save_pre = op.save_pre, L.mask = op.mask;
+  return cudaSuccess;
+}
+cudaError_t launch_operand_bound(RowSrc& s, int rows_per_sample, int batch, float* amax, cudaStream_t st) {
+  if (s.kind != SRC_STREAM && s.kind != SRC_BCAST) return cudaErrorInvalidValue;
+  const long long n = (long long)(s.kind == SRC_STREAM ? (long long)batch * s.src_rows : (long long)rows_per_sample) * s.ld;
+  const cudaError_t e = launch_absmax_flat(s.base, n, amax, st);
+  s.bound = amax, s.bound_mul = 1.f, s.bound_mul_i = nullptr;
+  return e;
+}
+float tc_ln_bound(int N, float gamma_amax, float beta_amax) { return sqrtf((float)N) * gamma_amax + beta_amax; }
 cudaError_t launch_chain_tc3(const TcChain& ch_in, cudaStream_t stream) {
   TcChain ch = ch_in;
   using namespace t3;

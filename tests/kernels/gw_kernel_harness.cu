@@ -1,4 +1,5 @@
-// gw_kernel_harness.cu -- test-only shim over the internal launchers of libgwb200.so (tests/test_gpu_kernels.py).
+// gw_kernel_harness.cu -- test-only shim over the internal launchers of libgwb200.so (tests/test_gpu_kernels.py,
+// tests/test_gpu_wide_training.py).
 //
 // Host code only: flat extern "C" wrappers that the kernel tests call through ctypes, so that every CUDA primitive of the
 // training step, the forward's CUDA-core row ops and helpers, and the device-built graphs (tests/test_gpu_forward_simt.py,
@@ -10,6 +11,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "../../graph_weather_b200/csrc/gw_internal.h"
@@ -135,10 +137,10 @@ int h_wgrad_simt(const float* dY, int ldy, int N, const HSrc* a, int K, int rows
   return (int)launch_wgrad(dY, ldy, N, row_src(*a), K, rows, batch, dW, ldw, db, (cudaStream_t)stream);
 }
 
-// One training row op.  precision 0: fp32_simt (gw_simt.cu); 1: fp32 (fp16 hi/lo, 3 MMAs); 2: bf16.  The tensor-core precisions
-// build the one-layer chain the training step builds (gw_train.inl, train_op): weight image packed with its scale taken on the
-// device, stage-0 sources bounded by their whole tensor's absmax (fp32), K0 rounded to 64.  *lean: whether the chain
-// takes the lean path (-1 for fp32_simt).
+// One training row op of any N.  precision 0: fp32_simt (gw_simt.cu); 1: fp32 (fp16 hi/lo, 3 MMAs); 2: bf16.  The tensor-core
+// precisions run it as the training step does (gw_train.inl, train_op): the chain of tc_row_op_chain, its stage-0 sources bounded
+// by launch_operand_bound (fp32), cut by tc_column_block into blocks of at most TC_COL_BLOCK output columns, each with the image of
+// its rows of W from launch_pack_image.  *lean: bit j = column block j takes the lean path (-1 for fp32_simt).
 int h_row_op(int precision, const HOp* h, int* lean, int32_t* status, void* stream) {
   const cudaStream_t st = (cudaStream_t)stream;
   GemmOp op;
@@ -153,42 +155,36 @@ int h_row_op(int precision, const HOp* h, int* lean, int32_t* status, void* stre
   if (precision != 1 && precision != 2) return (int)cudaErrorInvalidValue;
   const bool split = precision == 1;
   const int parts = split ? 2 : 1;
-  Temps t(st);
-  unsigned char* img = nullptr;
-  float* wamax = nullptr;
-  float* bounds = nullptr;
-  H_TRY(t.get(&img, tc_packed_bytes(op.K, op.N, parts)));
-  H_TRY(t.get(&wamax, 1));
-  H_TRY(t.get(&bounds, 2));
-  H_TRY(cudaMemsetAsync(wamax, 0, sizeof(float), st));
-  H_TRY(cudaMemsetAsync(bounds, 0, 2 * sizeof(float), st));
-  H_TRY(launch_absmax(op.W, op.ldw, op.K, op.N, wamax, st));
-  H_TRY(launch_pack_weights(op.W, op.ldw, op.K, op.N, 1.f, parts, img, st, wamax));
   TcChain ch;
-  ch.rows_per_sample = op.rows_per_sample, ch.batch = op.batch;
-  ch.a0[0] = op.a[0], ch.a0[1] = op.a[1];
-  ch.K0 = (op.K + 63) / 64 * 64, ch.n_layers = 1, ch.split = split ? 1 : 0, ch.status = status;
+  H_TRY(tc_row_op_chain(op, &ch));
+  ch.split = split ? 1 : 0, ch.status = status;
+  Temps t(st);
+  float* bounds = nullptr;
+  H_TRY(t.get(&bounds, 2));
+  H_TRY(cudaMemsetAsync(bounds, 0, 2 * sizeof(float), st));
   if (split)
-    for (int a = 0; a < 2; ++a) {
-      RowSrc& s = ch.a0[a];
-      if (s.kind == SRC_NONE) continue;
-      if (s.kind != SRC_STREAM && s.kind != SRC_BCAST) return (int)cudaErrorInvalidValue;
-      const long long n = (long long)(s.kind == SRC_STREAM ? (long long)op.batch * s.src_rows : (long long)op.rows_per_sample) * s.ld;
-      H_TRY(launch_absmax_flat(s.base, n, bounds + a, st));
-      s.bound = bounds + a, s.bound_mul = 1.f, s.bound_mul_i = nullptr;
-    }
-  TcLayer& L = ch.layer[0];
-  L.Wp = img, L.K = ch.K0, L.N = (op.N + 15) / 16 * 16, L.N32 = tc_packed_rows(op.N), L.n_valid = op.N, L.wamax = wamax;
-  L.bias = op.bias, L.add[0] = op.add[0], L.add[1] = op.add[1], L.relu = op.relu;
-  L.ln_g = op.ln_gamma, L.ln_b = op.ln_beta, L.residual = op.residual;
-  L.out = op.out, L.ldo = op.ldo, L.out_cols = op.N, L.save_pre = op.save_pre, L.mask = op.mask;
-  if (lean) *lean = tc3_chain_is_lean(ch) ? 1 : 0;
-  return (int)launch_chain_tc3(ch, st);
+    for (int a = 0; a < 2; ++a)
+      if (ch.a0[a].kind != SRC_NONE) H_TRY(launch_operand_bound(ch.a0[a], op.rows_per_sample, op.batch, bounds + a, st));
+  if (lean) *lean = 0;
+  for (int n0 = 0, j = 0; n0 < op.N; n0 += TC_COL_BLOCK, ++j) {
+    const int nb = std::min(TC_COL_BLOCK, op.N - n0);
+    TcChain blk;
+    H_TRY(tc_column_block(ch, n0, nb, &blk));
+    unsigned char* img = nullptr;
+    float* wamax = nullptr;
+    H_TRY(t.get(&img, tc_packed_bytes(op.K, nb, parts)));
+    H_TRY(t.get(&wamax, 1));
+    H_TRY(launch_pack_image(op.W + (size_t)n0 * op.ldw, op.ldw, op.K, nb, parts, img, wamax, st));
+    blk.layer[0].Wp = img, blk.layer[0].wamax = wamax;
+    if (lean && tc3_chain_is_lean(blk)) *lean |= 1 << j;
+    H_TRY(launch_chain_tc3(blk, st));
+  }
+  return 0;
 }
 
-// One inference chain (precision 1: fp32, 2: bf16), prepared as gw_api.cu prepares it: every weight image packed with the host's
-// power-of-two scale (tc_weight_scale of its device absmax), gain = K max|W|, off = max|bias|, ln_bound = sqrt(N) max|gamma| +
-// max|beta|, and every source bounded by the absmax of its whole table (launch_absmax_flat).  A layer with fused per-target sums
+// One inference chain (precision 1: fp32, 2: bf16), prepared as gw_api.cu prepares it: every weight image described by tc_weights
+// of its device absmax and packed with that scale, off = max|bias|, ln_bound = tc_ln_bound of the LayerNorm parameters' absmax,
+// and every source bounded by the absmax of its whole table (launch_absmax_flat).  A layer with fused per-target sums
 // gets a carry buffer (prefilled with NaN: a carry row read before it is written poisons the sum), and gw_seg_carry_kernel runs
 // after the chain, as in stage_processor / stage_decoder.  *lean: tc3_chain_is_lean.
 int h_chain(int precision, const HChain* h, int* lean, int32_t* status, void* stream) {
@@ -247,12 +243,11 @@ int h_chain(int precision, const HChain* h, int* lean, int32_t* status, void* st
     TcLayer& L = ch.layer[l];
     unsigned char* img = nullptr;
     H_TRY(t.get(&img, tc_packed_bytes(H.K, H.N, parts)));
-    const float scale = tc_weight_scale(hm[4 * l], parts);
-    H_TRY(launch_pack_weights(H.W, H.ldw, H.K, H.N, scale, parts, img, st));
-    L.Wp = img, L.K = (H.K + 63) / 64 * 64, L.N = (H.N + 15) / 16 * 16, L.N32 = tc_packed_rows(H.N), L.n_valid = H.N;
-    L.wscale_inv = 1.f / scale, L.gain = (float)H.K * hm[4 * l], L.off = hm[4 * l + 1];
+    const TcWeights w = tc_weights(img, H.K, H.N, hm[4 * l], parts);
+    H_TRY(launch_pack_weights(H.W, H.ldw, H.K, H.N, 1.f / w.winv, parts, img, st));
+    L.Wp = w.p, L.K = w.K, L.N = w.N, L.N32 = w.N32, L.n_valid = w.n_valid, L.wscale_inv = w.winv, L.gain = w.gain, L.off = hm[4 * l + 1];
     L.bias = H.bias, L.relu = H.relu, L.ln_g = H.ln_g, L.ln_b = H.ln_b;
-    if (H.ln_g) L.ln_bound = sqrtf((float)H.N) * hm[4 * l + 2] + hm[4 * l + 3];
+    if (H.ln_g) L.ln_bound = tc_ln_bound(H.N, hm[4 * l + 2], hm[4 * l + 3]);
     L.out = H.out, L.ldo = H.ldo, L.out_cols = H.out_cols, L.out_bound = H.out_bound;
     L.feeds_next = H.feeds_next, L.reuse_a = H.reuse_a;
     L.seg_dst = H.seg_dst, L.seg_out = H.seg_out, L.seg_ld = H.seg_ld, L.seg_rows = H.seg_rows, L.seg_maxdeg = (float)H.seg_maxdeg;

@@ -2,8 +2,8 @@
 from the same fp32 inputs, layer by layer (never against another kernel).
 
 Every chain gw_api.cu builds for the forecast is rebuilt here through h_chain (tests/kernels/gw_kernel_harness.cu), prepared as
-inference prepares it: host weight scales and gains, stage-0 bounds from the inputs' absmax, the carry pass after fused per-target
-sums.  Each runs in fp32 (fp16 hi/lo split) and bf16, on the lean path and under GW_TC3_NOFAST (the general path), and must:
+inference prepares it: weight images and LayerNorm bounds through the library's tc_weights and tc_ln_bound, stage-0 bounds from
+the inputs' absmax, the carry pass after fused per-target sums.  Each runs in fp32 (fp16 hi/lo split) and bf16, on the lean path and under GW_TC3_NOFAST (the general path), and must:
   (a) exact-integer data -- integers of at most 3 significant bits (both precisions) or 16 (fp32 only, so the lo parts are not
       zero) times 2^s, sparse +-1 weights, LayerNorm gamma = 0 so that a LayerNorm'd row is exactly beta + residual -- reproduce
       float64 bit for bit: every output, every per-target sum, carry and per-target constant.  s = -40 underflows any fp16

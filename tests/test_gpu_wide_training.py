@@ -12,8 +12,6 @@ The model: a train/run_fulll.py-shaped forecaster (597 + 24 features, 2 blocks, 
 train/run.py-shaped one (1024-wide, 605 + 40 features, 2 blocks, 30-degree grid) in fp32_simt, against torch.autograd on the
 CPU oracle."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -28,36 +26,9 @@ EXACT = [pytest.param(dict(exact=True, s=s), id=f"int_s{s}") for s in (-40, 0, 2
 FLOAT = tk.FLOAT
 
 
-WIDE_HARNESS = os.path.join(tk.ROOT, "tests", "kernels", "gw_wide_harness.cu")
-
-
-def _compile_wide_harness(out_dir):
-    """Builds the package, then tests/kernels/gw_wide_harness.cu (gw_kernel_harness.cu + h_row_op_blocks) against its
-    libgwb200.so, the way test_gpu_kernels.py builds its harness (undefined symbols are link errors)."""
-    ge.build()
-    so = os.path.join(str(out_dir), "libgwwideharness.so")
-    cmd = [ge.NVCC, "-shared", "-std=c++17", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_90a,code=sm_90a", WIDE_HARNESS, "-o", so,
-           "-L" + tk.PKG, "-lgwb200", "-lcudart", "-Xlinker", "-rpath," + tk.PKG, "-Xlinker", "--no-undefined"]  # fmt: skip
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, f"harness build failed:\n{r.stdout}{r.stderr}"
-    lib = ctypes.CDLL(so)
-    sigs = dict(tk._SIGNATURES, h_row_op_blocks=[ctypes.c_int, ctypes.POINTER(tk.HOp), ctypes.POINTER(ctypes.c_int), ctypes.c_void_p,
-                                                 ctypes.c_void_p])  # fmt: skip
-    for name, args in sigs.items():
-        fn = getattr(lib, name)
-        fn.restype, fn.argtypes = ctypes.c_int, args
-    return lib
-
-
-def test_wide_harness_builds_and_links(tmp_path):
-    """No GPU needed: the wide harness compiles and links against a fresh build."""
-    lib = _compile_wide_harness(tmp_path)
-    assert lib.h_sizeof_op() == ctypes.sizeof(tk.HOp)
-
-
 @pytest.fixture(scope="module")
 def hk(tmp_path_factory):
-    lib = _compile_wide_harness(tmp_path_factory.mktemp("gw_wide_harness"))
+    lib = tk._compile_harness(tmp_path_factory.mktemp("gw_wide_harness"))
     tk.HK = lib  # (the helpers of test_gpu_kernels call through it)
     return lib
 
@@ -225,15 +196,7 @@ def test_wide_wgrad_tc_is_repeatable(kind):
 
 # ---- column-blocked row ops ---------------------------------------------------------------------------------------------------
 class BlockedOp(tk.RowOp):
-    """A training row op of any N through h_row_op_blocks (the column blocks train_op runs); run() returns the lean mask."""
-
-    def run(self, prec, nofast=False):
-        saved = tk.HK.h_row_op
-        tk.HK.h_row_op = tk.HK.h_row_op_blocks  # (RowOp.run builds the HOp and calls HK.h_row_op)
-        try:
-            return super().run(prec, nofast)
-        finally:
-            tk.HK.h_row_op = saved
+    """A training row op of any N: h_row_op runs the column blocks train_op runs, and run() returns their lean mask."""
 
 
 def _bshape(name, d, rows=300, batch=2):
