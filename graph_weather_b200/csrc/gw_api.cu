@@ -105,6 +105,7 @@ struct gw_plan {
   gw_dims d;
   int device = 0;
   int n_in_cur = 0;
+  unsigned enc_graph_gen = 0;  // bumped whenever the encoder graph is replaced (the training step's chunk tables are built per graph)
   // graphs
   DevBuf<int32_t> enc_mesh, enc_perm, enc_ptr, lat_src, lat_dst, lat_ptr, dec_src, dec_ptr;
   DevBuf<float> enc_attr, lat_attr, dec_attr;
@@ -1282,6 +1283,7 @@ int gw_plan_set_encoder_graph(gw_plan* p, int32_t n_in, const int32_t* enc_mesh,
   GW_CUDA(cudaMemcpyAsync(p->enc_attr.p, attr, (size_t)n_in * p->d.enc_edge_attr_dim * 4, cudaMemcpyDeviceToDevice, st));
   p->n_in_cur = n_in;
   p->have_enc = true;
+  ++p->enc_graph_gen;
   GW_TRY(gw::encoder_degree(p, st));
   if (p->w_enc && !p->train_only) GW_TRY(gw::precompute_encoder_constants(p, st));  // per-call graphs (assimilator_encoder.py:118)
   return 0;
@@ -1326,6 +1328,7 @@ int gw_plan_build_obs_graph(gw_plan* p, const float* lat_lon_heights, int32_t n_
                                p->obs_ws.p, p->obs_ws.n, p->tc_status_dev, st));
   p->n_in_cur = n_obs;
   p->have_enc = true;
+  ++p->enc_graph_gen;
   GW_TRY(gw::encoder_degree(p, st));
   if (p->w_enc && !p->train_only) GW_TRY(gw::precompute_encoder_constants(p, st));  // per-call graphs (assimilator_encoder.py:118)
   return 0;

@@ -135,7 +135,7 @@ TRAIN_PRECISIONS = ("fp32_simt", "fp32", "bf16")
 
 
 def _validate_train_precision(train_precision: str, dims: dict):
-    """`train_precision` of GraphWeatherForecaster: the arithmetic of the training step (gw_train.inl).  'fp32_simt' exact fp32 on
+    """`train_precision` of GraphWeatherForecaster, GraphCast and GraphWeatherAssimilator: the arithmetic of the training step (gw_train.inl).  'fp32_simt' exact fp32 on
     CUDA cores; 'fp32' fp16 hi/lo split on tensor cores (3 MMAs per product, fp32 accumulation); 'bf16' bf16 tensor-core
     operands (fp32 accumulation, fp32 master weights, gradients and tape)."""
     if train_precision not in TRAIN_PRECISIONS:
@@ -170,6 +170,7 @@ class _Engine:
         self.plan: Optional[_capi.Plan] = None
         self.graph_uploaders = []  # callables(plan)
         self.generation = 0  # bumped whenever a new plan is created: per-plan upload caches key on it, never on pointers
+        self.obs_key = None  # the host-built observation graph the plan holds (AssimilatorEncoder._upload_obs)
         self._wfp = None
 
     def _create(self, device, max_batch):
@@ -223,18 +224,24 @@ def _maybe_check(plan):
         plan.status()
 
 
-class _ForecastTrainFn(torch.autograd.Function):
-    """autograd node of one training forward of GraphWeatherForecaster: forward = gw_train_forward (exact fp32, activations
-    kept in the plan), backward = gw_train_backward (gradients of every parameter under its reference name, and of the
-    features when they require grad).  One backward per forward: the plan holds a single tape."""
+class _TrainFn(torch.autograd.Function):
+    """autograd node of one training forward of a wrapper (GraphWeatherForecaster, GraphCast, GraphWeatherAssimilator): forward =
+    gw_train_forward (activations kept in the plan), backward = gw_train_backward (gradients of every parameter under its reference
+    name, and of the features when they require grad).  One backward per forward: the plan holds a single tape.
+
+    The wrapper supplies its training engine (`_training_engine()`), its named parameters (`_named()`) and its output shape
+    (`_out_shape(batch)`).  `obs` (the assimilator's lat_lon_heights, else None) is built into the training plan's observation
+    graph for this call, as inference builds it for every call."""
 
     @staticmethod
-    def forward(ctx, model, features, *params):
+    def forward(ctx, model, features, obs, *params):
         B = features.shape[0]
         eng = model._training_engine()
-        plan = eng.ensure(features.device, B, model._named())
+        plan = eng.ensure(features.device, B, model._named(), grow=None if obs is None else dict(n_in=obs.shape[0]))
+        if obs is not None:
+            model.encoder._upload_obs(eng, plan, obs)
         f = features.detach().to(torch.float32).contiguous()
-        out = torch.empty((B, model.decoder.num_latlons, model.output_dim), dtype=torch.float32, device=f.device)
+        out = torch.empty(model._out_shape(B), dtype=torch.float32, device=f.device)
         plan.train_forward(f, out)
         eng.tape_id = getattr(eng, "tape_id", 0) + 1
         ctx.model, ctx.plan, ctx.eng, ctx.tape_id = model, plan, eng, eng.tape_id
@@ -258,7 +265,12 @@ class _ForecastTrainFn(torch.autograd.Function):
         ctx.plan.train_backward(g, gfeat, list(zip(ctx.names, grads)))
         ctx.eng.tape_id += 1  # the tape is consumed
         _maybe_check(ctx.plan)
-        return (None, gfeat) + tuple(gr if need else None for gr, need in zip(grads, ctx.pgrad))
+        return (None, gfeat, None) + tuple(gr if need else None for gr, need in zip(grads, ctx.pgrad))
+
+
+def _wants_grad(model, features):
+    """A wrapper's forward takes the training step in train mode with autograd on and something to differentiate."""
+    return torch.is_grad_enabled() and model.training and (features.requires_grad or any(q.requires_grad for q in model.parameters()))
 
 
 def _prefixed(prefix, module):
@@ -516,7 +528,6 @@ class AssimilatorEncoder(nn.Module):
         self._precision = precision
         self._engine = None
         self.efficient_batching = False
-        self._obs_key = None
         self._lat_edge_index_t = {}
 
     def _upload_graphs(self, plan):
@@ -527,19 +538,20 @@ class AssimilatorEncoder(nn.Module):
     def _upload_obs(self, engine, plan, lat_lon_heights):
         """The reference rebuilds the observation graph on every forward (assimilator_encoder.py:118,170-216).  Here the
         upload is skipped only when the observation set is provably the same: the key is the CONTENT of lat_lon_heights
-        (it is copied to the host to build the graph anyway) plus the engine's plan generation, never a tensor address."""
+        (it is copied to the host to build the graph anyway) plus the engine's plan generation, never a tensor address.  The key
+        is kept per engine: the inference and training engines hold different plans."""
         if lat_lon_heights.is_cuda and os.environ.get("GW_B200_HOST_OBS_GRAPH", "0") != "1":
             # the observation graph is rebuilt ON THE DEVICE for every call, as the reference rebuilds it for every call
             # (assimilator_encoder.py:118): point location, edge attributes, slot-sorted CSR -- no host copy, no synchronisation
             plan.build_obs_graph(lat_lon_heights.detach().to(device=plan.device, dtype=torch.float32).contiguous())
-            self._obs_key = None
+            engine.obs_key = None
             return
         llh = lat_lon_heights.detach().to(device="cpu", dtype=torch.float64).contiguous().numpy()
         key = (engine.generation, llh.shape, hash(llh.tobytes()))
-        if key != self._obs_key:
+        if key != engine.obs_key:
             g = graphs.build_encoder_graph(llh[:, :2], self.resolution, heights=llh[:, 2])
             plan.set_encoder_graph(g.mesh_local, g.perm, g.ptr, g.edge_attr)
-            self._obs_key = key
+            engine.obs_key = key
 
     def _own_engine(self):
         if self._engine is None:
@@ -699,7 +711,10 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
         return self._train_engine
 
     def _wants_grad(self, features):
-        return torch.is_grad_enabled() and self.training and (features.requires_grad or any(q.requires_grad for q in self.parameters()))
+        return _wants_grad(self, features)
+
+    def _out_shape(self, batch):
+        return (batch, self.decoder.num_latlons, self.output_dim)
 
     def forward(self, features: torch.Tensor, t: int = 0) -> torch.Tensor:
         self._check_features(features)
@@ -708,7 +723,7 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
             # its activations and `loss.backward()` runs the CUDA backward.  Inference (`model.eval()` or `torch.no_grad()`) takes
             # the tensor-core path below.
             params = [q for _, q in self.named_parameters()]
-            out = _ForecastTrainFn.apply(self, features, *params)
+            out = _TrainFn.apply(self, features, None, *params)
             if self.constraint_type != "none":
                 # forecast.py:235-246 under autograd: the layer's backward adds the gradient of its `lr` input (the first
                 # feature_dim features) to the residual and encoder paths of features.grad
@@ -801,19 +816,24 @@ class GraphWeatherAssimilatorConfig:
     hidden_layers_decoder: int = 2
     norm_type: str = "LayerNorm"
     use_checkpointing: bool = False
+    train_precision: str = "fp32_simt"
 
     def build(self) -> "GraphWeatherAssimilator":
         return GraphWeatherAssimilator(**self.__dict__)
 
 
 class GraphWeatherAssimilator(nn.Module, PyTorchModelHubMixin):
-    """GraphWeatherAssimilator(output_lat_lons=..)(features, obs_lat_lon_heights): analysis.py:52-150."""
+    """GraphWeatherAssimilator(output_lat_lons=..)(features, obs_lat_lon_heights): analysis.py:52-150.  Inference and training
+    run on the device.  In train mode with autograd on, `loss.backward()` runs the CUDA backward (`train_precision`, as in
+    GraphWeatherForecaster; use_checkpointing=True selects the bounded-memory step).  The observation graph is rebuilt for every
+    training forward, as for every inference forward; `features.grad` is the gradient of the observation values, and
+    `obs_lat_lon_heights` gets none (the reference builds the graph in numpy)."""
 
     def __init__(self, output_lat_lons: list, resolution: int = 2, observation_dim: int = 2, analysis_dim: int = 78,
                  node_dim: int = 256, edge_dim: int = 256, num_blocks: int = 9, hidden_dim_processor_node: int = 256,
                  hidden_dim_processor_edge: int = 256, hidden_layers_processor_node: int = 2, hidden_layers_processor_edge: int = 2,
                  hidden_dim_decoder: int = 128, hidden_layers_decoder: int = 2, norm_type: str = "LayerNorm",
-                 use_checkpointing: bool = False, precision: str = "auto"):  # fmt: skip
+                 use_checkpointing: bool = False, precision: str = "auto", train_precision: str = "fp32_simt"):  # fmt: skip
         super().__init__()
         output_lat_lons = _latlon_list(output_lat_lons)
         self.encoder = AssimilatorEncoder(resolution=resolution, input_dim=observation_dim, output_dim=node_dim,
@@ -839,14 +859,34 @@ class GraphWeatherAssimilator(nn.Module, PyTorchModelHubMixin):
         dims.update(n_out=self.decoder.num_latlons, n_dec_edges=self.decoder._dims["n_dec_edges"], out_dim=analysis_dim,
                     residual_dim=0, hidden_dec=hidden_dim_decoder, hidden_layers_dec=hidden_layers_decoder, num_blocks=num_blocks)  # fmt: skip
         self.analysis_dim = analysis_dim
+        self.use_checkpointing = use_checkpointing
         self._engine = _Engine(dims, precision)
         self._engine.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
+        _validate_train_precision(train_precision, dims)
+        self.train_precision = train_precision
+
+    def _named(self):
+        return [(k, v) for k, v in self.state_dict(keep_vars=True).items()]
+
+    def _out_shape(self, batch):
+        return (batch, self.decoder.num_latlons, self.analysis_dim)
+
+    def _training_engine(self):
+        """The plan the training step runs on (created on first use; the inference engine stays as it is), as
+        GraphWeatherForecaster._training_engine.  Its observation graph is built by every training forward."""
+        if getattr(self, "_train_engine", None) is None:
+            eng = _Engine(self._engine.dims, self.train_precision, train_only=bool(self.use_checkpointing))
+            eng.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
+            self.__dict__["_train_engine"] = eng
+        return self._train_engine
 
     def forward(self, features: torch.Tensor, obs_lat_lon_heights: torch.Tensor) -> torch.Tensor:
         if features.device.type != "cuda":
             _no_host_path("GraphWeatherAssimilator.forward")
+        if _wants_grad(self, features):
+            return _TrainFn.apply(self, features, obs_lat_lon_heights, *[q for _, q in self.named_parameters()])
         B, nobs = features.shape[0], obs_lat_lon_heights.shape[0]
-        named = [(k, v) for k, v in self.state_dict(keep_vars=True).items()]
+        named = self._named()
         plan = self._engine.ensure(features.device, B, named, grow=dict(n_in=nobs))
         self.encoder._upload_obs(self._engine, plan, obs_lat_lon_heights)
         f = features.detach().to(torch.float32).contiguous()
@@ -861,20 +901,30 @@ class GraphWeatherAssimilator(nn.Module, PyTorchModelHubMixin):
 # ---------------------------------------------------------------------------------------------------------------
 class GraphCast(nn.Module):
     """graph_weather/models/graphcast/model.py:21-285: Encoder + Processor + Decoder with hierarchical gradient-checkpoint
-    controls and `efficient_batching`.  Forward-only here: the checkpoint setters are accepted and recorded (they do not
-    change forward results in the reference either), and efficient / replicated batching are the same computation -- the
-    CUDA path always shares one graph across the batch (the reference proves the equivalence in
-    tests/models/layers/test_efficient_batching.py)."""
+    controls and `efficient_batching`.  Efficient and replicated batching are the same computation -- the CUDA path always
+    shares one graph across the batch (the reference proves the equivalence in tests/models/layers/test_efficient_batching.py).
+
+    Inference and training run on the device.  In train mode with autograd on, `loss.backward()` runs the CUDA backward
+    (`train_precision`, as in GraphWeatherForecaster; features.grad includes the residual path of the full input).  The
+    checkpoint controls choose the training step, read at every training forward:
+      * the bounded-memory step (a training-only plan that recomputes the grid-sized stages chunk by chunk in the backward) when
+        use_checkpointing, set_checkpoint_model(True), set_checkpoint_encoder(True) or set_checkpoint_decoder(True) is set --
+        GraphCastConfig.full_checkpointing and balanced_checkpointing;
+      * the taped step otherwise.
+    set_checkpoint_processor(segments) on its own keeps the processor's tape: the CUDA step has no processor-segment recompute
+    (DESIGN.md section 9).  Checkpointing never changes the forward's result, in the reference or here."""
 
     def __init__(self, lat_lons: list, resolution: int = 2, input_dim: int = 78, output_dim: int = 78, hidden_dim: int = 256,
                  num_processor_blocks: int = 9, hidden_layers: int = 2, mlp_norm_type: str = "LayerNorm",
-                 use_checkpointing: bool = False, efficient_batching: bool = False, precision: str = "auto"):  # fmt: skip
+                 use_checkpointing: bool = False, efficient_batching: bool = False, precision: str = "auto",
+                 train_precision: str = "fp32_simt"):  # fmt: skip
         super().__init__()
         lat_lons = _latlon_list(lat_lons)
         self.lat_lons = lat_lons
         self.input_dim = input_dim
         self.output_dim = output_dim
         self.efficient_batching = efficient_batching
+        self.use_checkpointing = use_checkpointing
         self.encoder = Encoder(lat_lons=lat_lons, resolution=resolution, input_dim=input_dim, output_dim=hidden_dim,
                                output_edge_dim=hidden_dim, hidden_dim_processor_node=hidden_dim, hidden_dim_processor_edge=hidden_dim,
                                hidden_layers_processor_node=hidden_layers, hidden_layers_processor_edge=hidden_layers,
@@ -898,6 +948,34 @@ class GraphCast(nn.Module):
                     residual_dim=output_dim, hidden_dec=hidden_dim, hidden_layers_dec=hidden_layers, num_blocks=num_processor_blocks)  # fmt: skip
         self._engine = _Engine(dims, precision)
         self._engine.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
+        _validate_train_precision(train_precision, dims)
+        self.train_precision = train_precision
+
+    def _named(self):
+        return [(k, v) for k, v in self.state_dict(keep_vars=True).items()]
+
+    def _out_shape(self, batch):
+        return (batch, self.decoder.num_latlons, self.output_dim)
+
+    def _bounded_step(self) -> bool:
+        return bool(self.use_checkpointing or self._checkpoint_model or self._checkpoint_encoder or self._checkpoint_decoder)
+
+    def _training_engine(self):
+        """The engine of the step the checkpoint controls select now (class docstring): the taped or the bounded one, each
+        created on first use.  Only one holds a plan: switching strategy closes the other's, so a backward of a forward made
+        under the other strategy raises "one backward per forward"."""
+        engines = self.__dict__.setdefault("_train_engines", {})
+        bounded = self._bounded_step()
+        if bounded not in engines:
+            eng = _Engine(self._engine.dims, self.train_precision, train_only=bounded)
+            eng.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
+            engines[bounded] = eng
+        other = engines.get(not bounded)
+        if other is not None and other.plan is not None:
+            other.plan.close()
+            other.plan = None
+        self.__dict__["_train_engine"] = engines[bounded]
+        return engines[bounded]
 
     # hierarchical checkpointing controls (model.py:118-174)
     def set_checkpoint_model(self, checkpoint_flag: bool):
@@ -922,8 +1000,10 @@ class GraphCast(nn.Module):
         if features.shape[-1] != self.output_dim:  # the reference adds the full input as the residual (model.py:203, decoder.py:93)
             raise RuntimeError(f"The size of tensor a ({self.output_dim}) must match the size of tensor b ({features.shape[-1]}) "
                                "at non-singleton dimension 2")  # fmt: skip
+        if _wants_grad(self, features):
+            return _TrainFn.apply(self, features, None, *[q for _, q in self.named_parameters()])
         B = features.shape[0]
-        plan = self._engine.ensure(features.device, B, [(k, v) for k, v in self.state_dict(keep_vars=True).items()])
+        plan = self._engine.ensure(features.device, B, self._named())
         f = features.detach().to(torch.float32).contiguous()
         out = torch.empty((B, self.decoder.num_latlons, self.output_dim), dtype=torch.float32, device=f.device)
         plan.forward(f, out)

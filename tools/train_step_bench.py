@@ -1,8 +1,15 @@
-"""Times one training step (forward with tape + NormalizedMSELoss + backward + SGD update) of GraphWeatherForecaster.
-    python tools/train_step_bench.py [--grid 0.25deg|1deg|2deg|10deg] [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16]
-                                     [--feature-dim F] [--aux-dim A] [--num-blocks NB] [--width W]
-                                     [--constraint-type none|additive|multiplicative|softmax] [--use-checkpointing] [--fit-batch]
-The model defaults to the README's 78 + 24 features, 9 blocks, 256-wide.  The reference's ERA5 training scripts:
+"""Times one training step (forward with tape + NormalizedMSELoss + backward + SGD update) of GraphWeatherForecaster, GraphCast or
+GraphWeatherAssimilator.
+    python tools/train_step_bench.py [--model forecaster|graphcast|assimilator] [--grid 0.25deg|1deg|2deg|5deg|10deg] [--batch B]
+                                     [--steps K] [--train-precision fp32_simt|fp32|bf16] [--feature-dim F] [--aux-dim A]
+                                     [--num-blocks NB] [--width W] [--constraint-type none|additive|multiplicative|softmax]
+                                     [--use-checkpointing] [--fit-batch] [--n-obs N]
+The model defaults to the README's 78 + 24 features, 9 blocks, 256-wide.  --model graphcast: GraphCast(input_dim = output_dim =
+--feature-dim, hidden_dim = --width or 256); its bounded step is selected by --use-checkpointing (the same step
+GraphCastConfig.balanced_checkpointing / full_checkpointing select).  --model assimilator: GraphWeatherAssimilator(output_lat_lons =
+the grid, analysis_dim = --feature-dim) on --n-obs observations (2 values each) at random (lat, lon, height), a new set for every
+step, so every step rebuilds the observation graph; the reference README's configuration is --grid 5deg --feature-dim 24 --batch 1
+--n-obs 2660.  The reference's ERA5 training scripts:
     train/run_fulll.py  --feature-dim 597 --aux-dim 24 --num-blocks 6 (1-degree grid)
     train/run.py        --feature-dim 605 --aux-dim 40 --num-blocks 6 --width 1024 --grid 2deg
 (--width sets the node / edge / hidden / decoder widths together.)
@@ -67,7 +74,8 @@ def constraint_backward_time(model, x, F, reps=20):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--grid", default="1deg", choices=["0.25deg", "1deg", "2deg", "10deg"])
+    ap.add_argument("--model", default="forecaster", choices=["forecaster", "graphcast", "assimilator"])
+    ap.add_argument("--grid", default="1deg", choices=["0.25deg", "1deg", "2deg", "5deg", "10deg"])
     ap.add_argument("--batch", type=int, default=2)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--train-precision", default="fp32_simt", choices=["fp32_simt", "fp32", "bf16"])
@@ -78,38 +86,60 @@ def main():
     ap.add_argument("--constraint-type", default="none", choices=["none", "additive", "multiplicative", "softmax"])
     ap.add_argument("--use-checkpointing", action="store_true", help="the bounded-memory training step (training-only plan)")
     ap.add_argument("--fit-batch", action="store_true", help="report the largest batch that should fit, confirmed by one run")
+    ap.add_argument("--n-obs", type=int, default=2660, help="observations per step (--model assimilator)")
     a = ap.parse_args()
+    if a.model != "forecaster" and a.constraint_type != "none":
+        ap.error("--constraint-type applies to --model forecaster")
     import __graft_entry__ as ge
 
     ge.build()
-    from graph_weather_b200 import GraphWeatherForecaster, NormalizedMSELoss
+    from graph_weather_b200 import GraphCast, GraphWeatherAssimilator, GraphWeatherForecaster, NormalizedMSELoss
 
     if a.grid == "0.25deg":
         import numpy as np
 
         ll = [(float(lat), float(lon)) for lat in np.linspace(-90.0, 90.0, 721) for lon in np.arange(0.0, 360.0, 0.25)]
     else:
-        step = {"1deg": 1, "2deg": 2, "10deg": 10}[a.grid]
+        step = {"1deg": 1, "2deg": 2, "5deg": 5, "10deg": 10}[a.grid]
         ll = [(float(lat), float(lon)) for lat in range(-90, 90, step) for lon in range(0, 360, step)]
     torch.manual_seed(0)
-    dims = dict(feature_dim=a.feature_dim, aux_dim=a.aux_dim, num_blocks=a.num_blocks)
-    if a.width is not None:
-        dims.update(node_dim=a.width, edge_dim=a.width, hidden_dim_processor_node=a.width, hidden_dim_processor_edge=a.width,
-                    hidden_dim_decoder=a.width)  # fmt: skip
-    model = GraphWeatherForecaster(ll, train_precision=a.train_precision, constraint_type=a.constraint_type, use_checkpointing=a.use_checkpointing,
-                                   **dims).cuda().train()  # fmt: skip
     F = a.feature_dim
+    if a.model == "graphcast":
+        dims = dict(input_dim=F, output_dim=F, num_processor_blocks=a.num_blocks, hidden_dim=a.width or 256)
+        model = GraphCast(ll, train_precision=a.train_precision, use_checkpointing=a.use_checkpointing, **dims).cuda().train()
+        n_in, f_in = len(ll), F
+    elif a.model == "assimilator":
+        dims = dict(analysis_dim=F, num_blocks=a.num_blocks, n_obs=a.n_obs)
+        if a.width is not None:
+            dims.update(node_dim=a.width, edge_dim=a.width, hidden_dim_processor_node=a.width, hidden_dim_processor_edge=a.width,
+                        hidden_dim_decoder=a.width)  # fmt: skip
+        model = GraphWeatherAssimilator(output_lat_lons=ll, train_precision=a.train_precision, use_checkpointing=a.use_checkpointing,
+                                        **{k: v for k, v in dims.items() if k != "n_obs"}).cuda().train()  # fmt: skip
+        n_in, f_in = a.n_obs, 2
+    else:
+        dims = dict(feature_dim=F, aux_dim=a.aux_dim, num_blocks=a.num_blocks)
+        if a.width is not None:
+            dims.update(node_dim=a.width, edge_dim=a.width, hidden_dim_processor_node=a.width, hidden_dim_processor_edge=a.width,
+                        hidden_dim_decoder=a.width)  # fmt: skip
+        model = GraphWeatherForecaster(ll, train_precision=a.train_precision, constraint_type=a.constraint_type,
+                                       use_checkpointing=a.use_checkpointing, **dims).cuda().train()  # fmt: skip
+        n_in, f_in = len(ll), F + a.aux_dim
     crit = NormalizedMSELoss([1.0] * F, ll, normalize=True)
     opt = torch.optim.SGD(model.parameters(), lr=1e-3)
 
     def measure(batch, steps):
         """(ms/step, losses, torch peak bytes, train_peak_bytes, plan device_bytes, step function, inputs) of `steps` timed steps."""
-        x = torch.randn(batch, len(ll), F + a.aux_dim, device="cuda")
+        x = torch.randn(batch, n_in, f_in, device="cuda")
         y = torch.randn(batch, len(ll), F, device="cuda")
+        g = torch.Generator(device="cuda").manual_seed(1)
+
+        def obs():  # a new observation set: (lat, lon, height)
+            u = torch.rand(n_in, 3, device="cuda", generator=g)
+            return torch.stack([u[:, 0] * 180.0 - 90.0, u[:, 1] * 360.0, u[:, 2]], 1)
 
         def one():
             opt.zero_grad(set_to_none=True)
-            loss = crit(model(x), y)
+            loss = crit(model(x, obs()) if a.model == "assimilator" else model(x), y)
             loss.backward()
             opt.step()
             return loss
@@ -157,7 +187,7 @@ def main():
     phases = {k: round(v[1], 3) for k, v in tags.items() if k.startswith("train_") or k == "const"}
     plan.status()
     cbwd = constraint_backward_time(model, x, F) if a.constraint_type != "none" else None
-    print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "train_precision": a.train_precision, "grid": a.grid, "batch": a.batch,
+    print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "model": a.model, "train_precision": a.train_precision, "grid": a.grid, "batch": a.batch,
                       "use_checkpointing": a.use_checkpointing, "train_peak_gib": round(train_peak / 2**30, 3),
                       "plan_device_gib": round(plan_bytes / 2**30, 3),
                       "dims": dims, "constraint_type": a.constraint_type, "constraint_backward": cbwd,
