@@ -215,6 +215,19 @@ class _Engine:
         self._wfp = None
 
 
+def _new_engine(dims: dict, precision: str, uploaders, train_only: bool = False) -> _Engine:
+    eng = _Engine(dims, precision, train_only)
+    eng.graph_uploaders += uploaders
+    return eng
+
+
+def _own_engine(module, dims=None) -> _Engine:
+    """The engine of an Encoder, AssimilatorEncoder or decoder called on its own (created on first use)."""
+    if module._engine is None:
+        module._engine = _new_engine(module._dims if dims is None else dims, module._precision, [module._upload_graphs])
+    return module._engine
+
+
 def _maybe_check(plan):
     """Every forward ends with a non-blocking look at the plan's host-mapped status word; a non-zero word (fp16-range
     overflow, pipeline timeout, misalignment: include/gw_b200.h) escalates to the synchronising `plan.status()`, which
@@ -229,8 +242,8 @@ class _TrainFn(torch.autograd.Function):
     gw_train_forward (activations kept in the plan), backward = gw_train_backward (gradients of every parameter under its reference
     name, and of the features when they require grad).  One backward per forward: the plan holds a single tape.
 
-    The wrapper supplies its training engine (`_training_engine()`), its named parameters (`_named()`) and its output shape
-    (`_out_shape(batch)`).  `obs` (the assimilator's lat_lon_heights, else None) is built into the training plan's observation
+    The wrapper (`_Wrapper`) supplies its training engine (`_training_engine()`), its named parameters (`_named()`) and its output
+    shape (`_out_shape(batch)`).  `obs` (the assimilator's lat_lon_heights, else None) is built into the training plan's observation
     graph for this call, as inference builds it for every call."""
 
     @staticmethod
@@ -322,12 +335,6 @@ class Encoder(nn.Module):
         plan.set_encoder_graph(g.mesh_local, g.perm, g.ptr, g.edge_attr)
         plan.set_latent_graph(m.src, m.dst, m.ptr, m.edge_attr[m.perm])
 
-    def _own_engine(self):
-        if self._engine is None:
-            self._engine = _Engine(self._dims, self._precision)
-            self._engine.graph_uploaders.append(self._upload_graphs)
-        return self._engine
-
     def _latent_outputs(self, plan, batch, device):
         """(edge_index [2,B*El] int64, edge_attr [B*El,De]) in the reference's order and replication (encoder.py:224-242)."""
         m = self._g_lat
@@ -344,17 +351,26 @@ class Encoder(nn.Module):
             ref_attr = ref_attr.repeat(batch, 1)
         return self._lat_edge_index_t[key], ref_attr
 
-    def forward(self, features: torch.Tensor):
+    def _encode(self, features, what, lat_lon_heights=None):
+        """Encoder.forward and AssimilatorEncoder.forward; the assimilator's observation graph is uploaded for every call."""
         if features.device.type != "cuda":
-            _no_host_path("Encoder.forward")
+            _no_host_path(what)
         B = features.shape[0]
-        plan = self._own_engine().ensure(features.device, B, _prefixed("encoder", self))
+        eng = _own_engine(self)
+        if lat_lon_heights is None:
+            plan = eng.ensure(features.device, B, _prefixed("encoder", self))
+        else:
+            plan = eng.ensure(features.device, B, _prefixed("encoder", self), grow=dict(n_in=lat_lon_heights.shape[0]))
+            self._upload_obs(eng, plan, lat_lon_heights)
         f = features.detach().to(torch.float32).contiguous()
         x = torch.empty((B * self.num_h3, self.output_dim), dtype=torch.float32, device=f.device)
         plan.encoder_forward(f, x)
         _maybe_check(plan)
         ei, ea = self._latent_outputs(plan, B, f.device)
         return x, ei, ea
+
+    def forward(self, features: torch.Tensor):
+        return self._encode(features, "Encoder.forward")
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -453,19 +469,12 @@ class AssimilatorDecoder(nn.Module):
         g = self._g_dec
         plan.set_decoder_graph(g.src, g.ptr, g.edge_attr)
 
-    def _own_engine(self):
-        if self._engine is None:
-            dims = dict(self._dims)
-            dims["residual_dim"] = self.output_dim if self._residual else 0
-            self._engine = _Engine(dims, self._precision)
-            self._engine.graph_uploaders.append(self._upload_graphs)
-        return self._engine
-
     def _run(self, processor_features, batch_size, start):
         if processor_features.device.type != "cuda":
             _no_host_path("Decoder.forward")
         x = processor_features.detach().to(torch.float32).contiguous()
-        plan = self._own_engine().ensure(x.device, batch_size, _prefixed("decoder", self))
+        eng = _own_engine(self, dict(self._dims, residual_dim=self.output_dim if self._residual else 0))
+        plan = eng.ensure(x.device, batch_size, _prefixed("decoder", self))
         out = torch.empty((batch_size, self.num_latlons, self.output_dim), dtype=torch.float32, device=x.device)
         plan.decoder_forward(x, start, out, batch_size)
         _maybe_check(plan)
@@ -553,32 +562,86 @@ class AssimilatorEncoder(nn.Module):
             plan.set_encoder_graph(g.mesh_local, g.perm, g.ptr, g.edge_attr)
             engine.obs_key = key
 
-    def _own_engine(self):
-        if self._engine is None:
-            self._engine = _Engine(self._dims, self._precision)
-            self._engine.graph_uploaders.append(self._upload_graphs)
-        return self._engine
-
     _latent_outputs = Encoder._latent_outputs
+    _encode = Encoder._encode
 
     def forward(self, features: torch.Tensor, lat_lon_heights: torch.Tensor):
-        if features.device.type != "cuda":
-            _no_host_path("AssimilatorEncoder.forward")
-        B, nobs = features.shape[0], lat_lon_heights.shape[0]
-        eng = self._own_engine()
-        plan = eng.ensure(features.device, B, _prefixed("encoder", self), grow=dict(n_in=nobs))
-        self._upload_obs(eng, plan, lat_lon_heights)
-        f = features.detach().to(torch.float32).contiguous()
-        x = torch.empty((B * self.num_h3, self.output_dim), dtype=torch.float32, device=f.device)
-        plan.encoder_forward(f, x)
-        _maybe_check(plan)
-        ei, ea = self._latent_outputs(plan, B, f.device)
-        return x, ei, ea
+        return self._encode(features, "AssimilatorEncoder.forward", lat_lon_heights)
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # wrappers (forecast.py, analysis.py)
 # ---------------------------------------------------------------------------------------------------------------
+class _Wrapper(nn.Module):
+    """What GraphWeatherForecaster, GraphCast and GraphWeatherAssimilator share: one inference engine over the whole network
+    (encoder -> processor -> decoder in one plan), the training engines of `_TrainFn`, and the dispatch between the two."""
+
+    def _init_engine(self, out_dim, residual_dim, num_blocks, precision, train_precision):
+        """The network's plan dims from the encoder's and decoder's, the inference engine, and the `train_precision` check."""
+        dec = self.decoder._dims
+        dims = dict(self.encoder._dims)
+        dims.update(n_out=self.decoder.num_latlons, n_dec_edges=dec["n_dec_edges"], out_dim=out_dim, residual_dim=residual_dim,
+                    hidden_dec=dec["hidden_dec"], hidden_layers_dec=dec["hidden_layers_dec"], num_blocks=num_blocks)  # fmt: skip
+        self._engine = _new_engine(dims, precision, [self.encoder._upload_graphs, self.decoder._upload_graphs])
+        _validate_train_precision(train_precision, dims)
+        self.train_precision = train_precision
+
+    def _named(self):
+        return [(k, v) for k, v in self.state_dict(keep_vars=True).items()]
+
+    def _out_shape(self, batch):
+        return (batch, self.decoder.num_latlons, self.decoder.output_dim)
+
+    def _bounded_step(self) -> bool:
+        return bool(self.use_checkpointing)
+
+    def _training_engine(self):
+        """The plan the training step runs on, of precision `train_precision`; the inference engine stays as it is.  A
+        tensor-core training precision needs an sm_90 device: elsewhere the first training forward raises.
+
+        `_bounded_step()` (use_checkpointing=True, forecast.py:81; GraphCast adds its checkpoint controls), read at every training
+        forward, selects the step: a training-only plan whose step keeps only the mesh-sized activations and recomputes the
+        grid-sized stages chunk by chunk in the backward -- its working memory does not grow with the grid beyond one chunk (the
+        0.25 degree grid trains on one 80 GB card) -- or the taped step (the default), which is faster where it fits.  Each
+        engine is created on first use.  Only one holds a plan: switching closes the other's, so a backward of a forward made
+        under the other step raises "one backward per forward"."""
+        engines = self.__dict__.setdefault("_train_engines", {})
+        bounded = self._bounded_step()
+        if bounded not in engines:
+            engines[bounded] = _new_engine(self._engine.dims, self.train_precision, [self.encoder._upload_graphs, self.decoder._upload_graphs],
+                                           train_only=bounded)  # fmt: skip
+        other = engines.get(not bounded)
+        if other is not None and other.plan is not None:
+            other.plan.close()
+            other.plan = None
+        self.__dict__["_train_engine"] = engines[bounded]
+        return engines[bounded]
+
+    def _inference_plan(self, features, obs=None):
+        """The inference engine's plan for this batch (and for the assimilator, these observations) with the current weights."""
+        if obs is None:
+            return self._engine.ensure(features.device, features.shape[0], self._named())
+        plan = self._engine.ensure(features.device, features.shape[0], self._named(), grow=dict(n_in=obs.shape[0]))
+        self.encoder._upload_obs(self._engine, plan, obs)
+        return plan
+
+    def _infer(self, features, out, obs=None, out_ld=None):
+        """One inference forward into `out` (a float32 tensor, or the shape of one to allocate)."""
+        plan = self._inference_plan(features, obs)
+        f = features.detach().to(torch.float32).contiguous()
+        if not torch.is_tensor(out):
+            out = torch.empty(out, dtype=torch.float32, device=f.device)
+        plan.forward(f, out, out_ld=out_ld)
+        _maybe_check(plan)
+        return out
+
+    def _train_or_infer(self, features, obs=None):
+        """The training step in train mode with autograd on (`_wants_grad`), otherwise inference."""
+        if _wants_grad(self, features):
+            return _TrainFn.apply(self, features, obs, *[q for _, q in self.named_parameters()])
+        return self._infer(features, self._out_shape(features.shape[0]), obs)
+
+
 @dataclass
 class GraphWeatherForecasterConfig:
     """forecast.py:14-58"""
@@ -607,7 +670,7 @@ class GraphWeatherForecasterConfig:
         return GraphWeatherForecaster(**self.__dict__)
 
 
-class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
+class GraphWeatherForecaster(_Wrapper, PyTorchModelHubMixin):
     """GraphWeatherForecaster(lat_lons)(features): forecast.py:61-247, the main weather prediction model, optionally with physical
     constraints (constraint_type 'additive' | 'multiplicative' | 'softmax', upsampling factor 1); no thermalizer.  Inference and
     training (train mode with autograd on: `loss.backward()` runs the CUDA backward of the network and of the constraint layer)
@@ -656,20 +719,10 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
                                hidden_layers_processor_edge=hidden_layers_processor_edge, mlp_norm_type=norm_type,
                                hidden_dim_decoder=hidden_dim_decoder, hidden_layers_decoder=hidden_layers_decoder,
                                use_checkpointing=use_checkpointing, precision=precision)  # fmt: skip
-        dims = dict(self.encoder._dims)
-        dims.update(n_out=self.decoder.num_latlons, n_dec_edges=self.decoder._dims["n_dec_edges"], out_dim=output_dim,
-                    residual_dim=output_dim, hidden_dec=hidden_dim_decoder, hidden_layers_dec=hidden_layers_decoder,
-                    num_blocks=num_blocks)  # fmt: skip
-        self._engine = _Engine(dims, precision)
-        self._engine.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
-        _validate_train_precision(train_precision, dims)
-        self.train_precision = train_precision
+        self._init_engine(output_dim, output_dim, num_blocks, precision, train_precision)
         if self.constraint_type != "none":  # forecast.py:162-170 (any other string fails at the first forward, as there)
             self.constraint = PhysicalConstraintLayer(model=self, grid_shape=self.grid_shape, constraint_type=constraint_type,
                                                       upsampling_factor=1)  # fmt: skip
-
-    def _named(self):
-        return [(k, v) for k, v in self.state_dict(keep_vars=True).items()]
 
     def graph_to_grid(self, graph_tensor: torch.Tensor) -> torch.Tensor:
         """[B, N, C] -> [B, C, H, W] (forecast.py:194-203)."""
@@ -698,47 +751,19 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
         cell, _ = self._grid_mapping.tensors(out.device)
         return cell.to(torch.int32).contiguous()
 
-    def _training_engine(self):
-        """The plan the training step runs on, of precision `train_precision` (created on first use; the inference engine stays
-        as it is).  A tensor-core training precision needs an sm_90 device: elsewhere the first training forward raises.
-        use_checkpointing=True (forecast.py:81): a training-only plan, whose step keeps only the mesh-sized activations and
-        recomputes the grid-sized stages chunk by chunk in the backward -- its working memory does not grow with the grid beyond
-        one chunk (the 0.25 degree grid trains on one 80 GB card); the taped step (the default) is faster where it fits."""
-        if getattr(self, "_train_engine", None) is None:
-            eng = _Engine(self._engine.dims, self.train_precision, train_only=bool(self.use_checkpointing))
-            eng.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
-            self.__dict__["_train_engine"] = eng
-        return self._train_engine
-
-    def _wants_grad(self, features):
-        return _wants_grad(self, features)
-
-    def _out_shape(self, batch):
-        return (batch, self.decoder.num_latlons, self.output_dim)
-
     def forward(self, features: torch.Tensor, t: int = 0) -> torch.Tensor:
         self._check_features(features)
-        if self._wants_grad(features):
-            # train mode with autograd on, like every training caller of the reference (train/run.py:508-543): the forward keeps
-            # its activations and `loss.backward()` runs the CUDA backward.  Inference (`model.eval()` or `torch.no_grad()`) takes
-            # the tensor-core path below.
-            params = [q for _, q in self.named_parameters()]
-            out = _TrainFn.apply(self, features, None, *params)
-            if self.constraint_type != "none":
-                # forecast.py:235-246 under autograd: the layer's backward adds the gradient of its `lr` input (the first
-                # feature_dim features) to the residual and encoder paths of features.grad
-                cell = self._constraint_cell(out)
-                out = self.constraint.constrain_rows(out, features[..., : self.feature_dim], cell)
+        # train mode with autograd on, like every training caller of the reference (train/run.py:508-543): the forward keeps
+        # its activations and `loss.backward()` runs the CUDA backward.  Inference (`model.eval()` or `torch.no_grad()`) takes
+        # the tensor-core path.
+        out = self._train_or_infer(features)
+        if self.constraint_type == "none":
             return out
-        B = features.shape[0]
-        plan = self._engine.ensure(features.device, B, self._named())
-        f = features.detach().to(torch.float32).contiguous()
-        out = torch.empty((B, self.decoder.num_latlons, self.output_dim), dtype=torch.float32, device=f.device)
-        plan.forward(f, out)
-        if self.constraint_type != "none":
-            out = self._constrain(out, f)
-        _maybe_check(plan)
-        return out
+        if out.requires_grad:
+            # forecast.py:235-246 under autograd: the layer's backward adds the gradient of its `lr` input (the first
+            # feature_dim features) to the residual and encoder paths of features.grad
+            return self.constraint.constrain_rows(out, features[..., : self.feature_dim], self._constraint_cell(out))
+        return self._constrain(out, features)
 
     def forward_into(self, features: torch.Tensor, out: torch.Tensor, peers=None) -> torch.Tensor:
         """forward(features) written into a caller-provided [B, N, output_dim] tensor.  `peers` = (mode, byte deltas) makes the
@@ -748,10 +773,9 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
         self._check_features(features)
         if self.constraint_type != "none":
             raise NotImplementedError("forward_into: the constraint layer post-processes the forecast; gather its output instead")
-        B = features.shape[0]
-        if tuple(out.shape) != (B, self.decoder.num_latlons, self.output_dim) or not out.is_contiguous() or out.dtype != torch.float32:
+        if tuple(out.shape) != self._out_shape(features.shape[0]) or not out.is_contiguous() or out.dtype != torch.float32:
             raise RuntimeError("forward_into: `out` must be a contiguous float32 [B, N, output_dim] tensor")
-        plan = self._engine.ensure(features.device, B, self._named())
+        plan = self._inference_plan(features)
         f = features.detach().to(torch.float32).contiguous()
         if peers is not None:
             plan.set_output_peers(peers[0], peers[1])
@@ -775,7 +799,7 @@ class GraphWeatherForecaster(nn.Module, PyTorchModelHubMixin):
         state if return_all is False)."""
         self._check_features(features)
         B, N, Fin = features.shape
-        plan = self._engine.ensure(features.device, B, self._named())
+        plan = self._inference_plan(features)
         bufs = [features.detach().to(torch.float32).contiguous().clone(), None]
         bufs[1] = bufs[0].clone()  # aux columns are present in both from the start
         outs = torch.empty((steps if return_all else 1, B, N, self.output_dim), dtype=torch.float32, device=features.device)
@@ -822,7 +846,7 @@ class GraphWeatherAssimilatorConfig:
         return GraphWeatherAssimilator(**self.__dict__)
 
 
-class GraphWeatherAssimilator(nn.Module, PyTorchModelHubMixin):
+class GraphWeatherAssimilator(_Wrapper, PyTorchModelHubMixin):
     """GraphWeatherAssimilator(output_lat_lons=..)(features, obs_lat_lon_heights): analysis.py:52-150.  Inference and training
     run on the device.  In train mode with autograd on, `loss.backward()` runs the CUDA backward (`train_precision`, as in
     GraphWeatherForecaster; use_checkpointing=True selects the bounded-memory step).  The observation graph is rebuilt for every
@@ -855,51 +879,20 @@ class GraphWeatherAssimilator(nn.Module, PyTorchModelHubMixin):
                                           hidden_layers_processor_edge=hidden_layers_processor_edge, mlp_norm_type=norm_type,
                                           hidden_dim_decoder=hidden_dim_decoder, hidden_layers_decoder=hidden_layers_decoder,
                                           use_checkpointing=use_checkpointing, precision=precision)  # fmt: skip
-        dims = dict(self.encoder._dims)
-        dims.update(n_out=self.decoder.num_latlons, n_dec_edges=self.decoder._dims["n_dec_edges"], out_dim=analysis_dim,
-                    residual_dim=0, hidden_dec=hidden_dim_decoder, hidden_layers_dec=hidden_layers_decoder, num_blocks=num_blocks)  # fmt: skip
         self.analysis_dim = analysis_dim
         self.use_checkpointing = use_checkpointing
-        self._engine = _Engine(dims, precision)
-        self._engine.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
-        _validate_train_precision(train_precision, dims)
-        self.train_precision = train_precision
-
-    def _named(self):
-        return [(k, v) for k, v in self.state_dict(keep_vars=True).items()]
-
-    def _out_shape(self, batch):
-        return (batch, self.decoder.num_latlons, self.analysis_dim)
-
-    def _training_engine(self):
-        """The plan the training step runs on (created on first use; the inference engine stays as it is), as
-        GraphWeatherForecaster._training_engine.  Its observation graph is built by every training forward."""
-        if getattr(self, "_train_engine", None) is None:
-            eng = _Engine(self._engine.dims, self.train_precision, train_only=bool(self.use_checkpointing))
-            eng.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
-            self.__dict__["_train_engine"] = eng
-        return self._train_engine
+        self._init_engine(analysis_dim, 0, num_blocks, precision, train_precision)
 
     def forward(self, features: torch.Tensor, obs_lat_lon_heights: torch.Tensor) -> torch.Tensor:
         if features.device.type != "cuda":
             _no_host_path("GraphWeatherAssimilator.forward")
-        if _wants_grad(self, features):
-            return _TrainFn.apply(self, features, obs_lat_lon_heights, *[q for _, q in self.named_parameters()])
-        B, nobs = features.shape[0], obs_lat_lon_heights.shape[0]
-        named = self._named()
-        plan = self._engine.ensure(features.device, B, named, grow=dict(n_in=nobs))
-        self.encoder._upload_obs(self._engine, plan, obs_lat_lon_heights)
-        f = features.detach().to(torch.float32).contiguous()
-        out = torch.empty((B, self.decoder.num_latlons, self.analysis_dim), dtype=torch.float32, device=f.device)
-        plan.forward(f, out)
-        _maybe_check(plan)
-        return out
+        return self._train_or_infer(features, obs_lat_lon_heights)
 
 
 # ---------------------------------------------------------------------------------------------------------------
 # GraphCast wrapper (graphcast/model.py)
 # ---------------------------------------------------------------------------------------------------------------
-class GraphCast(nn.Module):
+class GraphCast(_Wrapper):
     """graph_weather/models/graphcast/model.py:21-285: Encoder + Processor + Decoder with hierarchical gradient-checkpoint
     controls and `efficient_batching`.  Efficient and replicated batching are the same computation -- the CUDA path always
     shares one graph across the batch (the reference proves the equivalence in tests/models/layers/test_efficient_batching.py).
@@ -943,39 +936,10 @@ class GraphCast(nn.Module):
         self._checkpoint_encoder = False
         self._checkpoint_processor_segments = 0
         self._checkpoint_decoder = False
-        dims = dict(self.encoder._dims)
-        dims.update(n_out=self.decoder.num_latlons, n_dec_edges=self.decoder._dims["n_dec_edges"], out_dim=output_dim,
-                    residual_dim=output_dim, hidden_dec=hidden_dim, hidden_layers_dec=hidden_layers, num_blocks=num_processor_blocks)  # fmt: skip
-        self._engine = _Engine(dims, precision)
-        self._engine.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
-        _validate_train_precision(train_precision, dims)
-        self.train_precision = train_precision
-
-    def _named(self):
-        return [(k, v) for k, v in self.state_dict(keep_vars=True).items()]
-
-    def _out_shape(self, batch):
-        return (batch, self.decoder.num_latlons, self.output_dim)
+        self._init_engine(output_dim, output_dim, num_processor_blocks, precision, train_precision)
 
     def _bounded_step(self) -> bool:
         return bool(self.use_checkpointing or self._checkpoint_model or self._checkpoint_encoder or self._checkpoint_decoder)
-
-    def _training_engine(self):
-        """The engine of the step the checkpoint controls select now (class docstring): the taped or the bounded one, each
-        created on first use.  Only one holds a plan: switching strategy closes the other's, so a backward of a forward made
-        under the other strategy raises "one backward per forward"."""
-        engines = self.__dict__.setdefault("_train_engines", {})
-        bounded = self._bounded_step()
-        if bounded not in engines:
-            eng = _Engine(self._engine.dims, self.train_precision, train_only=bounded)
-            eng.graph_uploaders += [self.encoder._upload_graphs, self.decoder._upload_graphs]
-            engines[bounded] = eng
-        other = engines.get(not bounded)
-        if other is not None and other.plan is not None:
-            other.plan.close()
-            other.plan = None
-        self.__dict__["_train_engine"] = engines[bounded]
-        return engines[bounded]
 
     # hierarchical checkpointing controls (model.py:118-174)
     def set_checkpoint_model(self, checkpoint_flag: bool):
@@ -1000,15 +964,7 @@ class GraphCast(nn.Module):
         if features.shape[-1] != self.output_dim:  # the reference adds the full input as the residual (model.py:203, decoder.py:93)
             raise RuntimeError(f"The size of tensor a ({self.output_dim}) must match the size of tensor b ({features.shape[-1]}) "
                                "at non-singleton dimension 2")  # fmt: skip
-        if _wants_grad(self, features):
-            return _TrainFn.apply(self, features, None, *[q for _, q in self.named_parameters()])
-        B = features.shape[0]
-        plan = self._engine.ensure(features.device, B, self._named())
-        f = features.detach().to(torch.float32).contiguous()
-        out = torch.empty((B, self.decoder.num_latlons, self.output_dim), dtype=torch.float32, device=f.device)
-        plan.forward(f, out)
-        _maybe_check(plan)
-        return out
+        return self._train_or_infer(features)
 
 
 class GraphCastConfig:

@@ -28,7 +28,7 @@ import torch.nn as nn
 
 from . import graphs, h3lite
 from .dynamic_graph_builder import DynamicGraphBuilder
-from .models import MLP, GraphProcessor, Processor, _Engine, _maybe_check, _no_host_path, _validate_precision
+from .models import MLP, GraphProcessor, Processor, _Engine, _maybe_check, _no_host_path, _validate_precision, _wants_grad
 
 
 @dataclass
@@ -215,7 +215,7 @@ class RegionalForecaster(nn.Module):
             raise ValueError(f"features has {N} rows per sample but lat_lons has {len(lat_lons)} coordinates")
         if features.shape[-1] < self.output_dim:
             raise RuntimeError(f"features needs at least output_dim ({self.output_dim}) channels for the residual add (:288)")
-        if torch.is_grad_enabled() and self.training and (features.requires_grad or any(q.requires_grad for q in self.parameters())):
+        if _wants_grad(self, features):
             # (the forecaster's backward, csrc/gw_train.inl, is not wired to this module: fail instead of returning a tensor
             # that silently carries no graph)
             raise NotImplementedError("RegionalForecaster: the training step is not built; call under torch.no_grad() or in eval() mode")

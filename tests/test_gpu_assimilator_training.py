@@ -18,7 +18,7 @@ import pytest
 import torch
 
 import __graft_entry__ as ge
-from test_gpu_train_precision import ILL_CONDITIONED  # (tests/ is on sys.path: pytest imports its modules by basename)
+from training_oracle import assimilator_oracle_step, check_bf16_bars, check_fp32_bars, rel_norm, train_step
 
 pytestmark = [pytest.mark.gpu, pytest.mark.training]
 
@@ -57,28 +57,9 @@ def _case(setup, n, seed, batch=1):
     return x, _obs(n, seed), target
 
 
-def _oracle(sd, g_static, x, obs, target, dtype=torch.float32):
-    """torch.autograd through analysis.py's forward (assimilator_encoder.py:118-168 + processor + assimilator decoder) and
-    MSELoss: (out, loss, d features, {name: grad})."""
-    from oracle import restate
-
-    sd_g = {k: v.to(dtype).clone().requires_grad_(True) for k, v in sd.items()}
-    g = {k: (v.to(dtype) if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in g_static.items()}
-    xg = x.to(dtype).clone().requires_grad_(True)
-    B, nobs = x.shape[0], obs.shape[0]
-    in_ei, in_ea = restate.assimilator_input_graph(obs, g["base_h3_grid"])
-    h3_nodes = torch.zeros((g["num_h3"], x.shape[-1]), dtype=dtype)
-    feats = torch.cat([xg, h3_nodes.unsqueeze(0).expand(B, -1, -1)], dim=1).reshape(-1, x.shape[-1])
-    h = restate.mlp(sd_g, "encoder.node_encoder", feats)
-    ea = restate.mlp(sd_g, "encoder.edge_encoder", in_ea.to(dtype)).repeat(B, 1)
-    h, _ = restate.graph_processor(sd_g, "encoder.graph_processor", h, restate._replicate(in_ei, B), ea, 1)
-    h = h.reshape(B, -1, h.shape[-1])[:, nobs:, :].reshape(-1, h.shape[-1])
-    lat_ea = restate.mlp(sd_g, "encoder.latent_edge_encoder", g["lat_edge_attr"].repeat(B, 1))
-    h = restate.processor_forward(sd_g, h, restate._replicate(g["lat_edge_index"], B), lat_ea, 9)
-    out = restate.assimilator_decoder_forward(sd_g, g, h, B)
-    loss = torch.nn.functional.mse_loss(out, target.to(dtype))
-    loss.backward()
-    return out.detach(), float(loss.detach()), xg.grad, {k: v.grad for k, v in sd_g.items()}
+def _oracle(sd, g_static, x, obs, target):
+    """The oracle step in fp32 and in fp64."""
+    return [assimilator_oracle_step(sd, g_static, x, obs, target, dt) for dt in (torch.float32, torch.float64)]
 
 
 def _model(setup, tp="fp32_simt", lean=False):
@@ -91,59 +72,24 @@ def _model(setup, tp="fp32_simt", lean=False):
 
 
 def _step(model, x, obs, target):
-    xc = x.cuda().requires_grad_(True)
-    out = model(xc, obs.cuda())
-    assert out.requires_grad
-    loss = torch.nn.functional.mse_loss(out, target.cuda())
-    loss.backward()
-    model._train_engine.plan.status()
-    grads = {k: q.grad.detach().cpu().clone() for k, q in model.named_parameters()}
-    model.zero_grad(set_to_none=True)
-    return out.detach().cpu(), float(loss), xc.grad.cpu(), grads
-
-
-def _rel_max(a, b):
-    return float((a.double() - b.double()).abs().max()) / (float(b.double().abs().max()) + 1e-30)
-
-
-def _rel_norm(a, b):
-    return float((a.double() - b.double()).norm()) / (float(b.double().norm()) + 1e-30)
+    return train_step(model, torch.nn.functional.mse_loss, x, target, obs=obs)
 
 
 def _check(tp, res, ref32, ref64, tag=""):
-    """The bars of tests/test_gpu_training.py (fp32_simt) and tests/test_gpu_lean_training.py (fp32, bf16)."""
-    out, loss, gx, grads = res
-    out32, loss32, gx32, g32 = ref32
-    _, _, gx64, g64 = ref64
-    assert set(grads) == set(g64) and len(grads) == 214
+    """The bars of tests/test_gpu_training.py (fp32_simt) and tests/test_gpu_lean_training.py (fp32, bf16), with the floor on the
+    observation values' gradient too; 214 parameters (the reference keeps the encoder's h3_nodes a plain tensor)."""
     if tp == "bf16":
-        assert float((out - out32).abs().max()) < 2e-2 and abs(loss - loss32) <= 1e-2 * abs(loss32)
-        big = max(float(g.abs().max()) for g in g64.values())
-        for k, g in grads.items():
-            ref = g64[k].double().flatten()
-            if float(ref.abs().max()) <= 1e-6 * big:
-                continue
-            cos = float(torch.nn.functional.cosine_similarity(g.double().flatten(), ref, dim=0))
-            assert cos >= (0.98 if k.startswith(ILL_CONDITIONED) else 0.99), (tag, k, cos)
-        cos = float(torch.nn.functional.cosine_similarity(gx.double().flatten(), gx64.double().flatten(), dim=0))
-        assert cos >= 0.98, (tag, cos)
-        return
-    assert float((out - out32).abs().max()) < 1e-4 and abs(loss - loss32) <= 1e-5 * abs(loss32), tag
-    floor = 2e-3 if tp == "fp32" else 0.0
-    e_ours, e_ref = _rel_max(gx, gx64), _rel_max(gx32, gx64)
-    print(f"{tag} {tp}: d observation values rel err vs fp64 {e_ours:.2e} (fp32 oracle {e_ref:.2e})")
-    assert e_ours < max(10 * e_ref + 2e-5, floor), (tag, e_ours, e_ref)
-    errs = sorted(((_rel_max(grads[k], g64[k]), _rel_max(g32[k], g64[k]), k) for k in grads), reverse=True)
-    print(f"{tag} {tp}: worst rel err vs fp64 {errs[:4]}")
-    for eo, er, k in errs:
-        assert eo < max(10 * er + 2e-5, floor), (tag, k, eo, er)
+        check_bf16_bars(res, ref32, ref64, n_params=214, cos_bar=0.99, ill_cos_bar=0.98, feat_cos=0.98, total_cos=None, tag=tag)
+    else:
+        check_fp32_bars(res, ref32, ref64, n_params=214, floor=2e-3 if tp == "fp32" else 0.0, feat_floor=True, median=False,
+                        ill=None, skip_zero=False, norm_bar=None, tag=f"{tag} {tp}")  # fmt: skip
 
 
 @pytest.fixture(scope="module")
 def case300(setup):
     x, obs, target = _case(setup, 300, 51)
     sd, g = setup[1], setup[2]
-    return x, obs, target, _oracle(sd, g, x, obs, target), _oracle(sd, g, x, obs, target, torch.float64)
+    return (x, obs, target, *_oracle(sd, g, x, obs, target))
 
 
 @pytest.mark.parametrize("lean", [False, True], ids=["taped", "bounded"])
@@ -171,7 +117,7 @@ def test_a_larger_observation_set_regrows_the_plan(setup, case300, monkeypatch, 
     res = _step(model, x2, obs2, target2)
     assert model._train_engine.generation == gen + 1 and model._train_engine.dims["n_in"] == 450
     sd, g = setup[1], setup[2]
-    _check("fp32_simt", res, _oracle(sd, g, x2, obs2, target2), _oracle(sd, g, x2, obs2, target2, torch.float64), "step 2")
+    _check("fp32_simt", res, *_oracle(sd, g, x2, obs2, target2), "step 2")
 
 
 @pytest.mark.parametrize("tp", ["fp32_simt", "bf16"])
@@ -188,9 +134,9 @@ def test_bounded_step_follows_the_observation_graph(setup, monkeypatch, tp):
     assert model._train_engine.generation == gen  # no new plan: the same plan took the second graph
     out_f, loss_f, gx_f, grads_f = _step(_model(setup, tp, True), xb, obs_b, tb)
     assert torch.equal(out, out_f) and loss == loss_f
-    worst = max((_rel_norm(grads[k], g), k) for k, g in grads_f.items() if float(g.norm()) > 0)
-    print(f"{tp}: set A then B vs fresh on B: worst gradient difference {worst}; features {_rel_norm(gx, gx_f):.2e}")
-    assert worst[0] <= 1e-6 and _rel_norm(gx, gx_f) <= 1e-6
+    worst = max((rel_norm(grads[k], g), k) for k, g in grads_f.items() if float(g.norm()) > 0)
+    print(f"{tp}: set A then B vs fresh on B: worst gradient difference {worst}; features {rel_norm(gx, gx_f):.2e}")
+    assert worst[0] <= 1e-6 and rel_norm(gx, gx_f) <= 1e-6
 
 
 @pytest.mark.parametrize("lean", [False, True], ids=["taped", "bounded"])

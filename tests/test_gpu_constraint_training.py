@@ -7,9 +7,8 @@ import pytest
 import torch
 
 import __graft_entry__ as ge
-from test_constraint_grads import _case_ids, fixture_inputs, grid_mapping, load_fixture, restate_constraint, restate_grads, rows_to_grid
-from test_gpu_train_precision import ILL_CONDITIONED
-from test_gpu_training import _grid
+from test_constraint_grads import _case_ids, fixture_inputs, grid_mapping, load_fixture, restate_grads, rows_to_grid
+from training_oracle import check_bf16_bars, check_fp32_bars, forecaster_case, grid, rel_max, rel_norm, train_step
 
 pytestmark = [pytest.mark.gpu, pytest.mark.training]
 
@@ -17,10 +16,6 @@ pytestmark = [pytest.mark.gpu, pytest.mark.training]
 @pytest.fixture(scope="module", autouse=True)
 def _built():
     ge.build()
-
-
-def _rel_max(a, b):
-    return float((a.double().cpu() - b.double().cpu()).abs().max()) / (float(b.double().abs().max()) + 1e-30)
 
 
 def _layer(ll, ctype, exp_factor=1.0):
@@ -45,14 +40,14 @@ def _check_against_oracle(ctype, a, hr, lr, dy, got, grid_shape, cell, last, row
     _, d_hr32, d_lr32 = restate_grads(ctype, hr, lr, dy, grid_shape, cell, last, a, torch.float32, rows=rows)
     _, d_hr64, d_lr64 = restate_grads(ctype, hr, lr, dy, grid_shape, cell, last, a, torch.float64, rows=rows)
     _, g_hr, g_lr = got
-    e_lr, r_lr = _rel_max(g_lr, d_lr64), _rel_max(d_lr32, d_lr64)
+    e_lr, r_lr = rel_max(g_lr, d_lr64), rel_max(d_lr32, d_lr64)
     assert e_lr <= max(10 * r_lr, 2e-6), (what, "d_lr", e_lr, r_lr)
     if ctype == "softmax":
         # d_hr is analytically 0: both are rounding noise, ours within a few times the reference's own noise
         noise = 4 * float(d_hr32.abs().max()) + 1e-7 * float(dy.abs().max() * lr.abs().max() * a)
         assert float(g_hr.abs().max()) <= noise, (what, float(g_hr.abs().max()), noise)
     else:
-        e_hr, r_hr = _rel_max(g_hr, d_hr64), _rel_max(d_hr32, d_hr64)
+        e_hr, r_hr = rel_max(g_hr, d_hr64), rel_max(d_hr32, d_hr64)
         assert e_hr <= max(10 * r_hr, 2e-6), (what, "d_hr", e_hr, r_hr)
     return d_hr32, d_lr32
 
@@ -103,7 +98,7 @@ def _regular(step_lat=20, step_lon=22.5):
 @pytest.mark.parametrize("ctype,a", [("additive", 1.0), ("multiplicative", 1.0), ("softmax", 1.0), ("softmax", 0.5)])
 def test_layer_on_the_10_degree_grid(ctype, a):
     """B = 2, C = 78 rows as the forecaster passes them (lr = the first 78 of 102 feature columns, a strided view)."""
-    ll = _grid(10)
+    ll = grid(10)
     grid_shape, cell, last = grid_mapping(ll)
     g = torch.Generator().manual_seed(5)
     hr = torch.randn(2, len(ll), 78, generator=g)
@@ -136,7 +131,7 @@ def test_additive_exact_integers_bit_for_bit():
 
 def test_additive_gradient_sums_to_zero():
     """y = hr + lr - mean(hr): shifting hr by a constant leaves y unchanged, so sum_r d_hr = 0 per sample and channel."""
-    ll = _grid(10)
+    ll = grid(10)
     grid_shape, _, _ = grid_mapping(ll)
     g = torch.Generator().manual_seed(4)
     hr, lr, dy = (torch.randn(2, len(ll), 78, generator=g) for _ in range(3))
@@ -207,42 +202,10 @@ def test_no_grad_path_is_unchanged(fixture_case):
 SHIFT = {"additive": 0.0, "multiplicative": 3.0, "softmax": 0.0}
 
 
-def _oracle_step(sd, ll, x, target, var, ctype, dtype):
-    """tests/test_gpu_training.py's oracle step with the restated constraint layer appended (forecast.py:235-246)."""
-    from oracle import restate
-
-    grid_shape, cell, last = grid_mapping(ll)
-    sd_g = {k: v.to(dtype).clone().requires_grad_(True) for k, v in sd.items()}
-    xg = x.to(dtype).clone().requires_grad_(True)
-    g = {k: (v.to(dtype) if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in restate.build_forecaster_graphs(ll).items()}
-    ex, ei, ea = restate.encoder_forward(sd_g, g, xg)
-    px = restate.processor_forward(sd_g, ex, ei, ea, 9)
-    out = restate.assimilator_decoder_forward(sd_g, g, px, x.shape[0]) + xg[..., :78]
-    out = restate_constraint(ctype, rows_to_grid(out, grid_shape), rows_to_grid(xg[..., :78], grid_shape), grid_shape, cell, last)
-    loss = restate.normalized_mse_loss(out, target.to(dtype), var, ll, True)
-    loss.backward()
-    return out.detach(), float(loss.detach()), xg.grad, {k: v.grad for k, v in sd_g.items()}
-
-
-_ORACLE = {}
-
-
 def _case(ctype):
     """The seeded 10-degree, batch-2 case of tests/test_gpu_train_precision.py (the first 78 input channels shifted by SHIFT[ctype])
-    and its oracle steps in fp32 and fp64."""
-    from oracle import weights
-
-    if ctype not in _ORACLE:
-        ll = _grid(10)
-        sd = weights.make_state_dict(weights.forecaster_shapes(), 21)
-        x = weights.make_features(2, len(ll), 102, 21)
-        x[..., :78] += SHIFT[ctype]
-        rng = np.random.Generator(np.random.PCG64(21))
-        target = torch.from_numpy(rng.standard_normal((2, len(ll), 78)).astype(np.float32))
-        var = rng.uniform(0.5, 2.0, 78).astype(np.float32).tolist()
-        _ORACLE[ctype] = (ll, sd, x, target, var, _oracle_step(sd, ll, x, target, var, ctype, torch.float32),
-                          _oracle_step(sd, ll, x, target, var, ctype, torch.float64))  # fmt: skip
-    return _ORACLE[ctype]
+    and its oracle steps, with the restated layer appended, in fp32 and fp64."""
+    return forecaster_case(10, 2, 21, constraint=ctype, shift=SHIFT[ctype])
 
 
 def _step(ctype, tp, ll, sd, x, target, var):
@@ -250,22 +213,7 @@ def _step(ctype, tp, ll, sd, x, target, var):
 
     model = GraphWeatherForecaster(ll, constraint_type=ctype, train_precision=tp).cuda().train()
     model.load_state_dict(sd)
-    crit = NormalizedMSELoss(var, ll, normalize=True)
-    xc = x.cuda().requires_grad_(True)
-    out = model(xc)
-    loss = crit(out, target.cuda())
-    loss.backward()
-    model._train_engine.plan.status()
-    grads = {k: q.grad.detach().cpu() for k, q in model.named_parameters()}
-    return model, out.detach().cpu(), float(loss.detach()), xc.grad.cpu(), grads
-
-
-def _rel_norm(a, b):
-    return float((a.double() - b.double()).norm()) / (float(b.double().norm()) + 1e-30)
-
-
-def _cos(a, b):
-    return float(torch.nn.functional.cosine_similarity(a.double().flatten(), b.double().flatten(), dim=0))
+    return train_step(model, NormalizedMSELoss(var, ll, normalize=True), x, target)
 
 
 # Additive on tensor cores.  y = hr + lr - mean(hr) centres the gradient entering the network (sum_r d_hr = 0 per sample and channel,
@@ -283,22 +231,24 @@ ADDITIVE_TC_NORM, ADDITIVE_TC_COS = 1e-2, 0.9
 @pytest.mark.parametrize("tp", ["fp32_simt", "fp32", "bf16"])
 @pytest.mark.parametrize("ctype", ["additive", "multiplicative", "softmax"])
 def test_constrained_training_step_matches_the_oracle(ctype, tp):
-    ll, sd, x, target, var, (out32, loss32, gx32, g32), (_, _, gx64, g64) = _case(ctype)
-    model, out, loss, gx, grads = _step(ctype, tp, ll, sd, x, target, var)
-    assert float((out - out32).abs().max()) < (2e-2 if tp == "bf16" else 1e-4)
-    assert abs(loss - loss32) <= (1e-2 if tp == "bf16" else 1e-5) * abs(loss32)
+    ll, sd, x, target, var, ref32, ref64 = _case(ctype)
+    out, loss, gx, grads = _step(ctype, tp, ll, sd, x, target, var)
     assert len(grads) == 215
-    # features.grad: the network's paths plus the layer's lr path
+    tag = f"{ctype} {tp}"
+    # features.grad: the network's paths plus the layer's lr path.  Softmax: the layer returns lr up to rounding, so d out / d hr
+    # is 0 and every parameter gradient is rounding noise: those are measured against the unconstrained step below instead (not
+    # against the additive step, whose last decoder bias has a zero gradient of its own).
+    ours = (out, loss, gx, None if ctype == "softmax" else grads)
     if tp == "bf16":
-        assert _cos(gx, gx64) >= 0.99
+        cos_bar, ill_cos_bar = (ADDITIVE_TC_COS, ADDITIVE_TC_COS) if ctype == "additive" else (0.99, 0.98)
+        check_bf16_bars(ours, ref32, ref64, n_params=215, cos_bar=cos_bar, ill_cos_bar=ill_cos_bar, feat_cos=0.99, total_cos=None,
+                        tag=tag)  # fmt: skip
     else:
-        e, r = _rel_max(gx, gx64), _rel_max(gx32, gx64)
-        print(f"{ctype} {tp}: d loss / d features rel err vs fp64 {e:.2e} (fp32 oracle {r:.2e})")
-        assert e < max(10 * r + 2e-5, 2e-3)
+        # numerically zero gradients (additive: the last decoder bias) are left out: their direction is noise
+        check_fp32_bars(ours, ref32, ref64, n_params=215, floor=2e-3, feat_floor=True, median=False, ill="max", skip_zero=True,
+                        norm_bar=ADDITIVE_TC_NORM if (ctype, tp) == ("additive", "fp32") else None, tag=tag)  # fmt: skip
     if ctype == "softmax":
-        # the layer returns lr up to rounding: d out / d hr is 0 and every parameter gradient is rounding noise.  (Measured against
-        # the unconstrained step: the additive step's last decoder bias has a zero gradient of its own.)
-        _, _, _, _, g_plain = _step("none", tp, ll, sd, x, target, var)
+        _, _, _, g_plain = _step("none", tp, ll, sd, x, target, var)
         worst = 0.0
         for k, gr in grads.items():
             assert torch.isfinite(gr).all(), k
@@ -306,28 +256,6 @@ def test_constrained_training_step_matches_the_oracle(ctype, tp):
             worst = max(worst, ratio)
             assert ratio <= 1e-4, (k, ratio)
         print(f"softmax {tp}: worst max|grad| / unconstrained {worst:.2e}")
-        return
-    big = max(float(g.abs().max()) for g in g64.values())
-    worst = []
-    for k, gr in grads.items():
-        if float(g64[k].abs().max()) <= 1e-6 * big:
-            continue  # numerically zero gradient (additive: the last decoder bias): its direction is noise
-        ill = k.startswith(ILL_CONDITIONED)
-        if tp == "bf16":
-            cos = _cos(gr, g64[k])
-            worst.append((cos, k))
-            assert cos >= (ADDITIVE_TC_COS if ctype == "additive" else 0.98 if ill else 0.99), (k, cos)
-        elif ctype == "additive" and tp == "fp32":
-            en = _rel_norm(gr, g64[k])
-            worst.append((en, k))
-            assert en < ADDITIVE_TC_NORM, (k, en)
-        else:
-            eo, er = _rel_max(gr, g64[k]), _rel_max(g32[k], g64[k])
-            bar = max(10 * er + 2e-5, 2e-3) * (5 if ill else 1)
-            worst.append((eo / bar, k))
-            assert eo < bar, (k, eo, er)
-    worst.sort(reverse=tp != "bf16")
-    print(f"{ctype} {tp}: worst {worst[:4]}")
 
 
 @pytest.mark.parametrize("tp", ["fp32", "bf16"])
@@ -362,7 +290,7 @@ def test_constrained_step_is_the_network_backward_of_the_layer_gradient(ctype, t
             assert torch.equal(a, b), k
             linear += 1
         else:
-            assert _rel_norm(a, b) <= 1e-5, (k, _rel_norm(a, b))
+            assert rel_norm(a, b) <= 1e-5, (k, rel_norm(a, b))
     assert linear > 100
 
 
@@ -371,7 +299,7 @@ def test_constrained_train_output_is_the_layer_on_the_plain_output(ctype):
     """Bit for bit: the constrained train-mode output is apply_rows (no grad) on the unconstrained train-mode output."""
     from graph_weather_b200 import GraphWeatherForecaster
 
-    ll, sd, x = _case_inputs(ctype)
+    ll, sd, x = _case(ctype)[:3]
     outs = {}
     for c in (ctype, "none"):
         model = GraphWeatherForecaster(ll, constraint_type=c, train_precision="fp32").cuda().train()
@@ -385,23 +313,13 @@ def test_constrained_train_output_is_the_layer_on_the_plain_output(ctype):
     assert torch.equal(y.detach(), ref)
 
 
-def _case_inputs(ctype):
-    from oracle import weights
-
-    ll = _grid(10)
-    sd = weights.make_state_dict(weights.forecaster_shapes(), 21)
-    x = weights.make_features(2, len(ll), 102, 21)
-    x[..., :78] += SHIFT[ctype]
-    return ll, sd, x
-
-
 def test_loss_falls_at_one_degree():
     """1-degree grid, additive constraint, bf16: four AdamW steps on a fixed batch lower the loss (seeded weights, as the
     1-degree step of tests/test_gpu_train_precision.py)."""
     from graph_weather_b200 import GraphWeatherForecaster, NormalizedMSELoss
     from oracle import weights
 
-    ll = _grid(1)
+    ll = grid(1)
     model = GraphWeatherForecaster(ll, constraint_type="additive", train_precision="bf16").cuda().train()
     model.load_state_dict(weights.make_state_dict(weights.forecaster_shapes(), 5))
     crit = NormalizedMSELoss([1.0] * 78, ll, normalize=True)

@@ -8,8 +8,7 @@ import pytest
 import torch
 
 import __graft_entry__ as ge
-from test_gpu_train_precision import ILL_CONDITIONED  # (tests/ is on sys.path: pytest imports its modules by basename)
-from test_gpu_training import _grid, _oracle_step
+from training_oracle import ILL_CONDITIONED, check_bf16_bars, check_fp32_bars, forecaster_case, grid, rel_norm, train_step
 
 pytestmark = [pytest.mark.gpu, pytest.mark.training]
 
@@ -22,40 +21,18 @@ def _built():
 @pytest.fixture(scope="module")
 def case10():
     """The seeded 10-degree, batch-2 step of tests/test_gpu_training.py and its oracle results (fp32 and fp64)."""
-    from oracle import weights
-
-    ll = _grid(10)
-    sd = weights.make_state_dict(weights.forecaster_shapes(), 21)
-    x = weights.make_features(2, len(ll), 102, 21)
-    rng = np.random.Generator(np.random.PCG64(21))
-    target = torch.from_numpy(rng.standard_normal((2, len(ll), 78)).astype(np.float32))
-    var = rng.uniform(0.5, 2.0, 78).astype(np.float32).tolist()
-    return ll, sd, x, target, var, _oracle_step(sd, ll, x, target, var), _oracle_step(sd, ll, x, target, var, torch.float64)
+    return forecaster_case(10, 2, 21)
 
 
 def _step(tp, ll, sd, x, target, var, lean, feat_grad=True, **kw):
-    """One training forward + loss + backward; returns (model, out, loss, d features, {name: grad})."""
+    """One training step of a fresh forecaster: (model, out, loss, d features, {name: grad})."""
     from graph_weather_b200 import GraphWeatherForecaster, NormalizedMSELoss
 
     model = GraphWeatherForecaster(ll, train_precision=tp, use_checkpointing=lean, **kw).cuda().train()
     model.load_state_dict(sd)
-    crit = NormalizedMSELoss(var, ll, normalize=True)
-    xc = x.cuda().requires_grad_(feat_grad)
-    out = model(xc)
-    loss = crit(out, target.cuda())
-    loss.backward()
-    model._train_engine.plan.status()
+    res = train_step(model, NormalizedMSELoss(var, ll, normalize=True), x, target, feat_grad=feat_grad)
     assert model._train_engine.plan.train_only == lean
-    grads = {k: q.grad.detach().cpu() for k, q in model.named_parameters()}
-    return model, out.detach().cpu(), float(loss), (xc.grad.cpu() if feat_grad else None), grads
-
-
-def _rel_max(a, b):
-    return float((a.double() - b.double()).abs().max()) / (float(b.double().abs().max()) + 1e-30)
-
-
-def _rel_norm(a, b):
-    return float((a.double() - b.double()).norm()) / (float(b.double().norm()) + 1e-30)
+    return (model, *res)
 
 
 # chunk sizes of the 10-degree grid: one point (every encoder chunk is one mesh slot, every decoder chunk one point), a
@@ -72,36 +49,22 @@ def test_forward_equals_the_taped_step(case10, monkeypatch, tp, chunk):
     _, out_l, loss_l, gx_l, g_l = _step(tp, ll, sd, x, target, var, True)
     assert torch.equal(out_l, out_t)
     assert loss_l == loss_t
-    worst = max((_rel_norm(g_l[k], g), k) for k, g in g_t.items() if float(g.norm()) > 0)
-    print(f"{tp} chunk {chunk}: worst norm-relative gradient difference to the taped step {worst}; features {_rel_norm(gx_l, gx_t):.2e}")
-    assert worst[0] <= 1e-5 and _rel_norm(gx_l, gx_t) <= 1e-5
+    worst = max((rel_norm(g_l[k], g), k) for k, g in g_t.items() if float(g.norm()) > 0)
+    print(f"{tp} chunk {chunk}: worst norm-relative gradient difference to the taped step {worst}; features {rel_norm(gx_l, gx_t):.2e}")
+    assert worst[0] <= 1e-5 and rel_norm(gx_l, gx_t) <= 1e-5
 
 
 @pytest.mark.parametrize("tp", ["fp32_simt", "fp32", "bf16"])
 def test_gradients_match_the_oracle(case10, monkeypatch, tp):
     """10 degrees, batch 2, 18 decoder chunks: the bars test_gpu_training.py / test_gpu_train_precision.py hold the taped step to."""
-    ll, sd, x, target, var, (out32, loss32, gx32, g32), (_, loss64, gx64, g64) = case10
+    ll, sd, x, target, var, ref32, ref64 = case10
     monkeypatch.setenv("GW_B200_TRAIN_CHUNK", "37")
-    model, out, loss, gx, grads = _step(tp, ll, sd, x, target, var, True)
-    assert len(grads) == 215
+    _, *ours = _step(tp, ll, sd, x, target, var, True)
     if tp == "bf16":
-        assert float((out - out32).abs().max()) < 2e-2 and abs(loss - loss32) <= 1e-2 * abs(loss32)
-        big = max(float(g.abs().max()) for g in g64.values())
-        for k, g in grads.items():
-            ref = g64[k].double().flatten()
-            if float(ref.abs().max()) <= 1e-6 * big:
-                continue
-            cos = float(torch.nn.functional.cosine_similarity(g.double().flatten(), ref, dim=0))
-            assert cos >= (0.98 if k.startswith(ILL_CONDITIONED) else 0.99), (k, cos)
-        return
-    assert float((out - out32).abs().max()) < 1e-4 and abs(loss - loss32) <= 1e-5 * abs(loss32)
-    floor = 2e-3 if tp == "fp32" else 0.0
-    e_ours, e_ref = _rel_max(gx, gx64), _rel_max(gx32, gx64)
-    assert e_ours < 10 * e_ref + 2e-5, (e_ours, e_ref)
-    errs = sorted(((_rel_max(grads[k], g64[k]), _rel_max(g32[k], g64[k]), k) for k in grads), reverse=True)
-    print(f"{tp}: worst rel err vs fp64 {errs[:4]}")
-    for eo, er, k in errs:
-        assert eo < max(10 * er + 2e-5, floor), (k, eo, er)
+        check_bf16_bars(ours, ref32, ref64, n_params=215, cos_bar=0.99, ill_cos_bar=0.98, feat_cos=None, total_cos=None)
+    else:
+        check_fp32_bars(ours, ref32, ref64, n_params=215, floor=2e-3 if tp == "fp32" else 0.0, feat_floor=False, median=False,
+                        ill=None, skip_zero=False, norm_bar=None)  # fmt: skip
 
 
 @pytest.mark.parametrize("tp", ["fp32", "bf16"])
@@ -130,7 +93,7 @@ def test_wide_model(monkeypatch):
     """train/run_fulll.py's 597 + 24 features (6 blocks here 2), fp32_simt, 10 degrees, batch 2, many chunks vs the taped step."""
     from oracle import weights
 
-    ll = _grid(10)
+    ll = grid(10)
     kw = dict(feature_dim=597, aux_dim=24, num_blocks=2)
     from graph_weather_b200 import GraphWeatherForecaster
 
@@ -143,8 +106,8 @@ def test_wide_model(monkeypatch):
     monkeypatch.setenv("GW_B200_TRAIN_CHUNK", "37")
     _, out_l, loss_l, gx_l, g_l = _step("fp32_simt", ll, sd, x, target, var, True, **kw)
     assert torch.equal(out_l, out_t) and loss_l == loss_t
-    worst = max((_rel_norm(g_l[k], g), k) for k, g in g_t.items() if float(g.norm()) > 0)
-    assert worst[0] <= 1e-5 and _rel_norm(gx_l, gx_t) <= 1e-5, worst
+    worst = max((rel_norm(g_l[k], g), k) for k, g in g_t.items() if float(g.norm()) > 0)
+    assert worst[0] <= 1e-5 and rel_norm(gx_l, gx_t) <= 1e-5, worst
 
 
 @pytest.mark.parametrize("ctype", ["additive", "softmax"])
@@ -157,14 +120,14 @@ def test_constrained_step(case10, monkeypatch, ctype):
     # (under the additive constraint the last decoder bias has an analytically zero gradient, sum_r d_hr = 0: its computed value
     # is rounding noise in both steps, so numerically zero gradients are left out)
     big = max(float(g.norm()) for g in g_t.values())
-    worst = max((_rel_norm(g_l[k], g), k) for k, g in g_t.items() if float(g.norm()) > 1e-6 * big)
-    assert worst[0] <= 1e-5 and _rel_norm(gx_l, gx_t) <= 1e-5, worst
+    worst = max((rel_norm(g_l[k], g), k) for k, g in g_t.items() if float(g.norm()) > 1e-6 * big)
+    assert worst[0] <= 1e-5 and rel_norm(gx_l, gx_t) <= 1e-5, worst
 
 
 def _one_degree():
     from oracle import weights
 
-    ll = _grid(1)
+    ll = grid(1)
     sd = weights.make_state_dict(weights.forecaster_shapes(), 5)
     x = weights.make_features(1, len(ll), 102, 5)
     rng = np.random.Generator(np.random.PCG64(5))
@@ -186,13 +149,13 @@ def test_one_degree_against_the_taped_step(tp):
         assert float((out_l - out_t).abs().max()) < 1e-4
     else:
         assert torch.equal(out_l, out_t)
-    errs = sorted(((_rel_norm(g_l[k], g), k) for k, g in g_t.items() if float(g.norm()) > 0), reverse=True)
+    errs = sorted(((rel_norm(g_l[k], g), k) for k, g in g_t.items() if float(g.norm()) > 0), reverse=True)
     print(f"1 deg {tp}: loss {loss_l:.7f} vs {loss_t:.7f}; peak {peak_l / 2**30:.2f} GiB vs taped {peak_t / 2**30:.2f} GiB; "
           f"above 1e-5: {[(f'{e:.1e}', k) for e, k in errs if e > 1e-5]}")
     # Bars.  fp32_simt: only the summation order of dPd and of the weight gradients differs (measured <= 1.3e-6).  fp32: each chunk's
     # operands are scaled from the chunk's magnitudes, so activations differ in their last bits too (measured 1.5e-5).  bf16: the
     # forward is identical, but a last-bit difference of dPd flips the bf16 rounding of single operands of every data gradient
-    # upstream; the tensors summed over the whole graph (ILL_CONDITIONED, test_gpu_train_precision.py) magnify it (measured 1.7e-3
+    # upstream; the tensors summed over the whole graph (ILL_CONDITIONED, tests/training_oracle.py) magnify it (measured 1.7e-3
     # for h3_nodes, 5.6e-4 for node_encoder.model.0.weight, at most 4.9e-5 for every other parameter).
     for e, k in errs:
         bar = {"fp32_simt": 1e-5, "fp32": 5e-5, "bf16": 5e-3 if k.startswith(ILL_CONDITIONED) else 2e-4}[tp]
@@ -204,7 +167,7 @@ def test_memory_does_not_grow_with_the_grid(monkeypatch):
     from graph_weather_b200 import GraphWeatherForecaster
 
     def peak(step, lean):
-        ll = _grid(step)
+        ll = grid(step)
         model = GraphWeatherForecaster(ll, train_precision="bf16", use_checkpointing=lean).cuda().train()
         x = torch.randn(1, len(ll), 102, device="cuda")
         model(x).square().mean().backward()

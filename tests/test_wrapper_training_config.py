@@ -94,3 +94,15 @@ def test_graphcast_strategy_selects_the_step():
     assert g._training_engine().train_only is True
     assert g._engine.train_only is False
     assert GraphCast(LL, num_processor_blocks=1, use_checkpointing=True)._training_engine().train_only is True
+
+
+def test_use_checkpointing_assigned_later_selects_the_step():
+    """Every wrapper reads use_checkpointing at each training forward, as GraphCast reads its checkpoint controls."""
+    from graph_weather_b200 import GraphCast, GraphWeatherAssimilator, GraphWeatherForecaster
+
+    for m in (GraphWeatherForecaster(LL, num_blocks=1), GraphWeatherAssimilator(output_lat_lons=LL, analysis_dim=5, num_blocks=1),
+              GraphCast(LL, num_processor_blocks=1)):  # fmt: skip
+        for flag in (False, True, False):
+            m.use_checkpointing = flag
+            assert m._training_engine().train_only is flag, type(m).__name__
+            assert m._train_engine is m._training_engine()
