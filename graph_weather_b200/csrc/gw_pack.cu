@@ -56,11 +56,15 @@ cudaError_t launch_pack_weights(const float* W, int ldw, int K_src, int N_src, f
   return cudaGetLastError();
 }
 
+// max |W| of a weight view; a NaN entry makes it +inf (fmaxf would drop the NaN and leave it finite), so that the chain's operand
+// range ladder flags non-finite weights, biases and LayerNorm parameters (status bit 3)
 __global__ void gw_absmax_kernel(const float* __restrict__ W, int ldw, int K_src, int N_src, float* out_max) {
   float m = 0.f;
   const size_t total = (size_t)N_src * K_src;
-  for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x)
-    m = fmaxf(m, fabsf(W[(e / K_src) * (size_t)ldw + (e % K_src)]));
+  for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    const float a = fabsf(W[(e / K_src) * (size_t)ldw + (e % K_src)]);
+    m = a <= m ? m : (a == a ? a : __int_as_float(0x7f800000));
+  }
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int*>(out_max), __float_as_int(m));  // m >= 0: int order == float order
 }

@@ -42,7 +42,7 @@ __device__ __forceinline__ float fetch_src(const RowSrc& s, int b, int i, int k)
     case SRC_GATHER_BCAST_RELU: {
       float v = __ldg(s.base + ((size_t)b * s.src_rows + __ldg(s.idx + i)) * s.ld + s.col0 + k) +
                 __ldg(s.base2 + (size_t)i * s.ld2 + k);
-      return fmaxf(v, 0.f);
+      return v < 0.f ? 0.f : v;  // torch.relu: a NaN passes through (fmaxf would return 0)
     }
     default:
       return 0.f;
@@ -125,7 +125,7 @@ __global__ void __launch_bounds__(NT) gw_rowop_f32_kernel(const GemmOp op) {
 #pragma unroll
         for (int s = 0; s < 3; ++s)
           if (op.add[s].kind != SRC_NONE) x += fetch_src(op.add[s], b, li, gn);
-        if (op.relu) x = fmaxf(x, 0.f);
+        if (op.relu) x = x < 0.f ? 0.f : x;  // torch.relu: NaN stays NaN, -0.0 stays -0.0
       } else {
         x = 0.f;
       }
@@ -168,7 +168,8 @@ __global__ void __launch_bounds__(NT) gw_rowop_f32_kernel(const GemmOp op) {
         if (gn < N) {
           float x = v[j];
           if (op.residual.kind != SRC_NONE) x += fetch_src(op.residual, b, li, gn);
-          if (op.mask.kind != SRC_NONE && !(fetch_src(op.mask, b, li, gn) > 0.f)) x = 0.f;
+          // torch's threshold_backward: zero where mask <= 0, so a NaN mask entry lets the gradient through
+          if (op.mask.kind != SRC_NONE && fetch_src(op.mask, b, li, gn) <= 0.f) x = 0.f;
           op.out[(size_t)gr * op.ldo + gn] = x;
         }
       }

@@ -293,9 +293,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gw_chain_tc3_kernel(const __gr
       const float wa = ldbound(L.wamax);
       const float winv = L.wamax ? 1.f / tc_weight_scale(wa, ch.split ? 2 : 1) : L.wscale_inv, gain = L.wamax ? (float)L.K * wa : L.gain;
       scl[2 * l] = winv / sc;  // (a reuse_a layer multiplies the same operand: m and sc are unchanged)
-      float mo = L.ln_g ? L.ln_bound : fmaf(m, gain, L.off) + srcbound(L.add[0]) + srcbound(L.add[1]);
+      // (a LayerNorm'd row is bounded by its parameters alone, but the value it normalises must be finite too: a NaN bias there
+      // would make the whole row NaN)
+      const float pre = fmaf(m, gain, L.off) + srcbound(L.add[0]) + srcbound(L.add[1]);
+      float mo = L.ln_g ? L.ln_bound : pre;
       mo += srcbound(L.residual);
-      bad = bad || !(mo < 3.0e38f);
+      bad = bad || !(mo < 3.0e38f) || !(pre < 3.0e38f);
       if (blockIdx.x == 0) {
         if (L.out_bound) {  // (two layers may fill halves of one tensor: its bound is the larger one)
           const bool again = l > 0 && ch.layer[l - 1].out_bound == L.out_bound;

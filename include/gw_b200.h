@@ -181,8 +181,10 @@ int gw_latent_edge_features(gw_plan* plan, float* edge_attr_out, void* stream);
 
 /* Synchronises `stream` and returns (then clears) the plan's device status word: 0 = ok;
  * bit 0: an activation left the fp16 range in GW_PREC_FP32_TC (results invalid: rerun with GW_PREC_FP32_SIMT);
- * bit 1: internal pipeline timeout; bit 2: shared-memory misalignment; bit 3: a magnitude bound overflowed (inf / nan
- * inputs); bit 4: an observation could not be located on the mesh (non-finite coordinates).  Non-zero must be treated as failure.  (Operands are range-scaled from rigorous per-tensor magnitude bounds, so
+ * bit 1: internal pipeline timeout; bit 2: shared-memory misalignment; bit 3: a magnitude bound is not finite: the features or
+ * a weight matrix hold an inf / NaN (inference also checks every bias and LayerNorm parameter).  The tensor-core precisions,
+ * GW_PREC_FP32_TC and GW_PREC_BF16_TC, refuse such inputs this way in inference and in both training steps; GW_PREC_FP32_SIMT
+ * never sets it and propagates them as torch does; bit 4: an observation could not be located on the mesh (non-finite coordinates).  Non-zero must be treated as failure.  (Operands are range-scaled from rigorous per-tensor magnitude bounds, so
  * bit 0 is a guard that finite inputs cannot trip.) */
 int gw_plan_status(gw_plan* plan, int32_t* status_out, void* stream);
 /* Non-blocking read of the same word (it lives in host-mapped memory): reflects every kernel that has COMPLETED so far
