@@ -7,6 +7,7 @@ from __future__ import annotations
 import ctypes
 import os
 import re
+import weakref
 
 import torch
 
@@ -76,6 +77,11 @@ _SIGNATURES = {
     "gw_train_forward": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp]),
     "gw_train_backward": (ctypes.c_int, [_vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
     "gw_train_peak_bytes": (_i64, [_vp]),
+    "gw_tape_create": (ctypes.c_int, [_vp, ctypes.POINTER(_vp)]),
+    "gw_tape_destroy": (ctypes.c_int, [_vp, _vp]),
+    "gw_train_forward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp]),
+    "gw_train_backward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
+    "gw_tape_bytes": (_i64, [_vp]),
     "gw_launch_count": (_i64, []),
     "gw_launch_count_reset": (None, []),
 }
@@ -156,6 +162,7 @@ class Plan:
         with torch.cuda.device(self.device):
             _check(create(ctypes.byref(self.dims), ctypes.byref(self.handle)))
         self._keep = []
+        self._tapes = weakref.WeakSet()
 
     def close(self):
         if getattr(self, "handle", None) is not None and self.handle.value:
@@ -288,18 +295,32 @@ class Plan:
             _check(self.lib.gw_train_forward(self.handle, _ptr(features, torch.float32, d), _ptr(out, torch.float32, d), int(features.shape[0]),
                                              _stream(d)))  # fmt: skip
 
-    def train_backward(self, grad_out, grad_features, named_grads):
-        """grad_out [B, N, out] -> gradients written into `named_grads` (reference parameter name -> tensor shaped like the
-        parameter) and, if given, the gradient of the features."""
-        d = self.device
+    def _grad_table(self, named_grads):
         items = list(named_grads)
         arr = (GwParam * max(1, len(items)))()
         for i, (k, v) in enumerate(items):
             rows, cols = (v.shape[0], v.shape[1]) if v.dim() == 2 else (v.numel(), 1)
-            arr[i] = GwParam(k.encode(), _ptr(v, torch.float32, d).value, rows, cols)
+            arr[i] = GwParam(k.encode(), _ptr(v, torch.float32, self.device).value, rows, cols)
+        return arr, len(items)
+
+    def train_backward(self, grad_out, grad_features, named_grads):
+        """grad_out [B, N, out] -> gradients written into `named_grads` (reference parameter name -> tensor shaped like the
+        parameter) and, if given, the gradient of the features."""
+        d = self.device
+        arr, n = self._grad_table(named_grads)
         with torch.cuda.device(d):
             gf = _ptr(grad_features, torch.float32, d) if grad_features is not None else _vp()
-            _check(self.lib.gw_train_backward(self.handle, _ptr(grad_out, torch.float32, d), gf, arr, len(items), _stream(d)))
+            _check(self.lib.gw_train_backward(self.handle, _ptr(grad_out, torch.float32, d), gf, arr, n, _stream(d)))
+
+    def tape(self) -> "Tape":
+        """A new tape of this plan (gw_tape_create): one more training forward that stays differentiable alongside the others."""
+        t = Tape(self)
+        self._tapes.add(t)
+        return t
+
+    def live_tapes(self):
+        """The tapes made by `tape()` that are not destroyed yet (the built-in tape of train_forward is not among them)."""
+        return [t for t in list(self._tapes) if t.handle.value]
 
     def set_output_peers(self, mode: int, deltas=()):
         """Fused loss-boundary gather (gw_plan_set_output_peers): mode 0 off, 1 multicast alias, 2 peer mappings."""
@@ -351,3 +372,51 @@ class Plan:
         d = self.device
         with torch.cuda.device(d):
             _check(self.lib.gw_latent_edge_features(self.handle, _ptr(out, torch.float32, d), _stream(d)))
+
+
+class Tape:
+    """One gw_tape of a plan: what one training forward saves for its own backward.  It keeps its plan object referenced and is
+    destroyed (its memory released on the current stream) by `close()` or when it is garbage-collected.  Once its plan is
+    closed the tape is dead: its memory went with the plan, and a forward or backward on it raises."""
+
+    def __init__(self, plan: Plan):
+        self.plan = plan
+        self.lib = plan.lib
+        self.handle = _vp()
+        _check(self.lib.gw_tape_create(plan.handle, ctypes.byref(self.handle)))
+
+    def _plan_handle(self):
+        if not self.plan.handle.value:
+            raise RuntimeError("libgwb200: this tape is dead: its plan was closed, and its activations with it")
+        return self.plan.handle
+
+    def forward(self, features, out):
+        """gw_train_forward_tape: Plan.train_forward on this tape."""
+        d = self.plan.device
+        with torch.cuda.device(d):
+            _check(self.lib.gw_train_forward_tape(self._plan_handle(), self.handle, _ptr(features, torch.float32, d), _ptr(out, torch.float32, d),
+                                                  int(features.shape[0]), _stream(d)))  # fmt: skip
+
+    def backward(self, grad_out, grad_features, named_grads):
+        """gw_train_backward_tape: Plan.train_backward of this tape's forward; consumes the tape."""
+        d = self.plan.device
+        arr, n = self.plan._grad_table(named_grads)
+        with torch.cuda.device(d):
+            gf = _ptr(grad_features, torch.float32, d) if grad_features is not None else _vp()
+            _check(self.lib.gw_train_backward_tape(self._plan_handle(), self.handle, _ptr(grad_out, torch.float32, d), gf, arr, n, _stream(d)))
+
+    def bytes(self) -> int:
+        """gw_tape_bytes: what the tape holds now (between its forward and backward, the forward's saved tensors)."""
+        return int(self.lib.gw_tape_bytes(self.handle)) if self.handle.value else 0
+
+    def close(self):
+        if getattr(self, "handle", None) is not None and self.handle.value:
+            with torch.cuda.device(self.plan.device):
+                self.lib.gw_tape_destroy(self.handle, _stream(self.plan.device))
+            self.handle = _vp()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -19,6 +19,7 @@
 #include <cmath>
 #include <cstring>
 #include <map>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -106,6 +107,7 @@ struct gw_plan {
   int device = 0;
   int n_in_cur = 0;
   unsigned enc_graph_gen = 0;  // bumped whenever the encoder graph is replaced (the training step's chunk tables are built per graph)
+  unsigned wgen = 0;           // bumped by every gw_plan_set_weights (the training step's per-weight work and its tapes key on it)
   // graphs
   DevBuf<int32_t> enc_mesh, enc_perm, enc_ptr, lat_src, lat_dst, lat_ptr, dec_src, dec_ptr;
   DevBuf<float> enc_attr, lat_attr, dec_attr;
@@ -225,13 +227,15 @@ static int raw_bound(gw_plan* p, int slot, const float* x, long long n, cudaStre
   return 0;
 }
 
-// (the training step's phases, gw_train.inl: taped forward products, data gradients, weight gradients, per-step weight images and
-// operand bounds, and the memory-bound rest -- LayerNorm backward, segment sums, gathers, batch reductions)
+// (the training step's phases, gw_train.inl: taped forward products, data gradients, weight gradients, operand bounds, the
+// memory-bound rest -- LayerNorm backward, segment sums, gathers, batch reductions -- and the per-weight work done once per weight
+// upload: transposes and weight images)
 enum KernelTag { TAG_CONST = 0, TAG_ENC_GRID, TAG_ENC_MESH, TAG_PROC_P, TAG_PROC_EDGE, TAG_PROC_NODE, TAG_DEC_P, TAG_DEC_EDGE,
-                 TAG_DEC_NODE, TAG_TRAIN_FWD, TAG_TRAIN_DGRAD, TAG_TRAIN_WGRAD, TAG_TRAIN_PACK, TAG_TRAIN_OTHER, TAG_COUNT };
+                 TAG_DEC_NODE, TAG_TRAIN_FWD, TAG_TRAIN_DGRAD, TAG_TRAIN_WGRAD, TAG_TRAIN_PACK, TAG_TRAIN_OTHER, TAG_TRAIN_WEIGHTS,
+                 TAG_COUNT };
 static const char* kTagNames[TAG_COUNT] = {"const", "enc_grid", "enc_mesh", "proc_p", "proc_edge", "proc_node", "dec_p",
                                            "dec_edge", "dec_node", "train_fwd", "train_dgrad", "train_wgrad", "train_pack",
-                                           "train_other"};
+                                           "train_other", "train_weights"};
 
 static cudaEvent_t take_event(gw_plan* p) {
   if (p->ev_used == p->ev_pool.size()) {
@@ -1243,7 +1247,11 @@ int gw_plan_destroy(gw_plan* p) {
   p->h3_frames.release(), p->h3_lat.release(), p->h3_lng.release(), p->h3_cell_of.release(), p->h3_slot.release(), p->obs_ws.release();
   p->enc_chunk_seg.release(), p->enc_chunk_j0.release(), p->enc_seg_chunk0.release(), p->enc_partial.release();
   if (p->train) {
-    gw::tfree_all(p->train);
+    for (gw_tape* k : p->train->tapes) {  // every live tape's memory goes with the plan; the tapes stay as dead handles
+      gw::tape_release(p->train, k, p->train->st);
+      k->plan = nullptr;
+    }
+    p->train->tapes.clear();
     p->train->wT.release(), p->train->gbuf.release(), p->train->lat_perm_src.release(), p->train->lat_ptr_src.release();
     p->train->dec_perm_src.release(), p->train->dec_ptr_src.release(), p->train->iota.release(), p->train->sort_ws.release();
     p->train->enc_slot_sorted.release(), p->train->dec_cperm.release(), p->train->dec_cptr.release();
@@ -1372,6 +1380,7 @@ int gw_plan_set_weights(gw_plan* p, const gw_param* params, int32_t n, void* str
     GW_CHECK(params[i].name && params[i].data && params[i].rows > 0 && params[i].cols > 0, "malformed gw_param entry");
     total += ((size_t)params[i].rows * params[i].cols + 63) / 64 * 64;  // 256-byte aligned slices
   }
+  ++p->wgen;  // (even a failed upload has replaced what a tape's backward would differentiate)
   if (p->wbuf.n != total) GW_TRY(p->wbuf.alloc(total));
   p->params.clear();
   size_t off = 0;
@@ -1444,19 +1453,69 @@ int gw_forward_strided(gw_plan* p, const float* features, float* out, int32_t ou
   return gw::stage_decoder(p, p->xbuf0.p, gw::SL_X0, p->d.residual_dim > 0 ? features : nullptr, p->d.in_dim, out, out_ld, batch, st);
 }
 
-int gw_train_forward(gw_plan* p, const float* features, float* out, int32_t batch, void* stream) {
-  GW_TRY(gw::check_ready(p, batch, gw::NEED_ENC | gw::NEED_PROC | gw::NEED_DEC));
-  GW_CHECK(features && out, "null argument");
-  if (!p->train) p->train = new gw::TrainState();
-  return gw::train_forward(p, p->train, features, out, batch, (cudaStream_t)stream);
+// the plan's training state, made on first use with its built-in tape registered
+static gw::TrainState* train_state(gw_plan* p) {
+  if (!p->train) {
+    p->train = new gw::TrainState();
+    p->train->own.plan = p;
+    p->train->tapes.insert(&p->train->own);
+  }
+  return p->train;
 }
 
-int gw_train_backward(gw_plan* p, const float* grad_out, float* grad_features, const gw_param* grads, int32_t n, void* stream) {
-  GW_CHECK(p && grad_out && (n == 0 || grads), "null argument");
-  GW_CHECK(p->train != nullptr, "gw_train_backward needs a preceding gw_train_forward");
+int gw_tape_create(gw_plan* p, gw_tape** out) {
+  GW_CHECK(p && out, "null argument");
+  gw::TrainState* T = train_state(p);
+  gw_tape* k = new gw_tape();
+  k->plan = p;
+  T->tapes.insert(k);
+  *out = k;
+  return 0;
+}
+
+int gw_tape_destroy(gw_tape* k, void* stream) {
+  if (!k) return 0;
+  if (gw_plan* p = k->plan) {
+    GW_CHECK(k != &p->train->own, "gw_tape_destroy: the plan's built-in tape goes with the plan");
+    GW_CUDA(cudaSetDevice(p->device));
+    gw::tape_release(p->train, k, (cudaStream_t)stream);
+    p->train->tapes.erase(k);
+  }
+  delete k;
+  return 0;
+}
+
+int64_t gw_tape_bytes(const gw_tape* k) { return k ? (int64_t)k->bytes : 0; }
+
+// a tape of plan p that is still alive (its plan not destroyed)
+static int check_tape(gw_plan* p, gw_tape* k) {
+  GW_CHECK(k != nullptr, "null tape");
+  GW_CHECK(k->plan != nullptr, "this tape is dead: its plan was destroyed, and its activations with it");
+  GW_CHECK(k->plan == p, "this tape belongs to another plan");
+  return 0;
+}
+
+int gw_train_forward_tape(gw_plan* p, gw_tape* k, const float* features, float* out, int32_t batch, void* stream) {
+  GW_TRY(check_tape(p, k));
+  GW_TRY(gw::check_ready(p, batch, gw::NEED_ENC | gw::NEED_PROC | gw::NEED_DEC));
+  GW_CHECK(features && out, "null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rc = gw::train_forward(p, p->train, k, features, out, batch, st);
+  if (rc) gw::tape_release(p->train, k, st);  // a refused forward leaves no tape
+  return rc;
+}
+
+int gw_train_forward(gw_plan* p, const float* features, float* out, int32_t batch, void* stream) {
+  GW_CHECK(p != nullptr, "null plan");
+  return gw_train_forward_tape(p, &train_state(p)->own, features, out, batch, stream);
+}
+
+int gw_train_backward_tape(gw_plan* p, gw_tape* k, const float* grad_out, float* grad_features, const gw_param* grads, int32_t n, void* stream) {
+  GW_TRY(check_tape(p, k));
+  GW_CHECK(grad_out && (n == 0 || grads), "null argument");
   GW_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
-  GW_TRY(gw::train_backward(p, p->train, grad_out, grad_features, st));
+  GW_TRY(gw::train_backward(p, p->train, k, grad_out, grad_features, st));
   for (int i = 0; i < n; ++i) {  // gradients are handed out under the reference's parameter names, shaped like the parameters
     GW_CHECK(grads[i].name && grads[i].data, "malformed gw_param entry");
     auto it = p->params.find(grads[i].name);
@@ -1467,6 +1526,12 @@ int gw_train_backward(gw_plan* p, const float* grad_out, float* grad_features, c
                             cudaMemcpyDeviceToDevice, st));
   }
   return 0;
+}
+
+int gw_train_backward(gw_plan* p, const float* grad_out, float* grad_features, const gw_param* grads, int32_t n, void* stream) {
+  GW_CHECK(p != nullptr, "null argument");
+  GW_CHECK(p->train != nullptr, "gw_train_backward needs a preceding gw_train_forward");
+  return gw_train_backward_tape(p, &p->train->own, grad_out, grad_features, grads, n, stream);
 }
 
 int64_t gw_train_peak_bytes(const gw_plan* p) { return (p && p->train) ? (int64_t)p->train->peak_bytes : 0; }

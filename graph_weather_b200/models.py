@@ -17,6 +17,7 @@ there is no eager-PyTorch or CPU execution path -- CPU tensors raise.
 
 from __future__ import annotations
 
+import contextlib
 import os
 from dataclasses import dataclass
 from typing import Optional
@@ -240,7 +241,9 @@ def _maybe_check(plan):
 class _TrainFn(torch.autograd.Function):
     """autograd node of one training forward of a wrapper (GraphWeatherForecaster, GraphCast, GraphWeatherAssimilator): forward =
     gw_train_forward (activations kept in the plan), backward = gw_train_backward (gradients of every parameter under its reference
-    name, and of the features when they require grad).  One backward per forward: the plan holds a single tape.
+    name, and of the features when they require grad).  One backward per forward.  Outside `multi_step()` the forward runs on the
+    plan's built-in tape, which the next training forward replaces; inside it, on a tape of its own (`_capi.Tape`) that this node
+    owns: its backward consumes it, and dropping the graph without a backward frees it.
 
     The wrapper (`_Wrapper`) supplies its training engine (`_training_engine()`), its named parameters (`_named()`) and its output
     shape (`_out_shape(batch)`).  `obs` (the assimilator's lat_lon_heights, else None) is built into the training plan's observation
@@ -255,28 +258,52 @@ class _TrainFn(torch.autograd.Function):
             model.encoder._upload_obs(eng, plan, obs)
         f = features.detach().to(torch.float32).contiguous()
         out = torch.empty(model._out_shape(B), dtype=torch.float32, device=f.device)
-        plan.train_forward(f, out)
-        eng.tape_id = getattr(eng, "tape_id", 0) + 1
-        ctx.model, ctx.plan, ctx.eng, ctx.tape_id = model, plan, eng, eng.tape_id
+        ctx.tape, ctx.tape_id = None, None
+        if model.__dict__.get("_multi_step", 0):
+            tape = plan.tape()
+            try:
+                tape.forward(f, out)
+                _maybe_check(plan)
+            except BaseException:
+                tape.close()  # a refused forward leaves no tape
+                raise
+            ctx.tape = tape
+        else:
+            plan.train_forward(f, out)
+            eng.tape_id = getattr(eng, "tape_id", 0) + 1
+            ctx.tape_id = eng.tape_id
+            _maybe_check(plan)
+        ctx.model, ctx.plan, ctx.eng = model, plan, eng
         ctx.feat_shape, ctx.feat_grad = tuple(f.shape), bool(features.requires_grad)
         ctx.names = [k for k, _ in model.named_parameters()]
         ctx.pshapes = [tuple(q.shape) for q in params]
         ctx.pgrad = [bool(q.requires_grad) for q in params]
         ctx.keep = f  # the tape reads the features again in the backward (weight gradient of the first Linear)
-        _maybe_check(plan)
+        ctx.consumed = False
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        if ctx.eng.tape_id != ctx.tape_id or ctx.eng.plan is not ctx.plan:
-            raise RuntimeError("graph_weather_b200: backward of a forward whose activations were replaced by a later training "
-                               "forward (one backward per forward: the plan keeps a single tape)")
+        if ctx.consumed or (ctx.tape_id is not None and ctx.eng.tape_id != ctx.tape_id):
+            raise RuntimeError("graph_weather_b200: backward of a forward whose activations were consumed by an earlier backward or "
+                               "replaced by a later training forward outside multi_step() (one backward per forward)")
+        if ctx.eng.plan is not ctx.plan:
+            raise RuntimeError("graph_weather_b200: backward of a forward whose plan was replaced (a switch of the training step, a "
+                               "larger batch or .to()): its activations are gone (one backward per forward)")
         dev = grad_out.device
         g = grad_out.detach().to(torch.float32).contiguous()
         gfeat = torch.empty(ctx.feat_shape, dtype=torch.float32, device=dev) if ctx.feat_grad else None
         grads = [torch.empty(s, dtype=torch.float32, device=dev) for s in ctx.pshapes]
-        ctx.plan.train_backward(g, gfeat, list(zip(ctx.names, grads)))
-        ctx.eng.tape_id += 1  # the tape is consumed
+        if ctx.tape is None:
+            ctx.plan.train_backward(g, gfeat, list(zip(ctx.names, grads)))
+            ctx.eng.tape_id += 1  # the tape is consumed
+        else:
+            try:
+                ctx.tape.backward(g, gfeat, list(zip(ctx.names, grads)))
+            finally:  # consumed, or refused (weights replaced, plan closed): either way the tape is done
+                ctx.tape.close()
+                ctx.tape, ctx.consumed = None, True
+        ctx.consumed = True
         _maybe_check(ctx.plan)
         return (None, gfeat, None) + tuple(gr if need else None for gr, need in zip(grads, ctx.pgrad))
 
@@ -635,6 +662,29 @@ class _Wrapper(nn.Module):
         _maybe_check(plan)
         return out
 
+    @contextlib.contextmanager
+    def multi_step(self):
+        """Training forwards made inside this window each keep a tape of their own, so a loss summed over an autoregressive
+        rollout back-propagates through every step with one `backward()`:
+
+            with model.multi_step():
+                y1 = model(x0)
+                y2 = model(torch.cat([y1, aux1], -1))
+            (crit(y1, t1) + crit(y2, t2)).backward()
+
+        Each forward's autograd node owns its tape: the backward consumes it, and dropping the graph without a backward frees it.
+        Tapes made inside stay valid after the window exits; exiting only changes what later forwards do (outside it, a training
+        forward replaces the previous one's activations, as it always has).  A backward raises once its tape's plan was replaced
+        (a switch between the taped and the bounded step, a larger batch, `.to()`) or the weights were re-uploaded after its
+        forward (an optimiser step followed by another forward).  The memory of the window grows with the number of live tapes
+        (tools/train_step_bench.py --rollout K reports it)."""
+        depth = self.__dict__.get("_multi_step", 0)
+        self.__dict__["_multi_step"] = depth + 1
+        try:
+            yield self
+        finally:
+            self.__dict__["_multi_step"] = depth
+
     def _train_or_infer(self, features, obs=None):
         """The training step in train mode with autograd on (`_wants_grad`), otherwise inference."""
         if _wants_grad(self, features):
@@ -882,6 +932,10 @@ class GraphWeatherAssimilator(_Wrapper, PyTorchModelHubMixin):
         self.analysis_dim = analysis_dim
         self.use_checkpointing = use_checkpointing
         self._init_engine(analysis_dim, 0, num_blocks, precision, train_precision)
+
+    def multi_step(self):
+        raise NotImplementedError("GraphWeatherAssimilator.multi_step: the observation graph a training forward runs on belongs to the "
+                                  "plan, not to the forward, so several forwards cannot stay differentiable at once")
 
     def forward(self, features: torch.Tensor, obs_lat_lon_heights: torch.Tensor) -> torch.Tensor:
         if features.device.type != "cuda":

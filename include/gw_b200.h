@@ -140,11 +140,33 @@ int gw_forward_strided(gw_plan* plan, const float* features, float* out, int32_t
  * relative, not bit for bit); GW_PREC_FP32_TC (fp16 hi/lo split, 3 MMAs per product) or GW_PREC_BF16_TC (bf16 operands) on wgmma
  * tensor cores with fp32 accumulation, fp32 tape and fp32 gradients -- 256-wide dims and 2 hidden layers, sm_90a; their weight
  * gradients of layers with more than 16 inputs are reduced in a fixed order (bit for bit repeatable).  Timing tags train_fwd,
- * train_dgrad, train_wgrad, train_pack, train_other split a step (gw_timing_read). */
+ * train_dgrad, train_wgrad, train_pack (operand bounds), train_other and train_weights split a step (gw_timing_read).  The
+ * per-weight work -- transposed weights and, on tensor cores, the weight images -- is done once per gw_plan_set_weights, by the
+ * first step after it (tag train_weights).  These two calls run on the plan's built-in tape: the next gw_train_forward replaces
+ * it, and the backward of the replaced forward is gone. */
 int gw_train_forward(gw_plan* plan, const float* features, float* out, int32_t batch, void* stream);
 int gw_train_backward(gw_plan* plan, const float* grad_out, float* grad_features, const gw_param* grads, int32_t n, void* stream);
-/* High-water mark, in bytes, of the training step's stream-ordered working allocations over the last gw_train_forward and the
- * gw_train_backward after it (0 before the first step).  It depends on the shapes only, unlike device-wide figures on a shared card. */
+/* Tapes: several training forwards alive at once (a loss summed over a multi-step rollout, back-propagated once).  A tape holds
+ * what one forward saves for its backward; gw_train_forward_tape is gw_train_forward on `tape` (a second forward on the same tape
+ * replaces the first), gw_train_backward_tape is gw_train_backward that consumes it.  Tapes of one plan share its weights, graphs
+ * and gradient buffer, and run on the plan's stream.  Batches may differ between tapes.
+ *   gw_tape_destroy releases the tape's memory stream-ordered on `stream` and frees the handle.
+ *   gw_plan_destroy releases the memory of every tape of the plan and leaves them dead: a forward or backward on a dead tape
+ *   fails (gw_tape_destroy still frees the handle).
+ *   A backward fails when gw_plan_set_weights ran after the tape's forward (its gradient would be taken at other weights).
+ *   gw_tape_bytes: the bytes the tape holds -- between its forward and backward, what the forward saved (shape-determined);
+ *   0 after the backward. */
+typedef struct gw_tape gw_tape; /* opaque */
+int gw_tape_create(gw_plan* plan, gw_tape** out_tape);
+int gw_tape_destroy(gw_tape* tape, void* stream);
+int gw_train_forward_tape(gw_plan* plan, gw_tape* tape, const float* features, float* out, int32_t batch, void* stream);
+int gw_train_backward_tape(gw_plan* plan, gw_tape* tape, const float* grad_out, float* grad_features, const gw_param* grads,
+                           int32_t n, void* stream);
+int64_t gw_tape_bytes(const gw_tape* tape);
+/* High-water mark, in bytes, of the training step's stream-ordered working allocations -- every live tape plus the running step's
+ * temporaries -- since a training forward last began while no other tape held memory (0 before the first step).  For one tape at
+ * a time: over the last gw_train_forward and the gw_train_backward after it.  It depends on the shapes only, unlike device-wide
+ * figures on a shared card. */
 int64_t gw_train_peak_bytes(const gw_plan* plan);
 
 /* Multi-GPU loss boundary fused into the forecast's last chain (SURVEY.md 8(e): the one gather of the outputs).  After this call

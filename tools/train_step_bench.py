@@ -3,7 +3,7 @@ GraphWeatherAssimilator.
     python tools/train_step_bench.py [--model forecaster|graphcast|assimilator] [--grid 0.25deg|1deg|2deg|5deg|10deg] [--batch B]
                                      [--steps K] [--train-precision fp32_simt|fp32|bf16] [--feature-dim F] [--aux-dim A]
                                      [--num-blocks NB] [--width W] [--constraint-type none|additive|multiplicative|softmax]
-                                     [--use-checkpointing] [--fit-batch] [--n-obs N]
+                                     [--use-checkpointing] [--fit-batch] [--n-obs N] [--rollout K [--compare-plain]]
 The model defaults to the README's 78 + 24 features, 9 blocks, 256-wide.  --model graphcast: GraphCast(input_dim = output_dim =
 --feature-dim, hidden_dim = --width or 256); its bounded step is selected by --use-checkpointing (the same step
 GraphCastConfig.balanced_checkpointing / full_checkpointing select).  --model assimilator: GraphWeatherAssimilator(output_lat_lons =
@@ -20,6 +20,11 @@ grid bench.py uses).  Every run reports train_peak_bytes (the step's working all
 device_bytes.  --fit-batch: the largest batch whose step should fit on the card, from the device bytes the step needs at
 batches 1 and 2 (train_peak_bytes + plan bytes + torch's reserved peak, each linear in the batch), confirmed by one run at that
 batch in a fresh process.
+--rollout K: one step is a K-step autoregressive rollout trained as one -- K forwards inside model.multi_step(), each fed the
+previous forecast (the forecaster's auxiliary columns stay those of the first input), the summed loss, one backward chain and the
+SGD update; "rollout" reports gw_tape_bytes of each of the K tapes (what each forward keeps until the backward), and
+train_peak_bytes covers all of them.  --compare-plain (with --rollout 1) also times the window's one-step step and the plain step
+alternately, step by step, and reports both medians.
 With --constraint-type the step includes PhysicalConstraintLayer; the constraint backward
 (gw_constraint_backward, no timing tag of the plan) is also timed on its own with CUDA events around it, on the step's shapes."""
 import argparse
@@ -87,9 +92,15 @@ def main():
     ap.add_argument("--use-checkpointing", action="store_true", help="the bounded-memory training step (training-only plan)")
     ap.add_argument("--fit-batch", action="store_true", help="report the largest batch that should fit, confirmed by one run")
     ap.add_argument("--n-obs", type=int, default=2660, help="observations per step (--model assimilator)")
+    ap.add_argument("--rollout", type=int, default=0, help="K: one step is K forwards inside model.multi_step() and one backward")
+    ap.add_argument("--compare-plain", action="store_true", help="with --rollout 1: alternate the window's step with the plain one")
     a = ap.parse_args()
     if a.model != "forecaster" and a.constraint_type != "none":
         ap.error("--constraint-type applies to --model forecaster")
+    if a.rollout and a.model == "assimilator":
+        ap.error("--rollout: GraphWeatherAssimilator has no multi_step()")
+    if a.compare_plain and a.rollout != 1:
+        ap.error("--compare-plain compares the window's K = 1 step with the plain step: use --rollout 1")
     import __graft_entry__ as ge
 
     ge.build()
@@ -126,6 +137,7 @@ def main():
         n_in, f_in = len(ll), F + a.aux_dim
     crit = NormalizedMSELoss([1.0] * F, ll, normalize=True)
     opt = torch.optim.SGD(model.parameters(), lr=1e-3)
+    tape_bytes = []  # gw_tape_bytes of every tape of the last --rollout step, read before its backward
 
     def measure(batch, steps):
         """(ms/step, losses, torch peak bytes, train_peak_bytes, plan device_bytes, step function, inputs) of `steps` timed steps."""
@@ -137,12 +149,22 @@ def main():
             u = torch.rand(n_in, 3, device="cuda", generator=g)
             return torch.stack([u[:, 0] * 180.0 - 90.0, u[:, 1] * 360.0, u[:, 2]], 1)
 
-        def one():
+        def one(rollout=a.rollout):
             opt.zero_grad(set_to_none=True)
-            loss = crit(model(x, obs()) if a.model == "assimilator" else model(x), y)
+            if rollout:  # K forwards in one multi_step() window, each fed the previous forecast (+ the fixed aux columns)
+                with model.multi_step():
+                    inp, loss = x, 0.0
+                    for t in range(rollout):
+                        out = model(inp)
+                        loss = loss + crit(out, y)
+                        if t + 1 < rollout:
+                            inp = torch.cat([out, x[..., F:]], -1) if f_in > F else out
+                tape_bytes[:] = [t.bytes() for t in model._train_engine.plan.live_tapes()]
+            else:
+                loss = crit(model(x, obs()) if a.model == "assimilator" else model(x), y)
             loss.backward()
             opt.step()
-            return loss
+            return loss.detach()
 
         for _ in range(2):
             one()
@@ -177,6 +199,20 @@ def main():
         return
     ms, losses, peak, train_peak, plan_bytes, one, x = measure(a.batch, a.steps)
     free, total = torch.cuda.mem_get_info()
+    rollout = None
+    if a.rollout:
+        rollout = {"K": a.rollout, "tape_bytes": list(tape_bytes), "tape_gib": [round(v / 2**30, 3) for v in tape_bytes]}
+    if a.compare_plain:  # the window's K = 1 step and the plain step, alternated step by step (CUDA events around each)
+        times = {"window": [], "plain": []}
+        for i in range(2 * a.steps):
+            kind = "window" if i % 2 == 0 else "plain"
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            one(rollout=1 if kind == "window" else 0)
+            e1.record()
+            torch.cuda.synchronize()
+            times[kind].append(e0.elapsed_time(e1))
+        rollout["compare_plain_median_ms"] = {k: round(sorted(v)[len(v) // 2], 3) for k, v in times.items()}
     # per-phase device time of one more step (the plan's stream-ordered tape allocations are outside torch's allocator: the
     # device-wide figure is reported too)
     plan = model._train_engine.plan
@@ -188,7 +224,7 @@ def main():
     plan.status()
     cbwd = constraint_backward_time(model, x, F) if a.constraint_type != "none" else None
     print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "model": a.model, "train_precision": a.train_precision, "grid": a.grid, "batch": a.batch,
-                      "use_checkpointing": a.use_checkpointing, "train_peak_gib": round(train_peak / 2**30, 3),
+                      "use_checkpointing": a.use_checkpointing, "rollout": rollout, "train_peak_gib": round(train_peak / 2**30, 3),
                       "plan_device_gib": round(plan_bytes / 2**30, 3),
                       "dims": dims, "constraint_type": a.constraint_type, "constraint_backward": cbwd,
                       "n_params": sum(q.numel() for q in model.parameters()),
