@@ -74,8 +74,6 @@ _SIGNATURES = {
     "gw_constraint_backward_workspace_bytes": (_i64, [_i64, _i64, _i32]),
     "gw_constraint_backward": (ctypes.c_int, [_i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i64, _i64, _i32, ctypes.c_float, _vp, _vp]),
     "gw_normalized_mse_loss_grad": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i32, _vp, ctypes.c_float, _vp, _vp]),
-    "gw_train_forward": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp]),
-    "gw_train_backward": (ctypes.c_int, [_vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
     "gw_train_peak_bytes": (_i64, [_vp]),
     "gw_tape_create": (ctypes.c_int, [_vp, ctypes.POINTER(_vp)]),
     "gw_tape_destroy": (ctypes.c_int, [_vp, _vp]),
@@ -115,7 +113,7 @@ def load():
     for name, (res, args) in _SIGNATURES.items():
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = res, args
-    if lib.gw_abi_version() != 1:
+    if lib.gw_abi_version() != 2:
         raise RuntimeError("libgwb200.so ABI version mismatch")
     _lib = lib
     return lib
@@ -288,13 +286,6 @@ class Plan:
             _check(self.lib.gw_decoder_forward(self.handle, _ptr(x_in, torch.float32, d), sp, ld, _ptr(out, torch.float32, d),
                                                int(batch), _stream(d)))  # fmt: skip
 
-    def train_forward(self, features, out):
-        """Forward on the exact-fp32 plan that keeps the activations for `train_backward` (one backward per forward)."""
-        d = self.device
-        with torch.cuda.device(d):
-            _check(self.lib.gw_train_forward(self.handle, _ptr(features, torch.float32, d), _ptr(out, torch.float32, d), int(features.shape[0]),
-                                             _stream(d)))  # fmt: skip
-
     def _grad_table(self, named_grads):
         items = list(named_grads)
         arr = (GwParam * max(1, len(items)))()
@@ -303,15 +294,6 @@ class Plan:
             arr[i] = GwParam(k.encode(), _ptr(v, torch.float32, self.device).value, rows, cols)
         return arr, len(items)
 
-    def train_backward(self, grad_out, grad_features, named_grads):
-        """grad_out [B, N, out] -> gradients written into `named_grads` (reference parameter name -> tensor shaped like the
-        parameter) and, if given, the gradient of the features."""
-        d = self.device
-        arr, n = self._grad_table(named_grads)
-        with torch.cuda.device(d):
-            gf = _ptr(grad_features, torch.float32, d) if grad_features is not None else _vp()
-            _check(self.lib.gw_train_backward(self.handle, _ptr(grad_out, torch.float32, d), gf, arr, n, _stream(d)))
-
     def tape(self) -> "Tape":
         """A new tape of this plan (gw_tape_create): one more training forward that stays differentiable alongside the others."""
         t = Tape(self)
@@ -319,7 +301,7 @@ class Plan:
         return t
 
     def live_tapes(self):
-        """The tapes made by `tape()` that are not destroyed yet (the built-in tape of train_forward is not among them)."""
+        """The tapes made by `tape()` that are not destroyed yet."""
         return [t for t in list(self._tapes) if t.handle.value]
 
     def set_output_peers(self, mode: int, deltas=()):
@@ -391,14 +373,15 @@ class Tape:
         return self.plan.handle
 
     def forward(self, features, out):
-        """gw_train_forward_tape: Plan.train_forward on this tape."""
+        """gw_train_forward_tape: the forward that keeps its activations on this tape (a second forward replaces the first's)."""
         d = self.plan.device
         with torch.cuda.device(d):
             _check(self.lib.gw_train_forward_tape(self._plan_handle(), self.handle, _ptr(features, torch.float32, d), _ptr(out, torch.float32, d),
                                                   int(features.shape[0]), _stream(d)))  # fmt: skip
 
     def backward(self, grad_out, grad_features, named_grads):
-        """gw_train_backward_tape: Plan.train_backward of this tape's forward; consumes the tape."""
+        """gw_train_backward_tape: grad_out [B, N, out] -> gradients written into `named_grads` (reference parameter name -> tensor
+        shaped like the parameter) and, if given, the gradient of the features.  One backward per forward: it consumes the tape."""
         d = self.plan.device
         arr, n = self.plan._grad_table(named_grads)
         with torch.cuda.device(d):

@@ -60,7 +60,7 @@ bool tc3_chain_is_lean(const TcChain& ch);  // would the launch take the lean (p
 // A layer with a LayerNorm cannot be split: cudaErrorInvalidValue.
 constexpr int TC_COL_BLOCK = 256;
 cudaError_t tc_column_block(const TcChain& ch, int n0, int nb, TcChain* out);
-// The one-layer chain of a training row op (gw_train.inl, train_op): stage 0 = op.a with K0 = K rounded to 64, layer 0 = the op's
+// The one-layer chain of a training row op (gw_train.cu, train_op): stage 0 = op.a with K0 = K rounded to 64, layer 0 = the op's
 // bias, addends, ReLU, LayerNorm, residual, output, pre-LayerNorm store and mask over all N columns -- the `ch` tc_column_block
 // cuts into the blocks that run.  It sets no operand bounds, weight image, split or status.  cudaErrorInvalidValue for an op no
 // chain runs: an add[2] addend, no a[0], or a LayerNorm wider than TC_COL_BLOCK.
@@ -81,7 +81,7 @@ cudaError_t launch_absmax(const float* W, int ldw, int K_src, int N_src, float* 
 // The training step's image of W, scale taken on the device: *wamax = max|W| (reset first), then the pack.  A chain layer given
 // this image takes wamax as its TcLayer::wamax.
 cudaError_t launch_pack_image(const float* W, int ldw, int K_src, int N_src, int parts, void* img, float* wamax, cudaStream_t stream);
-// A weight image packed with a scale the host chose from max|W| (the inference plans' images, gw_api.cu): what its chain layer
+// A weight image packed with a scale the host chose from max|W| (the inference plans' images, gw_forward.cu): what its chain layer
 // needs to know of it.  Pack it with wscale = 1 / winv (a power of two: exact).
 struct TcWeights {
   const void* p = nullptr;

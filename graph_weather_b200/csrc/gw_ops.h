@@ -17,7 +17,7 @@ enum SrcKind : int32_t {
   SRC_BCAST = 2,       // base[i*ld + col0 + k]                                  same rows for every sample
   SRC_GATHER = 3,      // base[(b*src_rows + idx[i])*ld + col0 + k]              per-sample table, shared index
   SRC_SEGSUM = 4,      // sum_{j in [ptr[i],ptr[i+1])} base[(b*src_rows + eid(j))*ld + col0 + k], eid = perm ? perm[j] : j
-  SRC_GATHER_BCAST_RELU = 5,  // relu(GATHER(base, idx) + base2[i*ld2 + k])     decoder edge layer-1, see gw_api.cu
+  SRC_GATHER_BCAST_RELU = 5,  // relu(GATHER(base, idx) + base2[i*ld2 + k])     decoder edge layer-1, see gw_forward.cu
   SRC_BGATHER = 6,     // base[idx[i]*ld + col0 + k]                             batch-invariant table, gathered
 };
 
@@ -95,9 +95,9 @@ struct TcLayer {
   float seg_maxdeg = 0.f;            // longest segment (bound of the sums)
   float* seg_bound = nullptr;        // device float set to the bound of the segment sums
   const float* seg_add = nullptr;    // [seg_rows, seg_ld] or null: a per-target constant added to every complete sum (the sum of a
-                                     // constant residual over the target's rows, hoisted out of the row loop: gw_api.cu S_dec)
+                                     // constant residual over the target's rows, hoisted out of the row loop: gw_forward.cu S_dec)
   const float* seg_add_bound = nullptr;  // device float: magnitude bound of seg_add
-  // training step (gw_train.inl), general path only: the value entering LayerNorm is also stored to save_pre (same ldo / out_cols
+  // training step (gw_train.cu), general path only: the value entering LayerNorm is also stored to save_pre (same ldo / out_cols
   // as out; GemmOp::save_pre), and the result is zeroed wherever mask(row, n) <= 0 (the ReLU's backward, applied last; GemmOp::mask)
   float* save_pre = nullptr;
   RowSrc mask;

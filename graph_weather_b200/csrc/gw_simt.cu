@@ -315,7 +315,7 @@ cudaError_t launch_segsum_chunked(const float* base, int ld, const int32_t* ptr,
   return cudaGetLastError();
 }
 
-// ---- backward primitives (exact fp32; gw_train.inl) -------------------------------------------------------------------------
+// ---- backward primitives (exact fp32; gw_train.cu) --------------------------------------------------------------------------
 // dW[n, k] += sum_r dY[r, n] * A[r, k]   (and db[n] += sum_r dY[r, n]) over R = rows_per_sample * batch rows, A assembled from a row
 // source like the forward kernel does (N > 256: one launch per block of 256 outputs).  Tile: all N <= 256 output rows x 32
 // k-columns per CTA column (blockIdx.y), the rows are

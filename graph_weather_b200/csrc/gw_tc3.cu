@@ -1072,7 +1072,7 @@ static void tc3_mark_lean(TcChain& ch) {
     if (ok && listed) ch.fast |= 1 << l;
   }
 }
-// Would launch_chain_tc3 run this chain on the lean path?  (gw_api.cu asks before it decides whether the forecast's 78-column output
+// Would launch_chain_tc3 run this chain on the lean path?  (gw_forward.cu asks before it decides whether the forecast's 78-column output
 // layer rides in the node chain or runs as a general-path chain of its own.)
 bool tc3_chain_is_lean(const TcChain& ch_in) {
   TcChain ch = ch_in;

@@ -1,5 +1,5 @@
 // gw_wgrad_tc.cu -- weight gradient of a Linear layer on Hopper tensor cores (wgmma), for the training step of the tensor-core
-// precisions (gw_train.inl):
+// precisions (gw_train.cu):
 //     dW[o, k] += sum_r dY[r, o] . A(r, k)        db[o] += sum_r dY[r, o]
 // over R = batch x rows_per_sample rows (up to ~3.6 M: the decoder's edges at 1 degree, batch 8).  The reduction runs over the
 // rows, so each CTA takes a contiguous range of them and forms a partial dW block; a second kernel sums the partials in a fixed

@@ -136,7 +136,7 @@ TRAIN_PRECISIONS = ("fp32_simt", "fp32", "bf16")
 
 
 def _validate_train_precision(train_precision: str, dims: dict):
-    """`train_precision` of GraphWeatherForecaster, GraphCast and GraphWeatherAssimilator: the arithmetic of the training step (gw_train.inl).  'fp32_simt' exact fp32 on
+    """`train_precision` of GraphWeatherForecaster, GraphCast and GraphWeatherAssimilator: the arithmetic of the training step (gw_train.cu).  'fp32_simt' exact fp32 on
     CUDA cores; 'fp32' fp16 hi/lo split on tensor cores (3 MMAs per product, fp32 accumulation); 'bf16' bf16 tensor-core
     operands (fp32 accumulation, fp32 master weights, gradients and tape)."""
     if train_precision not in TRAIN_PRECISIONS:
@@ -172,6 +172,7 @@ class _Engine:
         self.graph_uploaders = []  # callables(plan)
         self.generation = 0  # bumped whenever a new plan is created: per-plan upload caches key on it, never on pointers
         self.obs_key = None  # the host-built observation graph the plan holds (AssimilatorEncoder._upload_obs)
+        self.last_tape = None  # tape of the last training forward made outside multi_step(): the next one closes it (_TrainFn)
         self._wfp = None
 
     def _create(self, device, max_batch):
@@ -240,10 +241,11 @@ def _maybe_check(plan):
 
 class _TrainFn(torch.autograd.Function):
     """autograd node of one training forward of a wrapper (GraphWeatherForecaster, GraphCast, GraphWeatherAssimilator): forward =
-    gw_train_forward (activations kept in the plan), backward = gw_train_backward (gradients of every parameter under its reference
-    name, and of the features when they require grad).  One backward per forward.  Outside `multi_step()` the forward runs on the
-    plan's built-in tape, which the next training forward replaces; inside it, on a tape of its own (`_capi.Tape`) that this node
-    owns: its backward consumes it, and dropping the graph without a backward frees it.
+    gw_train_forward_tape (activations kept on a tape, `_capi.Tape`), backward = gw_train_backward_tape (gradients of every
+    parameter under its reference name, and of the features when they require grad).  One backward per forward.  Every forward
+    makes a tape that this node owns: its backward consumes it, and dropping the graph without a backward frees it.  Outside
+    `multi_step()` a forward first closes the tape of the previous forward made outside a window (`_Engine.last_tape`), which
+    replaces that forward's activations; inside it, a forward closes nothing.
 
     The wrapper (`_Wrapper`) supplies its training engine (`_training_engine()`), its named parameters (`_named()`) and its output
     shape (`_out_shape(batch)`).  `obs` (the assimilator's lat_lon_heights, else None) is built into the training plan's observation
@@ -258,33 +260,31 @@ class _TrainFn(torch.autograd.Function):
             model.encoder._upload_obs(eng, plan, obs)
         f = features.detach().to(torch.float32).contiguous()
         out = torch.empty(model._out_shape(B), dtype=torch.float32, device=f.device)
-        ctx.tape, ctx.tape_id = None, None
-        if model.__dict__.get("_multi_step", 0):
-            tape = plan.tape()
-            try:
-                tape.forward(f, out)
-                _maybe_check(plan)
-            except BaseException:
-                tape.close()  # a refused forward leaves no tape
-                raise
-            ctx.tape = tape
-        else:
-            plan.train_forward(f, out)
-            eng.tape_id = getattr(eng, "tape_id", 0) + 1
-            ctx.tape_id = eng.tape_id
+        in_window = bool(model.__dict__.get("_multi_step", 0))
+        if not in_window and eng.last_tape is not None:
+            eng.last_tape.close()  # stream-ordered, ahead of this forward's allocations
+            eng.last_tape = None
+        tape = plan.tape()
+        try:
+            tape.forward(f, out)
             _maybe_check(plan)
+        except BaseException:
+            tape.close()  # a refused forward leaves no tape
+            raise
+        if not in_window:
+            eng.last_tape = tape
+        ctx.tape = tape
         ctx.model, ctx.plan, ctx.eng = model, plan, eng
         ctx.feat_shape, ctx.feat_grad = tuple(f.shape), bool(features.requires_grad)
         ctx.names = [k for k, _ in model.named_parameters()]
         ctx.pshapes = [tuple(q.shape) for q in params]
         ctx.pgrad = [bool(q.requires_grad) for q in params]
         ctx.keep = f  # the tape reads the features again in the backward (weight gradient of the first Linear)
-        ctx.consumed = False
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        if ctx.consumed or (ctx.tape_id is not None and ctx.eng.tape_id != ctx.tape_id):
+        if ctx.tape is None or not ctx.tape.handle.value:
             raise RuntimeError("graph_weather_b200: backward of a forward whose activations were consumed by an earlier backward or "
                                "replaced by a later training forward outside multi_step() (one backward per forward)")
         if ctx.eng.plan is not ctx.plan:
@@ -294,16 +294,11 @@ class _TrainFn(torch.autograd.Function):
         g = grad_out.detach().to(torch.float32).contiguous()
         gfeat = torch.empty(ctx.feat_shape, dtype=torch.float32, device=dev) if ctx.feat_grad else None
         grads = [torch.empty(s, dtype=torch.float32, device=dev) for s in ctx.pshapes]
-        if ctx.tape is None:
-            ctx.plan.train_backward(g, gfeat, list(zip(ctx.names, grads)))
-            ctx.eng.tape_id += 1  # the tape is consumed
-        else:
-            try:
-                ctx.tape.backward(g, gfeat, list(zip(ctx.names, grads)))
-            finally:  # consumed, or refused (weights replaced, plan closed): either way the tape is done
-                ctx.tape.close()
-                ctx.tape, ctx.consumed = None, True
-        ctx.consumed = True
+        try:
+            ctx.tape.backward(g, gfeat, list(zip(ctx.names, grads)))
+        finally:  # consumed, or refused (weights replaced, plan closed): either way the tape is done
+            ctx.tape.close()
+            ctx.tape = None
         _maybe_check(ctx.plan)
         return (None, gfeat, None) + tuple(gr if need else None for gr, need in zip(grads, ctx.pgrad))
 

@@ -216,7 +216,7 @@ class RegionalForecaster(nn.Module):
         if features.shape[-1] < self.output_dim:
             raise RuntimeError(f"features needs at least output_dim ({self.output_dim}) channels for the residual add (:288)")
         if _wants_grad(self, features):
-            # (the forecaster's backward, csrc/gw_train.inl, is not wired to this module: fail instead of returning a tensor
+            # (the forecaster's backward, csrc/gw_train.cu, is not wired to this module: fail instead of returning a tensor
             # that silently carries no graph)
             raise NotImplementedError("RegionalForecaster: the training step is not built; call under torch.no_grad() or in eval() mode")
         region, eng = self._region(lat_lons)

@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define GW_ABI_VERSION 1
+#define GW_ABI_VERSION 2
 
 /* arithmetic mode of the MLP contractions */
 #define GW_PREC_FP32_SIMT 0 /* fp32 FFMA on CUDA cores (exact fp32; any hidden size)                              */
@@ -72,7 +72,7 @@ int gw_plan_destroy(gw_plan* plan);
 /* A plan for training only (GraphWeatherForecaster(use_checkpointing=True)): graphs, weights and the training state, none of
  * the inference scratch, packed inference weights or weight constants.  gw_plan_set_weights on it binds the weights only;
  * gw_forward, gw_forward_strided, the stage entry points and gw_latent_edge_features on it fail.  Its training step is the
- * bounded-memory one: gw_train_forward keeps only the mesh-sized activations and the output, and gw_train_backward recomputes
+ * bounded-memory one: gw_train_forward_tape keeps only the mesh-sized activations and the output, and gw_train_backward_tape recomputes
  * the grid-sized stages (the encoder's lat/lon side, the decoder) chunk by chunk with the forward's own ops, releasing each
  * chunk's temporaries before the next.  Its peak working memory grows with the grid by at most one chunk.  Chunks hold a fixed
  * working-set budget divided by the batch, chosen from the shapes alone (never from free device memory): encoder chunks are whole
@@ -131,8 +131,9 @@ int gw_forward(gw_plan* plan, const float* features, float* out, int32_t batch, 
  * no concatenation pass exists between steps. */
 int gw_forward_strided(gw_plan* plan, const float* features, float* out, int32_t out_ld, int32_t batch, void* stream);
 
-/* Training step (SURVEY.md 8(f) row 2: "then backward"; every caller of the reference trains, train/run.py:508-543).
- * gw_train_forward is gw_forward that keeps the activations the backward needs; gw_train_backward consumes them: grad_out
+/* Training step (SURVEY.md 8(f) row 2: "then backward"; every caller of the reference trains, train/run.py:508-543).  A tape holds
+ * what one training forward saves for its backward.  gw_train_forward_tape is gw_forward that keeps the activations the backward
+ * needs on `tape` (a second forward on the same tape replaces the first); gw_train_backward_tape consumes them: grad_out
  * [batch, n_out, out_dim] -> gradients of every parameter, copied into the caller's tensors named like the parameters (`grads`:
  * reference state_dict keys, device pointers, parameter shapes), and, if grad_features is not NULL, the gradient of the input
  * features [batch, n_in, in_dim].  One backward per forward.  LayerNorm MLPs, dims <= 256.  The plan's precision is the step's
@@ -142,14 +143,9 @@ int gw_forward_strided(gw_plan* plan, const float* features, float* out, int32_t
  * gradients of layers with more than 16 inputs are reduced in a fixed order (bit for bit repeatable).  Timing tags train_fwd,
  * train_dgrad, train_wgrad, train_pack (operand bounds), train_other and train_weights split a step (gw_timing_read).  The
  * per-weight work -- transposed weights and, on tensor cores, the weight images -- is done once per gw_plan_set_weights, by the
- * first step after it (tag train_weights).  These two calls run on the plan's built-in tape: the next gw_train_forward replaces
- * it, and the backward of the replaced forward is gone. */
-int gw_train_forward(gw_plan* plan, const float* features, float* out, int32_t batch, void* stream);
-int gw_train_backward(gw_plan* plan, const float* grad_out, float* grad_features, const gw_param* grads, int32_t n, void* stream);
-/* Tapes: several training forwards alive at once (a loss summed over a multi-step rollout, back-propagated once).  A tape holds
- * what one forward saves for its backward; gw_train_forward_tape is gw_train_forward on `tape` (a second forward on the same tape
- * replaces the first), gw_train_backward_tape is gw_train_backward that consumes it.  Tapes of one plan share its weights, graphs
- * and gradient buffer, and run on the plan's stream.  Batches may differ between tapes.
+ * first step after it (tag train_weights).
+ * Several tapes keep several forwards alive at once (a loss summed over a multi-step rollout, back-propagated once).  Tapes of one
+ * plan share its weights, graphs and gradient buffer, and run on the plan's stream.  Batches may differ between tapes.
  *   gw_tape_destroy releases the tape's memory stream-ordered on `stream` and frees the handle.
  *   gw_plan_destroy releases the memory of every tape of the plan and leaves them dead: a forward or backward on a dead tape
  *   fails (gw_tape_destroy still frees the handle).
@@ -165,7 +161,7 @@ int gw_train_backward_tape(gw_plan* plan, gw_tape* tape, const float* grad_out, 
 int64_t gw_tape_bytes(const gw_tape* tape);
 /* High-water mark, in bytes, of the training step's stream-ordered working allocations -- every live tape plus the running step's
  * temporaries -- since a training forward last began while no other tape held memory (0 before the first step).  For one tape at
- * a time: over the last gw_train_forward and the gw_train_backward after it.  It depends on the shapes only, unlike device-wide
+ * a time: over the last gw_train_forward_tape and the gw_train_backward_tape after it.  It depends on the shapes only, unlike device-wide
  * figures on a shared card. */
 int64_t gw_train_peak_bytes(const gw_plan* plan);
 

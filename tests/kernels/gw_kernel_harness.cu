@@ -68,7 +68,7 @@ struct HLayer {  // one forward chain layer: out = residual + LN(relu(A . W^T + 
   float* seg_bound;
 };
 
-struct HChain {  // one inference chain as gw_api.cu builds it
+struct HChain {  // one inference chain as gw_forward.cu builds it
   int32_t rows, batch, K0, n_layers;
   HSrc a0[2];
   HLayer layer[6];
@@ -138,7 +138,7 @@ int h_wgrad_simt(const float* dY, int ldy, int N, const HSrc* a, int K, int rows
 }
 
 // One training row op of any N.  precision 0: fp32_simt (gw_simt.cu); 1: fp32 (fp16 hi/lo, 3 MMAs); 2: bf16.  The tensor-core
-// precisions run it as the training step does (gw_train.inl, train_op): the chain of tc_row_op_chain, its stage-0 sources bounded
+// precisions run it as the training step does (gw_train.cu, train_op): the chain of tc_row_op_chain, its stage-0 sources bounded
 // by launch_operand_bound (fp32), cut by tc_column_block into blocks of at most TC_COL_BLOCK output columns, each with the image of
 // its rows of W from launch_pack_image.  *lean: bit j = column block j takes the lean path (-1 for fp32_simt).
 int h_row_op(int precision, const HOp* h, int* lean, int32_t* status, void* stream) {
@@ -182,7 +182,7 @@ int h_row_op(int precision, const HOp* h, int* lean, int32_t* status, void* stre
   return 0;
 }
 
-// One inference chain (precision 1: fp32, 2: bf16), prepared as gw_api.cu prepares it: every weight image described by tc_weights
+// One inference chain (precision 1: fp32, 2: bf16), prepared as gw_forward.cu prepares it: every weight image described by tc_weights
 // of its device absmax and packed with that scale, off = max|bias|, ln_bound = tc_ln_bound of the LayerNorm parameters' absmax,
 // and every source bounded by the absmax of its whole table (launch_absmax_flat).  A layer with fused per-target sums
 // gets a carry buffer (prefilled with NaN: a carry row read before it is written poisons the sum), and gw_seg_carry_kernel runs

@@ -20,7 +20,7 @@ def test_library_exports_header_symbols():
     assert len(syms) >= 20
     for s in syms:
         assert hasattr(lib, s), s
-    assert lib.gw_abi_version() == 1
+    assert lib.gw_abi_version() == 2
     assert [lib.gw_timing_tag_name(i).decode() for i in range(lib.gw_timing_num_tags())][:3] == ["const", "enc_grid", "enc_mesh"]
 
 

@@ -1,7 +1,7 @@
 """The forward's tensor-core chains (gw_chain_tc3_kernel), one at a time, against float64 references that torch computes on the GPU
 from the same fp32 inputs, layer by layer (never against another kernel).
 
-Every chain gw_api.cu builds for the forecast is rebuilt here through h_chain (tests/kernels/gw_kernel_harness.cu), prepared as
+Every chain gw_forward.cu builds for the forecast is rebuilt here through h_chain (tests/kernels/gw_kernel_harness.cu), prepared as
 inference prepares it: weight images and LayerNorm bounds through the library's tc_weights and tc_ln_bound, stage-0 bounds from
 the inputs' absmax, the carry pass after fused per-target sums.  Each runs in fp32 (fp16 hi/lo split) and bf16, on the lean path and under GW_TC3_NOFAST (the general path), and must:
   (a) exact-integer data -- integers of at most 3 significant bits (both precisions) or 16 (fp32 only, so the lo parts are not
@@ -11,7 +11,7 @@ the inputs' absmax, the carry pass after fused per-target sums.  Each runs in fp
   (b) random floats (normal, an outlier column, 1e-3 / 1e-6 / 1e5 magnitudes) stay under per-precision bars on eps_F and eps_el
       (test_gpu_kernels._eps) for every stored tensor and every per-target sum;
 and in every case: the status word stays 0, every out_bound / seg_bound the chain writes bounds its tensor, memory outside the
-stored rows x columns keeps its NaN prefill bit for bit, and the lean flag is the one gw_api.cu relies on."""
+stored rows x columns keeps its NaN prefill bit for bit, and the lean flag is the one gw_forward.cu relies on."""
 import ctypes
 import os
 
@@ -152,7 +152,7 @@ class Chain:
         return next((L for L in self.layers if L.seg is not None), None)
 
     def without_seg(self):
-        """gw_api.cu's unfused variant (general path): the layer's rows are stored instead of summed (buffer "e_rows" when the
+        """gw_forward.cu's unfused variant (general path): the layer's rows are stored instead of summed (buffer "e_rows" when the
         fused layer stores none)."""
         layers, bufs = [], dict(self.bufs)
         for L in self.layers:
@@ -179,7 +179,7 @@ class Chain:
         if seg is not None:
             dst, nt, _, _ = seg.seg
             n_rows_per_target = torch.bincount(dst.long(), minlength=nt)
-            fill = 0.0 if bool((n_rows_per_target == 0).any()) else float("nan")  # gw_api.cu memsets the sums when a target has no rows
+            fill = 0.0 if bool((n_rows_per_target == 0).any()) else float("nan")  # gw_forward.cu memsets the sums when a target has no rows
             bufs["seg"] = torch.full((self.batch * nt, seg.N), fill, device="cuda")
         for l, L in enumerate(self.layers):
             y = h.layer[l]
@@ -270,7 +270,7 @@ class Chain:
         return want, scale
 
 
-# ---- the catalogue: the chains gw_api.cu builds --------------------------------------------------------------------------------
+# ---- the catalogue: the chains gw_forward.cu builds -------------------------------------------------------------------------------
 # name -> does the launcher send it to the lean path (GW_TC3_NOFAST unset)?
 LEAN = {"enc_grid": 1, "enc_mesh": 1, "proc_p": 1, "proc_edge": 1, "proc_edge_last": 1, "proc_node": 1, "dec_p": 1, "dec_edge": 1,
         "dec_edge_res": 1, "dec_node": 1, "dec_node_misaligned": 0, "dec_node5": 1, "dec_out_odd": 0, "dec_node_n24": 0, "dec_node_n150": 0,

@@ -1,9 +1,9 @@
 """-m gpu: the exact-fp32 CUDA-core row op (gw_rowop_f32_kernel, and gw_ln_rows_kernel for LayerNorm rows wider than 256) in the
-roles csrc/gw_api.cu gives it in the forward, and the forward's small helpers, one at a time against float64.
+roles csrc/gw_forward.cu gives it in the forward, and the forward's small helpers, one at a time against float64.
 
 This row op computes the weight constants every precision reads (xm0, e_enc, C1_enc, e_lat, e_dec, E1_dec), it is the whole
 forward of every model the tensor-core chains do not fit (hidden 64, the 32-wide regional model, 1024-wide models, the per-sample
-node decoder), and it is what the tensor-core forward is compared with.  Each variant below rebuilds one GemmOp gw_api.cu issues on
+node decoder), and it is what the tensor-core forward is compared with.  Each variant below rebuilds one GemmOp gw_forward.cu issues on
 the CUDA cores, named after its call site, at the widths of the models that run it.  The helpers of tests/test_gpu_kernels.py do
 the work (Data, Src, RowOp, the harness); the checks:
   * exact-integer data bit for bit (LayerNorm layers: the pre-LN value bit for bit, the normalised output within 1e-5);
@@ -118,7 +118,7 @@ def _ln(d, n):
 
 
 def variant(name, d, w, rows=None, batch=None):
-    """The GemmOps (one, or the two P halves) of one gw_api.cu call site, on the data of generator d."""
+    """The GemmOps (one, or the two P halves) of one gw_forward.cu call site, on the data of generator d."""
     D, hd, fin, nout = w["D"], w["hd"], w["fin"], w["nout"]
     batch1 = name.startswith("pre_")  # the constants are computed once, batch 1
     rows = rows or 300

@@ -323,7 +323,7 @@ H_ROWS = 150  # rows of the per-node tables the edge shapes gather from
 
 
 def _shape(name, d, rows=300, batch=2):
-    """The row ops gw_train.inl builds, on the data of generator d."""
+    """The row ops gw_train.cu builds, on the data of generator d."""
     R = rows * batch
     if name == "hidden":  # hidden layer: K = N = 256, relu (the lean path)
         return RowOp(rows, batch, [stream(d.operand(R, 256), rows)], d.weight(256, 256), 256, 256, bias=d.addend(256), relu=True)

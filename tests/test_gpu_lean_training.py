@@ -219,7 +219,7 @@ def test_quarter_degree_trains():
         opt.step()
     plan = model._train_engine.plan
     plan.status()
-    # bar: the chunk budget (4 GiB, gw_train.inl) with a quarter of slack, and the mesh-sized terms: per processor block about
+    # bar: the chunk budget (4 GiB, gw_train.cu) with a quarter of slack, and the mesh-sized terms: per processor block about
     # 12 tensors of the latent edges (tape and backward temporaries) at batch 1, 8 more for the encoder / decoder mesh sides
     El, De, nb = 41162, 256, 9
     bar = 1.25 * 4 * 2**30 + (12 * nb + 8) * El * De * 4 + 2**30

@@ -414,7 +414,7 @@ GUARD_KINDS = [pytest.param(k, id=n) for k, n in ((STREAM, "stream"), (BCAST, "b
 @pytest.mark.parametrize("prec", [FP32, BF16], ids=["fp32", "bf16"])
 @pytest.mark.parametrize("kind", GUARD_KINDS)
 def test_chain_refuses_non_finite(kind, prec, value):
-    """An inference chain (h_chain, prepared as gw_api.cu prepares it) with one NaN / +inf / -inf in its stage-0 source, an
+    """An inference chain (h_chain, prepared as gw_forward.cu prepares it) with one NaN / +inf / -inf in its stage-0 source, an
     addend, the residual, either weight, either bias, LayerNorm gamma or beta: status bit 3 and return code 0, no store outside
     the output rows x columns, and the next clean launch gives status 0 and the clean output bit for bit."""
     c = GuardChain(kind)

@@ -1,4 +1,4 @@
-"""-m gpu: the training step on tensor cores (`train_precision="fp32"` / `"bf16"`, gw_train.inl + gw_wgrad_tc.cu) against the
+"""-m gpu: the training step on tensor cores (`train_precision="fp32"` / `"bf16"`, gw_train.cu + gw_wgrad_tc.cu) against the
 CPU autograd oracle (fp32 and the fp64 ground truth), against the exact-fp32 training path, and its side conditions:
 convergence, repeatable weight gradients, raw input magnitudes, the 1-degree grid, and an untouched inference path."""
 import numpy as np

@@ -19,7 +19,7 @@ def test_abi_symbols_are_declared_and_bound():
     for name in ("gw_plan_create_train", "gw_train_peak_bytes"):
         assert name in declared and name in _capi._SIGNATURES
     with open(_capi.HEADER_PATH) as f:
-        assert "#define GW_ABI_VERSION 1" in f.read()
+        assert "#define GW_ABI_VERSION 2" in f.read()
 
 
 @pytest.mark.parametrize("flag", [False, True])
