@@ -354,7 +354,9 @@ static int build_chunks(gw_plan* p, TrainState* T, int batch) {
     const int pe = chunk_points(p, batch, 1.0);
     for (int s0 = 0; s0 < H;) {
       int s1 = s0 + 1;
-      while (s1 < H && eptr[s1 + 1] - eptr[s0] <= pe) ++s1;
+      // (leading slots without points join the first slot that has some, even one larger than the budget: a chunk of no
+      // points would run its row ops on zero rows)
+      while (s1 < H && (eptr[s1 + 1] - eptr[s0] <= pe || (T->enc_chunks.empty() && eptr[s1] == eptr[s0]))) ++s1;
       if (eptr[s1] == eptr[s0] && !T->enc_chunks.empty()) {  // trailing slots without points join the previous chunk
         T->enc_chunks.back().s1 = s1;
       } else {

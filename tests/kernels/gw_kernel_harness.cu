@@ -1,5 +1,5 @@
 // gw_kernel_harness.cu -- test-only shim over the internal launchers of libgwb200.so (tests/test_gpu_kernels.py,
-// tests/test_gpu_wide_training.py).
+// tests/test_gpu_wide_training.py, tests/test_gpu_chunk_primitives.py).
 //
 // Host code only: flat extern "C" wrappers that the kernel tests call through ctypes, so that every CUDA primitive of the
 // training step, the forward's CUDA-core row ops and helpers, and the device-built graphs (tests/test_gpu_forward_simt.py,
@@ -306,6 +306,30 @@ int h_batch_reduce(const float* in, int ld_in, long long rows, int width, int ba
 int h_gather_rows(const float* in, int ld_in, int src_rows, const int32_t* idx, long long rows, int width, int batch, float* out, int ld_out,
                   int accumulate, void* stream) {
   return (int)launch_gather_rows(in, ld_in, src_rows, idx, rows, width, batch, out, ld_out, accumulate != 0, (cudaStream_t)stream);
+}
+
+// ---- the bounded-memory step's row movement (gw_train.cu: build_chunks, enc_fwd / enc_bwd / enc_node_bwd, dec_fwd / dec_bwd) ----
+// launch_segsum over a CSR slice whose entries start at ptr_base, optionally adding to what out holds (tests/test_gpu_chunk_primitives.py)
+int h_segsum_range(const float* base, int ld, int width, const int32_t* ptr, const int32_t* perm, int src_rows, int rows, int batch, float* out,
+                   int ldo, int ptr_base, int accumulate, void* stream) {
+  return (int)launch_segsum(base, ld, width, ptr, perm, src_rows, rows, batch, out, ldo, (cudaStream_t)stream, ptr_base, accumulate != 0);
+}
+
+// launch_gather_rows from a table that holds the targets idx_base .. idx_base + src_rows - 1 only
+int h_gather_rows_base(const float* in, int ld_in, int src_rows, const int32_t* idx, long long rows, int width, int batch, float* out, int ld_out,
+                       int accumulate, int idx_base, void* stream) {
+  return (int)launch_gather_rows(in, ld_in, src_rows, idx, rows, width, batch, out, ld_out, accumulate != 0, (cudaStream_t)stream, idx_base);
+}
+
+// scatter 0: out row (b, j) = in row (b, idx[j]) of other_rows per sample; scatter 1: out row (b, idx[j]) = in row (b, j)
+int h_permute_rows(const float* in, int ld_in, const int32_t* idx, long long rows, int other_rows, int width, int batch, float* out, int ld_out,
+                   int scatter, void* stream) {
+  return (int)launch_permute_rows(in, ld_in, idx, rows, other_rows, width, batch, out, ld_out, scatter != 0, (cudaStream_t)stream);
+}
+
+// dst[r, c] += src[r, c] for c < width
+int h_strided_add(const float* src, int ld_src, float* dst, int ld_dst, long long rows, int width, void* stream) {
+  return (int)launch_strided_add(src, ld_src, dst, ld_dst, rows, width, (cudaStream_t)stream);
 }
 
 int h_transpose(const float* W, int rows, int cols, float* WT, void* stream) {

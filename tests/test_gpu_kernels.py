@@ -89,6 +89,10 @@ _SIGNATURES = {
     "h_segsum_chunked": [_vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _i32, _vp],
     "h_batch_reduce": [_vp, _i32, _i64, _i32, _i32, _vp, _i32, _i32, _vp],
     "h_gather_rows": [_vp, _i32, _i32, _vp, _i64, _i32, _i32, _vp, _i32, _i32, _vp],
+    "h_segsum_range": [_vp, _i32, _i32, _vp, _vp, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _vp],
+    "h_gather_rows_base": [_vp, _i32, _i32, _vp, _i64, _i32, _i32, _vp, _i32, _i32, _i32, _vp],
+    "h_permute_rows": [_vp, _i32, _vp, _i64, _i32, _i32, _i32, _vp, _i32, _i32, _vp],
+    "h_strided_add": [_vp, _i32, _vp, _i32, _i64, _i32, _vp],
     "h_transpose": [_vp, _i32, _i32, _vp, _vp],
     "h_pad_rows": [_vp, _i32, _i32, _vp, _i32, _i64, _vp, _vp],
     "h_absmax_flat": [_vp, _i64, _vp, _vp],
