@@ -171,7 +171,11 @@ int bind_all(gw_plan* p) {
     p->w_proc = true;
   }
   if (has("decoder.edge_encoder.model.0.weight")) {
-    GW_TRY(bind_mlp(p, "decoder.edge_encoder", 2, He, De, 2, true, &p->dec_edge_enc));  // 2 hidden layers hard-coded: assimilator_decoder.py:109
+    // 2 hidden layers in the forecaster / assimilator decoders (hard-coded, assimilator_decoder.py:109); hidden_layers_processor_edge
+    // in the regional forecaster's decoder_edge_encoder (regional_forecast.py:206-213): the depth is that of the table's Linears
+    int dec_edge_L = 0;
+    while (has(("decoder.edge_encoder.model." + std::to_string(2 * (dec_edge_L + 1)) + ".weight").c_str())) ++dec_edge_L;
+    GW_TRY(bind_mlp(p, "decoder.edge_encoder", 2, He, De, dec_edge_L, true, &p->dec_edge_enc));
     GW_TRY(bind_mlp(p, "decoder.graph_processor.blocks.0.edge_model.edge_mlp", 2 * Dn + De, He, De, Le, true, &p->dec_blk_edge));
     GW_TRY(bind_mlp(p, "decoder.graph_processor.blocks.0.node_model.node_mlp", Dn + De, Hn, Dn, Ln, true, &p->dec_blk_node));
     // (no norm in the forecaster / assimilator decoders, decoder.py / assimilator_decoder.py; the regional forecaster builds its

@@ -30,7 +30,8 @@ cudaError_t launch_ln_bwd(const float* dy, int ld_dy, const float* z, int ld_z, 
 constexpr int LN_BWD_MAX_N = 1024;  // widest row launch_ln_bwd takes (rows of more than 256 columns run on a kernel of their own)
 cudaError_t launch_batch_reduce(const float* in, int ld_in, long long rows, int width, int batch, float* out, int ld_out, bool accumulate,
                                 cudaStream_t st);
-// idx_base: `in` holds the targets idx_base .. idx_base + src_rows - 1 only (a chunk of the training step's grid-sized stages)
+// idx_base: `in` holds the targets idx_base .. idx_base + src_rows - 1 only (a chunk of the training step's grid-sized stages).
+// Any width and strides: float4 where they and both pointers allow it, one float per thread otherwise.
 cudaError_t launch_gather_rows(const float* in, int ld_in, int src_rows, const int32_t* idx, long long rows, int width, int batch, float* out,
                                int ld_out, bool accumulate, cudaStream_t st, int idx_base = 0);
 // rows through a permutation, per sample: gather (out row j = in row idx[j] of other_rows) or scatter (out row idx[j] of other_rows = in row j)
@@ -46,7 +47,8 @@ cudaError_t launch_segsum_chunked(const float* base, int ld, const int32_t* ptr,
 cudaError_t launch_seg_carry(const float* carry, const int32_t* seg_dst, int rows, int seg_rows, int batch, float* out, int ldo,
                              cudaStream_t stream);
 // ptr_base: subtracted from every ptr entry (a CSR slice over a range of rows that starts at row ptr_base of the full table);
-// accumulate: out += the segment sums (a per-segment sum split over row ranges, added in the order of the calls)
+// accumulate: out += the segment sums (a per-segment sum split over row ranges, added in the order of the calls).  Any width and
+// strides: float4 where they and both pointers allow it, one float per thread otherwise, summing each column in the same order.
 cudaError_t launch_segsum(const float* base, int ld, int width, const int32_t* ptr, const int32_t* perm, int src_rows,
                           int rows, int batch, float* out, int ldo, cudaStream_t stream, int ptr_base = 0, bool accumulate = false);
 

@@ -180,12 +180,27 @@ __global__ void __launch_bounds__(NT) gw_rowop_f32_kernel(const GemmOp op) {
 // out[(b*rows + i), :] = sum over CSR segment i of base rows (left to right, the reference's scatter_add order).
 // One 64-thread CTA per (segment, sample): float4 per thread across 256 columns, rows read fully coalesced.  Serves the
 // encoder's lat/lon -> mesh aggregation, whose segments are very skewed (a polar cell collects thousands of points).
+// VEC = false: one float per thread, for widths, strides or base pointers that float4 cannot address (an edge_dim of 30); each
+// column is summed in the same order, so a width the float4 path also takes gives the same bits either way.
+template <bool VEC>
 __global__ void __launch_bounds__(64) gw_segsum_kernel(const float* __restrict__ base, int ld, int width,
                                                        const int32_t* __restrict__ ptr, const int32_t* __restrict__ perm,
                                                        int src_rows, int rows, float* __restrict__ out, int ldo, int ptr_base,
                                                        int accumulate) {
   const int i = blockIdx.x, b = blockIdx.y;
   const int j0 = __ldg(ptr + i) - ptr_base, j1 = __ldg(ptr + i + 1) - ptr_base;
+  if (!VEC) {
+    for (int c = threadIdx.x; c < width; c += 64) {
+      float acc = 0.f;
+      for (int j = j0; j < j1; ++j) {
+        const int e = perm ? __ldg(perm + j) : j;
+        acc += __ldg(base + ((size_t)b * src_rows + e) * ld + c);
+      }
+      float* o = out + ((size_t)b * rows + i) * ldo + c;
+      *o = accumulate ? *o + acc : acc;
+    }
+    return;
+  }
   for (int c = threadIdx.x * 4; c < width; c += 256) {
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int j = j0; j < j1; ++j) {
@@ -202,11 +217,16 @@ __global__ void __launch_bounds__(64) gw_segsum_kernel(const float* __restrict__
   }
 }
 
+// float4 access to rows of stride ld from p: 16-byte aligned rows, whole float4 per row
+static bool float4_rows(const void* p, int ld, int width) { return !(reinterpret_cast<uintptr_t>(p) & 15) && !(ld & 3) && !(width & 3); }
+
 cudaError_t launch_segsum(const float* base, int ld, int width, const int32_t* ptr, const int32_t* perm, int src_rows,
                           int rows, int batch, float* out, int ldo, cudaStream_t stream, int ptr_base, bool accumulate) {
   if (rows <= 0 || batch <= 0) return cudaSuccess;
-  if ((width & 3) || (ld & 3) || (ldo & 3)) return cudaErrorInvalidValue;
-  gw_segsum_kernel<<<dim3(rows, batch), 64, 0, stream>>>(base, ld, width, ptr, perm, src_rows, rows, out, ldo, ptr_base, accumulate ? 1 : 0);
+  if (float4_rows(base, ld, width) && float4_rows(out, ldo, width))
+    gw_segsum_kernel<true><<<dim3(rows, batch), 64, 0, stream>>>(base, ld, width, ptr, perm, src_rows, rows, out, ldo, ptr_base, accumulate ? 1 : 0);
+  else
+    gw_segsum_kernel<false><<<dim3(rows, batch), 64, 0, stream>>>(base, ld, width, ptr, perm, src_rows, rows, out, ldo, ptr_base, accumulate ? 1 : 0);
   count_launch();
   return cudaGetLastError();
 }
@@ -568,17 +588,27 @@ cudaError_t launch_batch_reduce(const float* in, int ld_in, long long rows, int 
   return cudaGetLastError();
 }
 // out[(b * rows + j), c] (+)= in[(b * src_rows + idx[j] - idx_base), c]   (gradient of a per-target sum: every row receives its target's
-// gradient; idx_base: the first target of a table that holds a range of targets)
+// gradient; idx_base: the first target of a table that holds a range of targets).  VEC: four columns per thread (float4), else one
+// (any width, stride and alignment).
+template <bool VEC>
 __global__ void gw_gather_rows_kernel(const float* __restrict__ in, int ld_in, int src_rows, const int32_t* __restrict__ idx, long long rows, int width,
                                       int batch, float* __restrict__ out, int ld_out, int accumulate, int idx_base) {
-  const long long total = rows * batch * (width >> 2);
-  const int q = width >> 2;
+  constexpr int V = VEC ? 4 : 1;
+  const int q = width / V;
+  const long long total = rows * batch * q;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     const long long rj = e / q;
-    const int c = (int)(e - rj * q) * 4;
+    const int c = (int)(e - rj * q) * V;
     const long long b = rj / rows, j = rj - b * rows;
-    const float4 v = __ldg(reinterpret_cast<const float4*>(in + (b * src_rows + (__ldg(idx + j) - idx_base)) * ld_in + c));
-    float4* o = reinterpret_cast<float4*>(out + rj * ld_out + c);
+    const float* src = in + (b * src_rows + (__ldg(idx + j) - idx_base)) * ld_in + c;
+    float* dst = out + rj * ld_out + c;
+    if (!VEC) {
+      const float v = __ldg(src);
+      *dst = accumulate ? *dst + v : v;
+      continue;
+    }
+    const float4 v = __ldg(reinterpret_cast<const float4*>(src));
+    float4* o = reinterpret_cast<float4*>(dst);
     if (accumulate) {
       float4 t = *o;
       t.x += v.x, t.y += v.y, t.z += v.z, t.w += v.w;
@@ -590,9 +620,11 @@ __global__ void gw_gather_rows_kernel(const float* __restrict__ in, int ld_in, i
 }
 cudaError_t launch_gather_rows(const float* in, int ld_in, int src_rows, const int32_t* idx, long long rows, int width, int batch, float* out,
                                int ld_out, bool accumulate, cudaStream_t st, int idx_base) {
-  if (rows <= 0 || batch <= 0) return cudaSuccess;
-  if ((width & 3) || (ld_in & 3) || (ld_out & 3)) return cudaErrorInvalidValue;
-  gw_gather_rows_kernel<<<GRID_SMS * 8, 256, 0, st>>>(in, ld_in, src_rows, idx, rows, width, batch, out, ld_out, accumulate ? 1 : 0, idx_base);
+  if (rows <= 0 || batch <= 0 || width <= 0) return cudaSuccess;
+  if (float4_rows(in, ld_in, width) && float4_rows(out, ld_out, width))
+    gw_gather_rows_kernel<true><<<GRID_SMS * 8, 256, 0, st>>>(in, ld_in, src_rows, idx, rows, width, batch, out, ld_out, accumulate ? 1 : 0, idx_base);
+  else
+    gw_gather_rows_kernel<false><<<GRID_SMS * 8, 256, 0, st>>>(in, ld_in, src_rows, idx, rows, width, batch, out, ld_out, accumulate ? 1 : 0, idx_base);
   count_launch();
   return cudaGetLastError();
 }

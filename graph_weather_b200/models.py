@@ -606,6 +606,12 @@ class _Wrapper(nn.Module):
                     hidden_dec=dec["hidden_dec"], hidden_layers_dec=dec["hidden_layers_dec"], num_blocks=num_blocks)  # fmt: skip
         self._engine = _new_engine(dims, precision, [self.encoder._upload_graphs, self.decoder._upload_graphs])
         _validate_train_precision(train_precision, dims)
+        if dec["edge_dim"] != dims["edge_dim"]:
+            # GraphCast(hidden_dim != 256): the reference's decoder keeps its default 256-wide edges (graphcast/model.py:97-111
+            # passes no output_edge_dim) while the encoder and processor edges are hidden_dim wide
+            raise NotImplementedError(
+                f"decoder edge width {dec['edge_dim']} differs from the encoder's {dims['edge_dim']}: the CUDA plan runs one edge width "
+                "through the whole network, so this model is not supported (GraphCast runs with hidden_dim=256 only)")
         self.train_precision = train_precision
 
     def _named(self):

@@ -29,6 +29,14 @@ CASES = {
         kw=dict(node_dim=64, edge_dim=64, num_blocks=3, hidden_dim_processor_node=64, hidden_dim_processor_edge=64,
                 hidden_dim_decoder=32, feature_dim=10, aux_dim=4),
     ),  # fmt: skip
+    # every width or depth that could be swapped for another differs: node 48 / edge 80, processor hidden 96 / 64, hidden
+    # layers 1 (node) / 3 (edge) / 3 (decoder), decoder hidden 40, 7 + 5 input channels
+    "forecaster_mixed_shapes": dict(
+        step=10, batch=2, seed=8,
+        kw=dict(node_dim=48, edge_dim=80, num_blocks=2, hidden_dim_processor_node=96, hidden_dim_processor_edge=64,
+                hidden_layers_processor_node=1, hidden_layers_processor_edge=3, hidden_dim_decoder=40,
+                hidden_layers_decoder=3, feature_dim=7, aux_dim=5),
+    ),  # fmt: skip
 }
 STAGE_STRIDE = 53  # stage outputs are stored for every 53rd mesh row only (keeps fixtures small)
 

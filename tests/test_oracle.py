@@ -13,7 +13,7 @@ def _grid(step):
     return [(float(lat), float(lon)) for lat in range(-90, 90, step) for lon in range(0, 360, step)]
 
 
-@pytest.mark.parametrize("name", ["forecaster_10deg_b2", "forecaster_small_hidden64", "forecaster_5deg_b1"])
+@pytest.mark.parametrize("name", ["forecaster_10deg_b2", "forecaster_small_hidden64", "forecaster_5deg_b1", "forecaster_mixed_shapes"])
 def test_restatement_matches_reference(golden_dir, name):
     z = np.load(os.path.join(golden_dir, name + ".npz"))
     cfg = json.loads(str(z["config"]))
@@ -24,10 +24,11 @@ def test_restatement_matches_reference(golden_dir, name):
     fdim = kw.get("feature_dim", 78)
     x = weights.make_features(cfg["batch"], len(ll), fdim + kw.get("aux_dim", 24), cfg["seed"])
     nb = kw.get("num_blocks", 9)
+    hl = dict(hl_node=kw.get("hidden_layers_processor_node", 2), hl_edge=kw.get("hidden_layers_processor_edge", 2))
     with torch.no_grad():
-        enc_x, ei, ea = restate.encoder_forward(sd, g, x)
-        proc_x = restate.processor_forward(sd, enc_x, ei, ea, nb)
-    out = restate.forecaster_forward(sd, g, x, feature_dim=fdim, num_blocks=nb)
+        enc_x, ei, ea = restate.encoder_forward(sd, g, x, **hl)
+        proc_x = restate.processor_forward(sd, enc_x, ei, ea, nb, **hl)
+    out = restate.forecaster_forward(sd, g, x, feature_dim=fdim, num_blocks=nb, hl_dec=kw.get("hidden_layers_decoder", 2), **hl)
     # same ops in the same order on the same machine class: expect (near) bit equality; 1e-5 is the tolerance the
     # reference's own equivalence tests use (tests/models/layers/test_efficient_batching.py:53,91)
     assert np.abs(enc_x.numpy()[::53] - z["enc_x_sub"]).max() < 1e-5

@@ -1,6 +1,7 @@
 """The bars of tests/training_oracle.py, without a GPU: on a small case (30-degree grid, 2 blocks) each bar passes the fp32
 oracle's own step given as "ours", and fails it when one parameter's gradient is off by 1 % (the fp32 bars) or is noise (the bf16
-bar)."""
+bar).  The same holds on the mixed shape of tests/test_gpu_model_shapes.py (unequal node / edge and hidden widths, 1 / 3 / 3
+hidden layers), whose oracle takes its hidden-layer counts from the case's shape arguments."""
 import pytest
 import torch
 
@@ -28,6 +29,17 @@ BF16_BARS = {
 @pytest.fixture(scope="module")
 def case():
     return forecaster_case(30, 1, 7, num_blocks=2)
+
+
+# tests/test_gpu_model_shapes.py's mixed shape, and a parameter of its deepest edge MLP (model.4: the third hidden layer)
+MIXED = dict(node_dim=48, edge_dim=80, hidden_dim_processor_node=96, hidden_dim_processor_edge=64, hidden_layers_processor_node=1,
+             hidden_layers_processor_edge=3, hidden_dim_decoder=40, hidden_layers_decoder=3, feature_dim=7, aux_dim=5, num_blocks=2)
+MIXED_PARAM = "processor.graph_processor.blocks.1.edge_model.edge_mlp.model.4.weight"
+
+
+@pytest.fixture(scope="module")
+def mixed_case():
+    return forecaster_case(30, 1, 7, **MIXED)
 
 
 def _with(ref32, k, g):
@@ -59,3 +71,37 @@ def test_the_parameter_count_is_checked(case):
         check_fp32_bars(ref32, ref32, ref64, **dict(FP32_BARS["taped_simt"], n_params=len(ref32[3]) + 1))
     with pytest.raises(AssertionError):
         check_bf16_bars(ref32, ref32, ref64, **dict(BF16_BARS["taped"], n_params=len(ref32[3]) - 1))
+
+
+def test_mixed_shape_oracle_follows_the_shape(mixed_case):
+    """Every parameter of the shape gets a gradient of its own shape, and the 3-deep edge MLPs' last hidden layer is reached."""
+    from oracle import weights
+
+    ref32, ref64 = mixed_case[5:]
+    shapes = weights.forecaster_shapes(**MIXED)
+    assert list(ref64[3]) == list(shapes)
+    assert all(tuple(ref64[3][k].shape) == s for k, s in shapes.items())
+    assert float(ref64[3][MIXED_PARAM].abs().max()) > 0
+    assert float(ref64[3]["decoder.node_decoder.model.6.weight"].abs().max()) > 0  # Linear 3 of the 3-hidden-layer decoder
+
+
+# the fp32 bars tests/test_gpu_model_shapes.py holds its fp32_simt and fp32-mode steps to
+MIXED_FP32_BARS = {"fp32_simt": FP32_BARS["taped_simt"], "fp32_simt_floor": dict(FP32_BARS["taped_simt"], floor=2e-4),
+                   "fp32": dict(FP32_BARS["taped_simt"], floor=8e-3, feat_floor=True, median=False)}
+
+
+@pytest.mark.parametrize("name", list(MIXED_FP32_BARS))
+def test_fp32_bars_mixed_shape(mixed_case, name):
+    ref32, ref64 = mixed_case[5:]
+    check_fp32_bars(ref32, ref32, ref64, **MIXED_FP32_BARS[name])
+    with pytest.raises(AssertionError, match=MIXED_PARAM):
+        check_fp32_bars(_with(ref32, MIXED_PARAM, ref32[3][MIXED_PARAM] * 1.01), ref32, ref64, **MIXED_FP32_BARS[name])
+
+
+@pytest.mark.parametrize("bars", [BF16_BARS["taped"], dict(BF16_BARS["taped"], cos_bar=0.98, ill_cos_bar=0.975, total_cos=0.995)])
+def test_bf16_bars_mixed_shape(mixed_case, bars):
+    ref32, ref64 = mixed_case[5:]
+    check_bf16_bars(ref32, ref32, ref64, **bars)
+    noise = torch.randn(ref32[3][MIXED_PARAM].shape, generator=torch.Generator().manual_seed(0))
+    with pytest.raises(AssertionError, match=MIXED_PARAM):
+        check_bf16_bars(_with(ref32, MIXED_PARAM, noise), ref32, ref64, **bars)

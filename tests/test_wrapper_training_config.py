@@ -106,3 +106,13 @@ def test_use_checkpointing_assigned_later_selects_the_step():
             m.use_checkpointing = flag
             assert m._training_engine().train_only is flag, type(m).__name__
             assert m._train_engine is m._training_engine()
+
+
+def test_graphcast_with_another_edge_width_in_the_decoder_is_refused():
+    """GraphCast(hidden_dim=96): the reference's decoder keeps 256-wide edges while the encoder and processor use hidden_dim.  The
+    CUDA plan has one edge width, so the model is refused at construction, in words, instead of failing at its first forward."""
+    from graph_weather_b200 import GraphCast
+
+    with pytest.raises(NotImplementedError, match="decoder edge width 256 differs from the encoder's 96"):
+        GraphCast(LL, num_processor_blocks=1, hidden_dim=96)
+    GraphCast(LL, num_processor_blocks=1, hidden_layers=3)  # the 256-wide trunk with three hidden layers is taken

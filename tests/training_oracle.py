@@ -34,19 +34,22 @@ def cos(a, b):
     return float(torch.nn.functional.cosine_similarity(a.double().cpu().flatten(), b.double().cpu().flatten(), dim=0))
 
 
-def forecaster_oracle_step(sd, ll, x, target, var, dtype, feature_dim=78, num_blocks=9, constraint=None):
+def forecaster_oracle_step(sd, ll, x, target, var, dtype, feature_dim=78, num_blocks=9, constraint=None, hl_node=2, hl_edge=2,
+                           hl_dec=2):
     """One training step of the reference arithmetic on the CPU under torch.autograd, in fp32 (what the reference runs) or fp64
     (ground truth for the tolerances): encoder -> processor -> decoder + the first feature_dim features, then the restated
-    PhysicalConstraintLayer (forecast.py:235-246) when `constraint` names one, then NormalizedMSELoss.
+    PhysicalConstraintLayer (forecast.py:235-246) when `constraint` names one, then NormalizedMSELoss.  hl_node / hl_edge /
+    hl_dec are the hidden-layer counts of the node MLPs, the edge MLPs and the node decoder.
     Returns (out, loss, d features, {name: grad})."""
     from oracle import restate
 
     sd_g = {k: v.to(dtype).clone().requires_grad_(True) for k, v in sd.items()}
     xg = x.to(dtype).clone().requires_grad_(True)
     g = {k: (v.to(dtype) if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in restate.build_forecaster_graphs(ll).items()}
-    ex, ei, ea = restate.encoder_forward(sd_g, g, xg)
-    px = restate.processor_forward(sd_g, ex, ei, ea, num_blocks)
-    out = restate.assimilator_decoder_forward(sd_g, g, px, x.shape[0]) + xg[..., :feature_dim]
+    hl = dict(hl_node=hl_node, hl_edge=hl_edge)
+    ex, ei, ea = restate.encoder_forward(sd_g, g, xg, **hl)
+    px = restate.processor_forward(sd_g, ex, ei, ea, num_blocks, **hl)
+    out = restate.assimilator_decoder_forward(sd_g, g, px, x.shape[0], hl_dec=hl_dec, **hl) + xg[..., :feature_dim]
     if constraint is not None:
         from test_constraint_grads import grid_mapping, restate_constraint, rows_to_grid
 
@@ -87,8 +90,8 @@ _CASES = {}
 
 def forecaster_case(step, batch, seed, constraint=None, shift=0.0, **shape_kw):
     """A seeded forecaster case on the `step`-degree grid: (lat_lons, state_dict, features, target, variances, oracle step in fp32,
-    oracle step in fp64).  `shape_kw` are weights.forecaster_shapes' arguments (and the oracle's feature_dim / num_blocks); the
-    first feature_dim input channels are shifted by `shift`.  Cached per key: the oracle steps are the slow part."""
+    oracle step in fp64).  `shape_kw` are weights.forecaster_shapes' arguments (and the oracle's feature_dim / num_blocks /
+    hidden-layer counts); the first feature_dim input channels are shifted by `shift`.  Cached per key: the oracle steps are the slow part."""
     key = (step, batch, seed, constraint, shift, tuple(sorted(shape_kw.items())))
     if key not in _CASES:
         from oracle import weights
@@ -102,7 +105,9 @@ def forecaster_case(step, batch, seed, constraint=None, shift=0.0, **shape_kw):
         rng = np.random.Generator(np.random.PCG64(seed))
         target = torch.from_numpy(rng.standard_normal((batch, len(ll), F)).astype(np.float32))
         var = rng.uniform(0.5, 2.0, F).astype(np.float32).tolist()
-        refs = [forecaster_oracle_step(sd, ll, x, target, var, dt, F, nb, constraint) for dt in (torch.float32, torch.float64)]
+        hl = dict(hl_node=shape_kw.get("hidden_layers_processor_node", 2), hl_edge=shape_kw.get("hidden_layers_processor_edge", 2),
+                  hl_dec=shape_kw.get("hidden_layers_decoder", 2))
+        refs = [forecaster_oracle_step(sd, ll, x, target, var, dt, F, nb, constraint, **hl) for dt in (torch.float32, torch.float64)]
         _CASES[key] = (ll, sd, x, target, var, *refs)
     return _CASES[key]
 
