@@ -92,7 +92,8 @@ struct TcWeights {
   float gain = 0.f;                        // K_src * max|W|: |A.W^T| <= gain * max|A|
 };
 TcWeights tc_weights(const void* img, int K_src, int N_src, float wamax, int parts);
-// bound of a LayerNorm'd row of N columns: sqrt(N) max|gamma| + max|beta|
+// bound of a LayerNorm'd row of N real columns (n_valid, not the padded width): sqrt(N) max|gamma| + max|beta|, since a
+// normalised row has sum x^2 <= N
 float tc_ln_bound(int N, float gamma_amax, float beta_amax);
 // Power of two a weight image is stored times: fp16 hi|lo images (parts 2) bring max|W| into [2048, 4096) so the lo parts stay
 // normal (the host's pack_tc_weights uses the same rule); bf16 images are not scaled.

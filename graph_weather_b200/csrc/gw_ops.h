@@ -72,7 +72,7 @@ struct TcLayer {
   const float* bias = nullptr;
   RowSrc add[2];              // epilogue addends (SRC_BCAST / SRC_GATHER / SRC_STREAM), N wide
   int32_t relu = 0;
-  const float* ln_g = nullptr;  // LayerNorm over N (eps 1e-5) if non-null
+  const float* ln_g = nullptr;  // LayerNorm over the n_valid real columns (eps 1e-5) if non-null
   const float* ln_b = nullptr;
   RowSrc residual;            // added after LN
   float* out = nullptr;       // fp32 result rows -> out[(b*rows+i)*ldo + n], n < out_cols (null: not stored)
@@ -83,7 +83,7 @@ struct TcLayer {
   // operand range (gw_tc3.cu): a rigorous magnitude bound travels with every tensor so that each fp16-split operand can be
   // scaled by a power of two into the fp16 range.  |A . W^T| <= gain * max|A| with gain = K * max|W|; off = max|bias|.
   float gain = 0.f, off = 0.f;
-  float ln_bound = 0.f;       // LayerNorm layers: sqrt(N) * max|gamma| + max|beta| bounds the normalised row
+  float ln_bound = 0.f;       // LayerNorm layers: sqrt(n_valid) * max|gamma| + max|beta| bounds the normalised row
   float* out_bound = nullptr; // device float the kernel sets to the bound of this layer's result (CTA 0), for `out` consumers
   // fused per-target sum of the result rows (graph_net_block.py:188 scatter_sum): rows are grouped by target (seg_dst
   // non-decreasing, segments of <= 8 rows); each segment sum goes to seg_out, the part of a segment behind a 16-row group

@@ -1156,7 +1156,10 @@ cudaError_t launch_chain_tc3(const TcChain& ch_in, cudaStream_t stream) {
     if (!L.Wp || (L.K & 63) || (L.N & 15) || L.N > 256 || L.N <= 0 || L.n_valid <= 0 || L.n_valid > L.N) return cudaErrorInvalidValue;
     if (L.feeds_next && (L.N & 63)) return cudaErrorInvalidValue;
     if (L.ln_g && L.add[0].kind != SRC_NONE) return cudaErrorInvalidValue;  // addends are applied before ReLU, not before LayerNorm
-    if (L.ln_g && (L.n_valid != L.N || ++n_ln > 2)) return cudaErrorInvalidValue;
+    // A LayerNorm normalises over the n_valid real columns (ln_stats; the padding columns of the accumulator are exactly zero: zero
+    // weight rows and bias).  Padded ones (N = n_valid rounded up to 16) run only as the one-layer chain of a training row op, which
+    // takes the general epilogue: its stores, pre-LayerNorm store and residual stop at n_valid columns (out_cols, source widths).
+    if (L.ln_g && ((L.n_valid != L.N && ch.n_layers != 1) || ++n_ln > 2)) return cudaErrorInvalidValue;
     if (L.add[0].kind == SRC_NONE && L.add[1].kind != SRC_NONE) return cudaErrorInvalidValue;
     for (int a = 0; a < 2; ++a)
       if (L.add[a].kind != SRC_NONE && L.add[a].kind != SRC_STREAM && L.add[a].kind != SRC_BCAST && L.add[a].kind != SRC_GATHER &&

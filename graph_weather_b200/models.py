@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import contextlib
 import os
+import weakref
 from dataclasses import dataclass
 from typing import Optional
 
@@ -240,19 +241,22 @@ def _maybe_check(plan):
 
 
 class _TrainFn(torch.autograd.Function):
-    """autograd node of one training forward of a wrapper (GraphWeatherForecaster, GraphCast, GraphWeatherAssimilator): forward =
-    gw_train_forward_tape (activations kept on a tape, `_capi.Tape`), backward = gw_train_backward_tape (gradients of every
-    parameter under its reference name, and of the features when they require grad).  One backward per forward.  Every forward
-    makes a tape that this node owns: its backward consumes it, and dropping the graph without a backward frees it.  Outside
-    `multi_step()` a forward first closes the tape of the previous forward made outside a window (`_Engine.last_tape`), which
-    replaces that forward's activations; inside it, a forward closes nothing.
+    """autograd node of one training forward of a wrapper (GraphWeatherForecaster, GraphCast, GraphWeatherAssimilator,
+    RegionalForecaster): forward = gw_train_forward_tape (activations kept on a tape, `_capi.Tape`), backward =
+    gw_train_backward_tape (gradients of every bound parameter, and of the features when they require grad).  One backward per
+    forward.  Every forward makes a tape that this node owns: its backward consumes it, and dropping the graph without a backward
+    frees it.  Outside `multi_step()` a forward first closes the tape of the previous forward made outside a window
+    (`_Engine.last_tape`), which replaces that forward's activations; inside it, a forward closes nothing.
 
-    The wrapper (`_Wrapper`) supplies its training engine (`_training_engine()`), its named parameters (`_named()`) and its output
-    shape (`_out_shape(batch)`).  `obs` (the assimilator's lat_lon_heights, else None) is built into the training plan's observation
-    graph for this call, as inference builds it for every call."""
+    The wrapper supplies its training engine (`_training_engine()`), the tensors the plan uploads (`_named()`), its output shape
+    (`_out_shape(batch)`) and `bindings`: what the step differentiates, one (name the plan binds, tensor uploaded under that name,
+    parameter, gradient map) per entry of `params` (`_grad_bindings()`).  The step returns each gradient shaped like the uploaded
+    tensor; the map turns it into the parameter's gradient (None: it is the parameter's already).  `obs` (the assimilator's
+    lat_lon_heights, else None) is built into the training plan's observation graph for this call, as inference builds it for
+    every call."""
 
     @staticmethod
-    def forward(ctx, model, features, obs, *params):
+    def forward(ctx, model, features, obs, bindings, *params):
         B = features.shape[0]
         eng = model._training_engine()
         plan = eng.ensure(features.device, B, model._named(), grow=None if obs is None else dict(n_in=obs.shape[0]))
@@ -273,11 +277,13 @@ class _TrainFn(torch.autograd.Function):
             raise
         if not in_window:
             eng.last_tape = tape
+        tape.node = weakref.ref(ctx)  # alive while the graph that will run this backward is (`_pending_tape`)
         ctx.tape = tape
         ctx.model, ctx.plan, ctx.eng = model, plan, eng
         ctx.feat_shape, ctx.feat_grad = tuple(f.shape), bool(features.requires_grad)
-        ctx.names = [k for k, _ in model.named_parameters()]
-        ctx.pshapes = [tuple(q.shape) for q in params]
+        ctx.names = [name for name, _, _, _ in bindings]
+        ctx.pshapes = [tuple(bound.shape) for _, bound, _, _ in bindings]
+        ctx.maps = [to_param for _, _, _, to_param in bindings]
         ctx.pgrad = [bool(q.requires_grad) for q in params]
         ctx.keep = f  # the tape reads the features again in the backward (weight gradient of the first Linear)
         return out
@@ -300,7 +306,27 @@ class _TrainFn(torch.autograd.Function):
             ctx.tape.close()
             ctx.tape = None
         _maybe_check(ctx.plan)
-        return (None, gfeat, None) + tuple(gr if need else None for gr, need in zip(grads, ctx.pgrad))
+        return (None, gfeat, None, None) + tuple((gr if to_param is None else to_param(gr)) if need else None
+                                                 for gr, to_param, need in zip(grads, ctx.maps, ctx.pgrad))
+
+
+def _pending_tape(engine) -> bool:
+    """The engine's plan holds a tape that a backward still needs: made by a forward whose backward has not run, and whose autograd
+    graph is still alive (a dropped graph's tape is only waiting to be closed)."""
+    plan = engine.plan
+    return plan is not None and any(getattr(t, "node", None) is not None and t.node() is not None for t in plan.live_tapes())
+
+
+def _switch_training_engine(engines: dict, bounded: bool, make) -> _Engine:
+    """engines[bounded], created by make(bounded) on first use; the other step's engine gives up its plan (see
+    `_Wrapper._training_engine`)."""
+    if bounded not in engines:
+        engines[bounded] = make(bounded)
+    other = engines.get(not bounded)
+    if other is not None and other.plan is not None:
+        other.plan.close()
+        other.plan = None
+    return engines[bounded]
 
 
 def _wants_grad(model, features):
@@ -617,6 +643,10 @@ class _Wrapper(nn.Module):
     def _named(self):
         return [(k, v) for k, v in self.state_dict(keep_vars=True).items()]
 
+    def _grad_bindings(self):
+        """`_TrainFn`'s bindings: every parameter under its own name, its gradient as the step returns it."""
+        return [(k, q, q, None) for k, q in self.named_parameters()]
+
     def _out_shape(self, batch):
         return (batch, self.decoder.num_latlons, self.decoder.output_dim)
 
@@ -633,17 +663,13 @@ class _Wrapper(nn.Module):
         0.25 degree grid trains on one 80 GB card) -- or the taped step (the default), which is faster where it fits.  Each
         engine is created on first use.  Only one holds a plan: switching closes the other's, so a backward of a forward made
         under the other step raises "one backward per forward"."""
-        engines = self.__dict__.setdefault("_train_engines", {})
-        bounded = self._bounded_step()
-        if bounded not in engines:
-            engines[bounded] = _new_engine(self._engine.dims, self.train_precision, [self.encoder._upload_graphs, self.decoder._upload_graphs],
-                                           train_only=bounded)  # fmt: skip
-        other = engines.get(not bounded)
-        if other is not None and other.plan is not None:
-            other.plan.close()
-            other.plan = None
-        self.__dict__["_train_engine"] = engines[bounded]
-        return engines[bounded]
+        def make(bounded):
+            return _new_engine(self._engine.dims, self.train_precision, [self.encoder._upload_graphs, self.decoder._upload_graphs],
+                               train_only=bounded)  # fmt: skip
+
+        eng = _switch_training_engine(self.__dict__.setdefault("_train_engines", {}), self._bounded_step(), make)
+        self.__dict__["_train_engine"] = eng
+        return eng
 
     def _inference_plan(self, features, obs=None):
         """The inference engine's plan for this batch (and for the assimilator, these observations) with the current weights."""
@@ -689,7 +715,8 @@ class _Wrapper(nn.Module):
     def _train_or_infer(self, features, obs=None):
         """The training step in train mode with autograd on (`_wants_grad`), otherwise inference."""
         if _wants_grad(self, features):
-            return _TrainFn.apply(self, features, obs, *[q for _, q in self.named_parameters()])
+            bindings = self._grad_bindings()
+            return _TrainFn.apply(self, features, obs, bindings, *[q for _, _, q, _ in bindings])
         return self._infer(features, self._out_shape(features.shape[0]), obs)
 
 

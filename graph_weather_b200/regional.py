@@ -10,6 +10,11 @@ the reference's parameter names (`node_encoder`, `encoder_gnn`, `decoder_edge_en
 and hands them to the plan under the names the C ABI binds (include/gw_b200.h), with the region's embedding rows as
 `encoder.h3_nodes`.  A plan is sized for one region; a region with other counts gets its own plan (a handful are kept).
 
+Training (`train_precision`, as on the other wrappers): in train mode with autograd on, a forward runs the forecaster's CUDA
+training step on training plans of the region (`use_checkpointing=True`: the bounded-memory step).  `h3_embeddings.grad` is
+table-shaped, as the reference's: the region's rows at their cells, zero elsewhere.  A region's plans are kept while a backward
+still needs one of their tapes, so the losses of more regions than the cache holds can be summed into one `backward()`.
+
 Optional boundary nudging (:44-130): a distance-based relaxation prior plus a learned one-hidden-layer correction, blended
 with a caller-supplied global forecast.  It is a [B, N, 2F+1] -> 1 element-wise tail outside the GNN; it runs as device
 tensor ops (no kernels of this library), exactly the reference's arithmetic.
@@ -28,12 +33,15 @@ import torch.nn as nn
 
 from . import graphs, h3lite
 from .dynamic_graph_builder import DynamicGraphBuilder
-from .models import MLP, GraphProcessor, Processor, _Engine, _maybe_check, _no_host_path, _validate_precision, _wants_grad
+from .models import (MLP, GraphProcessor, Processor, _maybe_check, _new_engine, _no_host_path, _pending_tape, _switch_training_engine,
+                     _TrainFn, _validate_precision, _validate_train_precision, _Wrapper, _wants_grad)  # fmt: skip
 
 
 @dataclass
 class RegionalForecasterConfig:
-    """regional_forecast.py:16-41 (same fields and defaults) + `precision` of the CUDA path."""
+    """regional_forecast.py:16-41 (same fields and defaults) + `precision` of the CUDA path and `train_precision` of its training
+    step: None (the default) leaves the model inference-only, 'fp32_simt' | 'fp32' | 'bf16' train it as GraphWeatherForecaster's
+    `train_precision` does (the tensor-core values need the 256-wide trunk and output_dim <= 256)."""
 
     resolution: int = 2
     feature_dim: int = 78
@@ -53,6 +61,7 @@ class RegionalForecasterConfig:
     enable_nudging: bool = False
     nudging_hidden_dim: int = 64
     precision: str = "auto"
+    train_precision: Optional[str] = None
 
     def build(self) -> "RegionalForecaster":
         return RegionalForecaster(self)
@@ -107,6 +116,7 @@ class _RegionGraphs:
         lperm, self.lat_src, self.lat_dst, self.lat_ptr = graphs._finish_target_sorted(li[0], li[1], self.n_mesh)
         self.lat_attr = np.ascontiguousarray(lat.edge_attr.numpy()[lperm], dtype=np.float32)
         self.n_lat_edges = int(li.shape[1])
+        self.h3_idx = None  # h3_indices on the device (set with the region's embedding rows, RegionalForecaster._plan_named)
         # decoder = the encoder edges reversed (:247-249): exactly one edge per coordinate, from its own cell
         self.dec_src = self.mesh_local
         self.dec_ptr = np.arange(n + 1, dtype=np.int32)
@@ -159,8 +169,18 @@ class RegionalForecaster(nn.Module):
         )  # fmt: skip
         probe = dict(self._base_dims, n_in=1, n_out=1, n_mesh=1, n_lat_edges=1, n_dec_edges=1)
         _validate_precision(c.precision, probe)
+        if c.train_precision is not None:
+            _validate_train_precision(c.train_precision, probe)
+            if c.train_precision != "fp32_simt" and output_dim > 256:
+                raise ValueError(
+                    f"train_precision={c.train_precision!r} with output_dim={output_dim}: the node decoder ends in a LayerNorm over "
+                    "output_dim columns, and a LayerNorm'd row must stay in one tensor-core chain of at most 256 columns; use "
+                    "train_precision='fp32_simt'")  # fmt: skip
+        self.train_precision = c.train_precision
+        self.use_checkpointing = c.use_checkpointing
         # per-region state: graphs are cached like the reference's builder caches them (same list object -> same graphs)
-        self.__dict__["_regions"] = OrderedDict()  # id(lat_lons) -> (lat_lons, _RegionGraphs, _Engine)
+        self.__dict__["_regions"] = OrderedDict()  # id(lat_lons) -> (lat_lons, _RegionGraphs, engines)
+        self.__dict__["_active"] = None  # (graphs, engines) of the region of the current training forward
 
     # ---- the plan's view of the parameters -------------------------------------------------------------------------------
     _RENAME = (
@@ -174,14 +194,14 @@ class RegionalForecaster(nn.Module):
         ("node_decoder.", "decoder.node_decoder."),
     )
 
-    def _named(self, region: _RegionGraphs, device):
+    def _plan_named(self, region: _RegionGraphs):
         out = []
         for k, v in self.state_dict(keep_vars=True).items():
             if k == "h3_embeddings":  # the region's rows of the global table (:243); re-gathered only when the table changed
                 key = (v.data_ptr(), v._version, str(v.device))
                 if getattr(region, "_h3_key", None) != key:
-                    idx = torch.from_numpy(region.h3_indices).to(v.device)
-                    region._h3_rows, region._h3_key = v.detach()[idx].contiguous(), key
+                    region.h3_idx = torch.from_numpy(region.h3_indices).to(v.device)
+                    region._h3_rows, region._h3_key = v.detach()[region.h3_idx].contiguous(), key
                 out.append(("encoder.h3_nodes", region._h3_rows))
                 continue
             for a, b in self._RENAME:
@@ -190,22 +210,67 @@ class RegionalForecaster(nn.Module):
                     break
         return out
 
+    # ---- what _TrainFn asks of its wrapper, for the region of the current training forward -------------------------------
+    def _named(self):
+        return self._plan_named(self._active[0])
+
+    def _out_shape(self, batch):
+        return (batch, self._active[0].n_obs, self.output_dim)
+
+    def _training_engine(self):
+        """The region's training engine of precision `train_precision`: the bounded-memory step (a training-only plan) when
+        use_checkpointing is set, else the taped step; switching closes the region's other training plan (see
+        _Wrapper._training_engine)."""
+        region, engines = self._active
+
+        def make(bounded):
+            return _new_engine(engines["infer"].dims, self.train_precision, [region.upload], train_only=bounded)
+
+        eng = _switch_training_engine(engines, bool(self.use_checkpointing), make)
+        self.__dict__["_train_engine"] = eng
+        return eng
+
+    def _grad_bindings(self):
+        """The plan's parameters; `encoder.h3_nodes` (the region's rows of h3_embeddings) differentiates the table: the rows'
+        gradients go to the region's cells (unique, so a copy), every other row is zero.  The nudging layer is not bound: its
+        parameters are differentiated by torch."""
+        named = self._named()
+        table, idx = self.h3_embeddings, self._active[0].h3_idx
+
+        def to_table(g):
+            full = g.new_zeros(table.shape)
+            full[idx] = g
+            return full
+
+        return [(k, v, table, to_table) if k == "encoder.h3_nodes" else (k, v, v, None) for k, v in named]
+
+    multi_step = _Wrapper.multi_step
+
     def _region(self, lat_lons):
+        """The region's graphs and engines ({"infer": inference, False: taped step, True: bounded step}), built on first use.
+        Least recently used regions beyond _MAX_PLANS are dropped with their plans, except a region one of whose tapes a
+        backward still needs: the cache then holds more regions until those tapes are consumed or dropped, and shrinks back
+        at a later forward."""
         key = id(lat_lons)
         hit = self._regions.get(key)
         if hit is not None and hit[0] is lat_lons:
             self._regions.move_to_end(key)
-            return hit[1], hit[2]
-        g = _RegionGraphs(self.graph_builder, lat_lons)
-        dims = dict(self._base_dims, n_in=g.n_obs, n_out=g.n_obs, n_mesh=g.n_mesh, n_lat_edges=g.n_lat_edges, n_dec_edges=g.n_obs)
-        eng = _Engine(dims, self.config.precision)
-        eng.graph_uploaders.append(g.upload)
-        self._regions[key] = (lat_lons, g, eng)
-        while len(self._regions) > self._MAX_PLANS:
-            _, (_, _, old) = self._regions.popitem(last=False)
-            if old.plan is not None:
-                old.plan.close()
-        return g, eng
+            g, engines = hit[1], hit[2]
+        else:
+            g = _RegionGraphs(self.graph_builder, lat_lons)
+            dims = dict(self._base_dims, n_in=g.n_obs, n_out=g.n_obs, n_mesh=g.n_mesh, n_lat_edges=g.n_lat_edges, n_dec_edges=g.n_obs)
+            engines = {"infer": _new_engine(dims, self.config.precision, [g.upload])}
+            self._regions[key] = (lat_lons, g, engines)
+        for k in list(self._regions):
+            if len(self._regions) <= self._MAX_PLANS:
+                break
+            if k == key or any(_pending_tape(e) for e in self._regions[k][2].values()):
+                continue
+            for e in self._regions.pop(k)[2].values():
+                if e.plan is not None:
+                    e.plan.close()
+                    e.plan = None
+        return g, engines
 
     def forward(self, features: torch.Tensor, lat_lons: list, global_context: Optional[torch.Tensor] = None) -> torch.Tensor:
         if features.device.type != "cuda":
@@ -215,17 +280,25 @@ class RegionalForecaster(nn.Module):
             raise ValueError(f"features has {N} rows per sample but lat_lons has {len(lat_lons)} coordinates")
         if features.shape[-1] < self.output_dim:
             raise RuntimeError(f"features needs at least output_dim ({self.output_dim}) channels for the residual add (:288)")
-        if _wants_grad(self, features):
-            # (the forecaster's backward, csrc/gw_train.cu, is not wired to this module: fail instead of returning a tensor
-            # that silently carries no graph)
-            raise NotImplementedError("RegionalForecaster: the training step is not built; call under torch.no_grad() or in eval() mode")
-        region, eng = self._region(lat_lons)
-        named = self._named(region, features.device)
-        plan = eng.ensure(features.device, B, named)
-        f = features.detach().to(torch.float32).contiguous()
-        out = torch.empty((B, N, self.output_dim), dtype=torch.float32, device=f.device)
-        plan.forward(f, out)  # encoder -> processor -> decoder -> + features[..., :output_dim]
-        _maybe_check(plan)
+        train = _wants_grad(self, features)
+        if train and self.train_precision is None:
+            # (fail instead of returning a tensor that silently carries no graph)
+            raise NotImplementedError("RegionalForecaster: training needs RegionalForecasterConfig.train_precision ('fp32_simt', 'fp32' "
+                                      "or 'bf16'); call under torch.no_grad() or in eval() mode for inference")
+        region, engines = self._region(lat_lons)
+        if train:
+            self.__dict__["_active"] = (region, engines)
+            try:
+                bindings = self._grad_bindings()
+                out = _TrainFn.apply(self, features, None, bindings, *[q for _, _, q, _ in bindings])
+            finally:
+                self.__dict__["_active"] = None
+        else:
+            plan = engines["infer"].ensure(features.device, B, self._plan_named(region))
+            f = features.detach().to(torch.float32).contiguous()
+            out = torch.empty((B, N, self.output_dim), dtype=torch.float32, device=f.device)
+            plan.forward(f, out)  # encoder -> processor -> decoder -> + features[..., :output_dim]
+            _maybe_check(plan)
         if self.nudging is not None and global_context is not None:
             out = self.nudging(out, global_context.to(out.device), lat_lons)
         return out

@@ -1,9 +1,10 @@
-"""Times one training step (forward with tape + NormalizedMSELoss + backward + SGD update) of GraphWeatherForecaster, GraphCast or
-GraphWeatherAssimilator.
-    python tools/train_step_bench.py [--model forecaster|graphcast|assimilator] [--grid 0.25deg|1deg|2deg|5deg|10deg] [--batch B]
-                                     [--steps K] [--train-precision fp32_simt|fp32|bf16] [--feature-dim F] [--aux-dim A]
+"""Times one training step (forward with tape + NormalizedMSELoss + backward + SGD update) of GraphWeatherForecaster, GraphCast,
+GraphWeatherAssimilator or RegionalForecaster.
+    python tools/train_step_bench.py [--model forecaster|graphcast|assimilator|regional] [--grid 0.25deg|1deg|2deg|5deg|10deg]
+                                     [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16] [--feature-dim F] [--aux-dim A]
                                      [--num-blocks NB] [--width W] [--constraint-type none|additive|multiplicative|softmax]
                                      [--use-checkpointing] [--fit-batch] [--n-obs N] [--rollout K [--compare-plain]]
+                                     [--extent DEG] [--max-points N] [--moving-region]
 The model defaults to the README's 78 + 24 features, 9 blocks, 256-wide.  --model graphcast: GraphCast(input_dim = output_dim =
 --feature-dim, hidden_dim = --width or 256); its bounded step is selected by --use-checkpointing (the same step
 GraphCastConfig.balanced_checkpointing / full_checkpointing select).  --model assimilator: GraphWeatherAssimilator(output_lat_lons =
@@ -25,6 +26,11 @@ previous forecast (the forecaster's auxiliary columns stay those of the first in
 SGD update; "rollout" reports gw_tape_bytes of each of the K tapes (what each forward keeps until the backward), and
 train_peak_bytes covers all of them.  --compare-plain (with --rollout 1) also times the window's one-step step and the plain step
 alternately, step by step, and reports both medians.
+--model regional: RegionalForecaster (--feature-dim + --aux-dim features, --num-blocks, --width; the loss is torch's MSELoss) on
+synthetic regions shaped like the reference's RegionalDataset samples: a square box of side --extent degrees at a seeded random
+centre on the 0.25-degree grid, --max-points of its points drawn without replacement (--grid is not used).  One box is reused for
+every step, or with --moving-region a new box is drawn for every step, as the dataset does: that step also builds the region's
+graphs on the host, creates its plans and uploads the graphs and weights, so the difference of the two is the per-region set-up cost.
 With --constraint-type the step includes PhysicalConstraintLayer; the constraint backward
 (gw_constraint_backward, no timing tag of the plan) is also timed on its own with CUDA events around it, on the step's shapes."""
 import argparse
@@ -79,7 +85,7 @@ def constraint_backward_time(model, x, F, reps=20):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="forecaster", choices=["forecaster", "graphcast", "assimilator"])
+    ap.add_argument("--model", default="forecaster", choices=["forecaster", "graphcast", "assimilator", "regional"])
     ap.add_argument("--grid", default="1deg", choices=["0.25deg", "1deg", "2deg", "5deg", "10deg"])
     ap.add_argument("--batch", type=int, default=2)
     ap.add_argument("--steps", type=int, default=5)
@@ -94,7 +100,12 @@ def main():
     ap.add_argument("--n-obs", type=int, default=2660, help="observations per step (--model assimilator)")
     ap.add_argument("--rollout", type=int, default=0, help="K: one step is K forwards inside model.multi_step() and one backward")
     ap.add_argument("--compare-plain", action="store_true", help="with --rollout 1: alternate the window's step with the plain one")
+    ap.add_argument("--extent", type=float, default=20.0, help="side of the square region in degrees (--model regional)")
+    ap.add_argument("--max-points", type=int, default=2000, help="points per region (--model regional)")
+    ap.add_argument("--moving-region", action="store_true", help="a new region for every step (--model regional)")
     a = ap.parse_args()
+    if a.model == "regional" and (a.rollout or a.fit_batch):
+        ap.error("--model regional: no --rollout or --fit-batch")
     if a.model != "forecaster" and a.constraint_type != "none":
         ap.error("--constraint-type applies to --model forecaster")
     if a.rollout and a.model == "assimilator":
@@ -104,11 +115,12 @@ def main():
     import __graft_entry__ as ge
 
     ge.build()
+    import numpy as np
+
     from graph_weather_b200 import GraphCast, GraphWeatherAssimilator, GraphWeatherForecaster, NormalizedMSELoss
+    from graph_weather_b200.regional import RegionalForecasterConfig
 
     if a.grid == "0.25deg":
-        import numpy as np
-
         ll = [(float(lat), float(lon)) for lat in np.linspace(-90.0, 90.0, 721) for lon in np.arange(0.0, 360.0, 0.25)]
     else:
         step = {"1deg": 1, "2deg": 2, "5deg": 5, "10deg": 10}[a.grid]
@@ -127,6 +139,28 @@ def main():
         model = GraphWeatherAssimilator(output_lat_lons=ll, train_precision=a.train_precision, use_checkpointing=a.use_checkpointing,
                                         **{k: v for k, v in dims.items() if k != "n_obs"}).cuda().train()  # fmt: skip
         n_in, f_in = a.n_obs, 2
+    elif a.model == "regional":
+        dims = dict(feature_dim=F, aux_dim=a.aux_dim, num_blocks=a.num_blocks, extent=a.extent, max_points=a.max_points,
+                    moving_region=a.moving_region)  # fmt: skip
+        if a.width is not None:
+            dims.update(node_dim=a.width, edge_dim=a.width, hidden_dim_processor_node=a.width, hidden_dim_processor_edge=a.width,
+                        hidden_dim_decoder=a.width)  # fmt: skip
+        cfg = {k: v for k, v in dims.items() if k not in ("extent", "max_points", "moving_region")}
+        model = RegionalForecasterConfig(train_precision=a.train_precision, use_checkpointing=a.use_checkpointing, **cfg).build().cuda().train()
+        box_rng = np.random.default_rng(0)
+        lat_g, lon_g = np.arange(-90.0, 90.001, 0.25), np.arange(0.0, 360.0, 0.25)
+
+        def box():
+            """RegionalDataset._sample_box on the 0.25-degree grid: a new list of (lat, lon)."""
+            half = a.extent / 2.0
+            lat_c, lon_c = box_rng.uniform(lat_g.min() + half, lat_g.max() - half), box_rng.uniform(lon_g.min() + half, lon_g.max() - half)
+            glat, glon = np.meshgrid(lat_g[np.abs(lat_g - lat_c) <= half], lon_g[np.abs(lon_g - lon_c) <= half], indexing="ij")
+            pick = box_rng.choice(glat.size, size=min(a.max_points, glat.size), replace=False)
+            return [(float(p), float(q)) for p, q in zip(glat.ravel()[pick], glon.ravel()[pick])]
+
+        fixed = box()
+        ll = fixed
+        n_in, f_in = len(fixed), F + a.aux_dim
     else:
         dims = dict(feature_dim=F, aux_dim=a.aux_dim, num_blocks=a.num_blocks)
         if a.width is not None:
@@ -135,14 +169,14 @@ def main():
         model = GraphWeatherForecaster(ll, train_precision=a.train_precision, constraint_type=a.constraint_type,
                                        use_checkpointing=a.use_checkpointing, **dims).cuda().train()  # fmt: skip
         n_in, f_in = len(ll), F + a.aux_dim
-    crit = NormalizedMSELoss([1.0] * F, ll, normalize=True)
+    crit = torch.nn.functional.mse_loss if a.model == "regional" else NormalizedMSELoss([1.0] * F, ll, normalize=True)
     opt = torch.optim.SGD(model.parameters(), lr=1e-3)
     tape_bytes = []  # gw_tape_bytes of every tape of the last --rollout step, read before its backward
 
     def measure(batch, steps):
         """(ms/step, losses, torch peak bytes, train_peak_bytes, plan device_bytes, step function, inputs) of `steps` timed steps."""
         x = torch.randn(batch, n_in, f_in, device="cuda")
-        y = torch.randn(batch, len(ll), F, device="cuda")
+        y = torch.randn(batch, n_in if a.model == "regional" else len(ll), F, device="cuda")
         g = torch.Generator(device="cuda").manual_seed(1)
 
         def obs():  # a new observation set: (lat, lon, height)
@@ -160,6 +194,8 @@ def main():
                         if t + 1 < rollout:
                             inp = torch.cat([out, x[..., F:]], -1) if f_in > F else out
                 tape_bytes[:] = [t.bytes() for t in model._train_engine.plan.live_tapes()]
+            elif a.model == "regional":  # (every box has max_points points: the inputs keep their shapes)
+                loss = crit(model(x, box() if a.moving_region else fixed), y)
             else:
                 loss = crit(model(x, obs()) if a.model == "assimilator" else model(x), y)
             loss.backward()
@@ -223,7 +259,7 @@ def main():
     phases = {k: round(v[1], 3) for k, v in tags.items() if k.startswith("train_") or k == "const"}
     plan.status()
     cbwd = constraint_backward_time(model, x, F) if a.constraint_type != "none" else None
-    print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "model": a.model, "train_precision": a.train_precision, "grid": a.grid, "batch": a.batch,
+    print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "model": a.model, "train_precision": a.train_precision, "grid": None if a.model == "regional" else a.grid, "batch": a.batch,
                       "use_checkpointing": a.use_checkpointing, "rollout": rollout, "train_peak_gib": round(train_peak / 2**30, 3),
                       "plan_device_gib": round(plan_bytes / 2**30, 3),
                       "dims": dims, "constraint_type": a.constraint_type, "constraint_backward": cbwd,
