@@ -2,6 +2,8 @@
 // create / destroy, graph and weight upload, the forward entry points (gw_forward.cu), output peers, status, debug, timing.
 #include "gw_plan.h"
 
+#include <memory>
+
 namespace gw {
 
 static thread_local std::string g_err;
@@ -22,6 +24,14 @@ int check_ready(gw_plan* p, int batch, int need) {
 }
 
 }  // namespace gw
+
+// the training state first (its live tapes are released and left dead), then the host resources; the device buffers go with
+// their members
+gw_plan::~gw_plan() {
+  gw::train_destroy(this);
+  if (tc_status_host) cudaFreeHost(tc_status_host);
+  for (cudaEvent_t e : ev_pool) cudaEventDestroy(e);
+}
 
 // ===================================================================================================================
 // C ABI
@@ -99,21 +109,10 @@ static int plan_create(const gw_dims* dims, gw_plan** out_plan, bool train_only)
     gw::set_error("no CUDA device available (libgwb200 has no CPU fallback)");
     return 1;
   }
-  gw_plan* p = new gw_plan();
+  std::unique_ptr<gw_plan> p(new gw_plan());  // a failure below frees the plan and whatever it already holds
   p->d = d;
   p->train_only = train_only;
-  // every failure after this point releases the plan and whatever it already holds
-#define GW_CUDA_P(expr)                                                          \
-  do {                                                                           \
-    cudaError_t _e = (expr);                                                     \
-    if (_e != cudaSuccess) {                                                     \
-      std::string _m = std::string(#expr) + ": " + cudaGetErrorString(_e);       \
-      gw_plan_destroy(p);                                                        \
-      gw::set_error(_m);                                                         \
-      return 1;                                                                  \
-    }                                                                            \
-  } while (0)
-  GW_CUDA_P(cudaGetDevice(&p->device));
+  GW_CUDA(cudaGetDevice(&p->device));
   const size_t Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, Hn = d.hidden_node;
   const size_t max_hid = std::max({Dn, De, He, Hn, (size_t)d.hidden_dec, (size_t)d.out_dim});
   const size_t max_rows = std::max({(size_t)d.n_in, (size_t)d.n_out, (size_t)d.n_mesh, (size_t)d.n_lat_edges, (size_t)d.n_dec_edges});
@@ -144,21 +143,15 @@ static int plan_create(const gw_dims* dims, gw_plan** out_plan, bool train_only)
   rc |= p->dec_src.alloc(d.n_dec_edges) | p->dec_ptr.alloc(d.n_out + 1) | p->dec_attr.alloc((size_t)d.n_dec_edges * 2);
   rc |= p->dec_dst.alloc(d.n_dec_edges) | p->deg_stats.alloc(2) | p->enc_deg.alloc(2) | p->bounds.alloc(gw::SL_COUNT);
   rc |= p->zeros_h3.alloc((size_t)d.n_mesh * d.in_dim);
-  if (!train_only) rc |= alloc_inference_scratch(p, chunk);
-  if (rc) {
-    std::string keep = gw::g_err;
-    gw_plan_destroy(p);
-    gw::set_error(keep);
-    return 1;
-  }
-  GW_CUDA_P(cudaMemset(p->zeros_h3.p, 0, p->zeros_h3.bytes()));
-  GW_CUDA_P(cudaMemset(p->bounds.p, 0, p->bounds.bytes()));
-  GW_CUDA_P(cudaHostAlloc((void**)&p->tc_status_host, 64 * sizeof(int32_t), cudaHostAllocMapped));
+  if (!train_only) rc |= alloc_inference_scratch(p.get(), chunk);
+  GW_TRY(rc);
+  GW_CUDA(cudaMemset(p->zeros_h3.p, 0, p->zeros_h3.bytes()));
+  GW_CUDA(cudaMemset(p->bounds.p, 0, p->bounds.bytes()));
+  GW_CUDA(cudaHostAlloc((void**)&p->tc_status_host, 64 * sizeof(int32_t), cudaHostAllocMapped));
   std::memset(p->tc_status_host, 0, 64 * sizeof(int32_t));
-  GW_CUDA_P(cudaHostGetDevicePointer((void**)&p->tc_status_dev, p->tc_status_host, 0));
-#undef GW_CUDA_P
+  GW_CUDA(cudaHostGetDevicePointer((void**)&p->tc_status_dev, p->tc_status_host, 0));
   p->n_in_cur = d.n_in;
-  *out_plan = p;
+  *out_plan = p.release();
   return 0;
 }
 
@@ -166,20 +159,6 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan) { return plan_create
 int gw_plan_create_train(const gw_dims* dims, gw_plan** out_plan) { return plan_create(dims, out_plan, true); }
 
 int gw_plan_destroy(gw_plan* p) {
-  if (!p) return 0;
-  for (DevBuf<int32_t>* b : {&p->enc_mesh, &p->enc_perm, &p->enc_ptr, &p->lat_src, &p->lat_dst, &p->lat_ptr, &p->dec_src, &p->dec_ptr})
-    b->release();
-  for (DevBuf<float>* b : {&p->enc_attr, &p->lat_attr, &p->dec_attr, &p->wbuf, &p->zeros_h3, &p->e_enc, &p->xm0, &p->C1_enc,
-                           &p->e_lat, &p->e_dec, &p->E1_dec, &p->S_dec, &p->tmpP, &p->bufA, &p->bufB, &p->rows_n, &p->rows_e, &p->xbuf0,
-                           &p->xbuf1, &p->ebuf0, &p->ebuf1, &p->P})
-    b->release();
-  p->tc_packed.release(), p->tc_absmax.release(), p->agg_mesh.release(), p->agg_grid.release();
-  p->bounds.release(), p->dec_dst.release(), p->seg_carry.release(), p->deg_stats.release(), p->enc_deg.release();
-  p->h3_frames.release(), p->h3_lat.release(), p->h3_lng.release(), p->h3_cell_of.release(), p->h3_slot.release(), p->obs_ws.release();
-  p->enc_chunk_seg.release(), p->enc_chunk_j0.release(), p->enc_seg_chunk0.release(), p->enc_partial.release();
-  gw::train_destroy(p);
-  if (p->tc_status_host) cudaFreeHost(p->tc_status_host);
-  for (cudaEvent_t e : p->ev_pool) cudaEventDestroy(e);
   delete p;
   return 0;
 }

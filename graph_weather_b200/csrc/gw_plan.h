@@ -13,6 +13,7 @@
 #include <map>
 #include <set>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/gw_b200.h"
@@ -54,15 +55,25 @@ struct Mlp {  // views into the plan-owned weight buffer; Linear l: W[l] [out_l,
 };
 
 template <class T>
-struct DevBuf {
+struct DevBuf {  // owns its allocation: freed by the destructor, moved but never copied
   T* p = nullptr;
   size_t n = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), n(std::exchange(o.n, 0)) {}
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) release(), p = std::exchange(o.p, nullptr), n = std::exchange(o.n, 0);
+    return *this;
+  }
+  ~DevBuf() { release(); }
   int alloc(size_t count) {
     release();
     n = count;
     if (count == 0) return 0;
     cudaError_t e = cudaMalloc(&p, count * sizeof(T));
     if (e != cudaSuccess) {
+      cudaGetLastError();  // reported here: clear the runtime's record of it, or the next CUDA call's error check reports it again
       set_error(std::string("cudaMalloc(") + std::to_string(count * sizeof(T)) + " B): " + cudaGetErrorString(e));
       p = nullptr;
       n = 0;
@@ -85,6 +96,7 @@ struct TrainState;  // gw_train.cu
 using namespace gw;
 
 struct gw_plan {
+  ~gw_plan();  // gw_api.cu
   gw::TrainState* train = nullptr;  // training step state (gw_train.cu), created on first use, torn down by train_destroy
   bool train_only = false;          // gw_plan_create_train: graphs, weights and the bounded-memory (chunked) training step only
   int train_chunk_pts = 0;          // GW_B200_TRAIN_CHUNK: points per chunk of that step (0: from the shapes, gw_train.cu)
@@ -288,7 +300,7 @@ int encoder_degree(gw_plan* p, cudaStream_t st);
 enum { NEED_ENC = 1, NEED_PROC = 2, NEED_DEC = 4, NEED_INFER = 8 };
 int check_ready(gw_plan* p, int batch, int need);
 
-// gw_train.cu: releases the plan's training state for gw_plan_destroy; live tapes lose their memory and stay as dead handles
+// gw_train.cu: releases the plan's training state for ~gw_plan; live tapes lose their memory and stay as dead handles
 void train_destroy(gw_plan* p);
 
 }  // namespace gw

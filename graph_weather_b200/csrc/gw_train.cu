@@ -425,7 +425,6 @@ static int train_prepare(gw_plan* p, TrainState* T, int batch, cudaStream_t st) 
     }
     if (is_tc(p)) {  // the weight images of these weights are packed on first use (train_image)
       if (T->images_of != p->wbuf.p) {
-        for (auto& kv : T->images) kv.second.img.release(), kv.second.amax.release();
         T->images.clear();
         T->images_of = p->wbuf.p;
       }
@@ -921,12 +920,6 @@ void gw::train_destroy(gw_plan* p) {
     gw::tape_release(T, k, T->st);
     k->plan = nullptr;
   }
-  T->tapes.clear();
-  T->wT.release(), T->gbuf.release(), T->lat_perm_src.release(), T->lat_ptr_src.release();
-  T->dec_perm_src.release(), T->dec_ptr_src.release(), T->iota.release(), T->sort_ws.release();
-  T->enc_slot_sorted.release(), T->dec_cperm.release(), T->dec_cptr.release();
-  T->bslots.release(), T->wg_ws.release();
-  for (auto& kv : T->images) kv.second.img.release(), kv.second.amax.release();
   delete T;
   p->train = nullptr;
 }
