@@ -4,6 +4,7 @@ RuntimeError is raised."""
 
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import os
 import re
@@ -124,10 +125,6 @@ def _check(rc):
         raise RuntimeError("libgwb200: " + load().gw_last_error().decode())
 
 
-def _stream(device):
-    return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-
-
 def _ptr(t, dtype, device):
     if t.dtype != dtype or not t.is_contiguous() or t.device != device:
         raise RuntimeError(f"expected a contiguous {dtype} tensor on {device}, got {t.dtype} on {t.device}")
@@ -144,7 +141,8 @@ def launch_count_reset() -> None:
 
 class Plan:
     """Owns one gw_plan on one CUDA device.  train_only: a training-only plan (gw_plan_create_train), whose training step is the
-    bounded-memory one and which runs no inference forward."""
+    bounded-memory one and which runs no inference forward.  Every call runs on the caller's current stream, after the plan's
+    previous call (`_on_stream`): one plan may be used from several streams."""
 
     def __init__(self, device, train_only: bool = False, **dims):
         self.lib = load()
@@ -161,6 +159,24 @@ class Plan:
             _check(create(ctypes.byref(self.dims), ctypes.byref(self.handle)))
         self._keep = []
         self._tapes = weakref.WeakSet()
+        self._last_stream = None  # the stream of the last call that passed one, and an event behind that call's work
+        self._last_done = torch.cuda.Event()
+
+    @contextlib.contextmanager
+    def _on_stream(self):
+        """The current stream of the plan's device, as the call's `stream` argument, ordered after the plan's previous call.  Calls
+        on one plan share its scratch, so a call from another stream than the previous one first waits (on the device) for that
+        call's work; every call that passes a stream records the event behind its own work."""
+        d = self.device
+        s = torch.cuda.current_stream(d)
+        if self._last_stream is not None and self._last_stream != s.cuda_stream:
+            s.wait_event(self._last_done)
+        try:
+            with torch.cuda.device(d):
+                yield ctypes.c_void_p(s.cuda_stream)
+        finally:
+            self._last_done.record(s)
+            self._last_stream = s.cuda_stream
 
     def close(self):
         if getattr(self, "handle", None) is not None and self.handle.value:
@@ -188,9 +204,9 @@ class Plan:
         d = self.device
         m, pm, pt = (self._dev(a, torch.int32) for a in (enc_mesh, perm, ptr))
         at = self._dev(attr, torch.float32)
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             _check(self.lib.gw_plan_set_encoder_graph(self.handle, int(m.numel()), _ptr(m, torch.int32, d), _ptr(pm, torch.int32, d),
-                                                      _ptr(pt, torch.int32, d), _ptr(at, torch.float32, d), _stream(d)))  # fmt: skip
+                                                      _ptr(pt, torch.int32, d), _ptr(at, torch.float32, d), st))  # fmt: skip
             torch.cuda.current_stream(d).synchronize()  # the temporaries above are freed on return
 
     def set_h3_tables(self, tab: dict):
@@ -201,36 +217,36 @@ class Plan:
         co = self._dev(tab["cell_of"], torch.int32)
         slot = self._dev(H - 1 - tab["rank"], torch.int32)
         la, ln = self._dev(tab["cell_lat"], torch.float64), self._dev(tab["cell_lng"], torch.float64)
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             _check(self.lib.gw_plan_set_h3_tables(self.handle, int(tab["res"]), H, int(tab["lattice_n"]), _ptr(fr, torch.float64, d),
                                                   _ptr(co, torch.int32, d), _ptr(slot, torch.int32, d), _ptr(la, torch.float64, d),
                                                   _ptr(ln, torch.float64, d), float(tab["scale"]), float(tab["rot_cos"]), float(tab["rot_sin"]),
-                                                  _stream(d)))  # fmt: skip
+                                                  st))  # fmt: skip
             torch.cuda.current_stream(d).synchronize()  # the temporaries above are freed on return
 
     def build_obs_graph(self, lat_lon_heights):
         """[n_obs, 3] float32 (lat deg, lon deg, height) on the plan's device -> the encoder graph, built on the device."""
         d = self.device
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             _check(self.lib.gw_plan_build_obs_graph(self.handle, _ptr(lat_lon_heights, torch.float32, d), int(lat_lon_heights.shape[0]),
-                                                    _stream(d)))  # fmt: skip
+                                                    st))  # fmt: skip
 
     def set_latent_graph(self, src, dst, ptr, attr):
         d = self.device
         s, t, p = (self._dev(a, torch.int32) for a in (src, dst, ptr))
         at = self._dev(attr, torch.float32)
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             _check(self.lib.gw_plan_set_latent_graph(self.handle, _ptr(s, torch.int32, d), _ptr(t, torch.int32, d),
-                                                     _ptr(p, torch.int32, d), _ptr(at, torch.float32, d), _stream(d)))  # fmt: skip
+                                                     _ptr(p, torch.int32, d), _ptr(at, torch.float32, d), st))  # fmt: skip
             torch.cuda.current_stream(d).synchronize()
 
     def set_decoder_graph(self, src, ptr, attr):
         d = self.device
         s, p = (self._dev(a, torch.int32) for a in (src, ptr))
         at = self._dev(attr, torch.float32)
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             _check(self.lib.gw_plan_set_decoder_graph(self.handle, _ptr(s, torch.int32, d), _ptr(p, torch.int32, d),
-                                                      _ptr(at, torch.float32, d), _stream(d)))  # fmt: skip
+                                                      _ptr(at, torch.float32, d), st))  # fmt: skip
             torch.cuda.current_stream(d).synchronize()
 
     def set_weights(self, named_tensors):
@@ -241,50 +257,50 @@ class Plan:
         for i, (k, v) in enumerate(items):
             rows, cols = (v.shape[0], v.shape[1]) if v.dim() == 2 else (v.numel(), 1)
             arr[i] = GwParam(k.encode(), v.data_ptr(), rows, cols)
-        with torch.cuda.device(d):
-            _check(self.lib.gw_plan_set_weights(self.handle, arr, len(items), _stream(d)))
+        with self._on_stream() as st:
+            _check(self.lib.gw_plan_set_weights(self.handle, arr, len(items), st))
             torch.cuda.current_stream(d).synchronize()
 
     def forward(self, features, out, out_ld=None):
         """out: [batch, n_out, out_dim] contiguous, or (out_ld given) the first out_dim columns of rows `out_ld` floats apart."""
         d = self.device
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             if out_ld is None:
                 _check(self.lib.gw_forward(self.handle, _ptr(features, torch.float32, d), _ptr(out, torch.float32, d),
-                                           int(features.shape[0]), _stream(d)))  # fmt: skip
+                                           int(features.shape[0]), st))  # fmt: skip
             else:
                 if out.dtype != torch.float32 or out.device != d:
                     raise RuntimeError("strided forward needs a float32 tensor on the plan's device")
                 _check(self.lib.gw_forward_strided(self.handle, _ptr(features, torch.float32, d), ctypes.c_void_p(out.data_ptr()),
-                                                   int(out_ld), int(features.shape[0]), _stream(d)))  # fmt: skip
+                                                   int(out_ld), int(features.shape[0]), st))  # fmt: skip
 
     def encoder_forward(self, features, x_out):
         d = self.device
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             _check(self.lib.gw_encoder_forward(self.handle, _ptr(features, torch.float32, d), _ptr(x_out, torch.float32, d),
-                                               int(features.shape[0]), _stream(d)))  # fmt: skip
+                                               int(features.shape[0]), st))  # fmt: skip
 
     def processor_forward(self, x_in, x_out, batch):
         d = self.device
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             _check(self.lib.gw_processor_forward(self.handle, _ptr(x_in, torch.float32, d), _ptr(x_out, torch.float32, d),
-                                                 int(batch), _stream(d)))  # fmt: skip
+                                                 int(batch), st))  # fmt: skip
 
     def processor_forward_graph(self, x_in, x_out, edge_attr, src, dst, ptr):
         d = self.device
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             _check(self.lib.gw_processor_forward_graph(
                 self.handle, _ptr(x_in, torch.float32, d), _ptr(x_out, torch.float32, d), _ptr(edge_attr, torch.float32, d),
                 int(x_in.shape[0]), int(src.numel()), _ptr(src, torch.int32, d), _ptr(dst, torch.int32, d), _ptr(ptr, torch.int32, d),
-                _stream(d)))  # fmt: skip
+                st))  # fmt: skip
 
     def decoder_forward(self, x_in, start, out, batch):
         d = self.device
-        with torch.cuda.device(d):
+        with self._on_stream() as st:
             sp = _ptr(start, torch.float32, d) if start is not None else _vp()
             ld = int(start.shape[-1]) if start is not None else 0
             _check(self.lib.gw_decoder_forward(self.handle, _ptr(x_in, torch.float32, d), sp, ld, _ptr(out, torch.float32, d),
-                                               int(batch), _stream(d)))  # fmt: skip
+                                               int(batch), st))  # fmt: skip
 
     def _grad_table(self, named_grads):
         items = list(named_grads)
@@ -312,8 +328,8 @@ class Plan:
     def status(self) -> int:
         """Synchronising read of the device status word (0 = ok); raises on a non-zero status."""
         v = _i32(0)
-        with torch.cuda.device(self.device):
-            _check(self.lib.gw_plan_status(self.handle, ctypes.byref(v), _stream(self.device)))
+        with self._on_stream() as st:
+            _check(self.lib.gw_plan_status(self.handle, ctypes.byref(v), st))
         if v.value:
             raise RuntimeError(f"libgwb200 device status {v.value}: " + ("an operand left the fp16 range despite range scaling in precision 'fp32' (use 'fp32_simt'); " if v.value & 1 else "")
                                + ("pipeline timeout; " if v.value & 2 else "") + ("shared memory misaligned; " if v.value & 4 else "")
@@ -346,19 +362,20 @@ class Plan:
         """{tag: (launches, total_ms)} since the last read (synchronises the current stream)."""
         n = int(self.lib.gw_timing_num_tags())
         cnt, ms = (_i64 * n)(), (ctypes.c_double * n)()
-        with torch.cuda.device(self.device):
-            _check(self.lib.gw_timing_read(self.handle, cnt, ms, _stream(self.device)))
+        with self._on_stream() as st:
+            _check(self.lib.gw_timing_read(self.handle, cnt, ms, st))
         return {self.lib.gw_timing_tag_name(i).decode(): (int(cnt[i]), float(ms[i])) for i in range(n)}
 
     def latent_edge_features(self, out):
         d = self.device
-        with torch.cuda.device(d):
-            _check(self.lib.gw_latent_edge_features(self.handle, _ptr(out, torch.float32, d), _stream(d)))
+        with self._on_stream() as st:
+            _check(self.lib.gw_latent_edge_features(self.handle, _ptr(out, torch.float32, d), st))
 
 
 class Tape:
     """One gw_tape of a plan: what one training forward saves for its own backward.  It keeps its plan object referenced and is
-    destroyed (its memory released on the current stream) by `close()` or when it is garbage-collected.  Once its plan is
+    destroyed (its memory released on the current stream, ordered after the plan's previous call like every call of the plan) by
+    `close()` or when it is garbage-collected.  Once its plan is
     closed the tape is dead: its memory went with the plan, and a forward or backward on it raises."""
 
     def __init__(self, plan: Plan):
@@ -375,18 +392,18 @@ class Tape:
     def forward(self, features, out):
         """gw_train_forward_tape: the forward that keeps its activations on this tape (a second forward replaces the first's)."""
         d = self.plan.device
-        with torch.cuda.device(d):
+        with self.plan._on_stream() as st:
             _check(self.lib.gw_train_forward_tape(self._plan_handle(), self.handle, _ptr(features, torch.float32, d), _ptr(out, torch.float32, d),
-                                                  int(features.shape[0]), _stream(d)))  # fmt: skip
+                                                  int(features.shape[0]), st))  # fmt: skip
 
     def backward(self, grad_out, grad_features, named_grads):
         """gw_train_backward_tape: grad_out [B, N, out] -> gradients written into `named_grads` (reference parameter name -> tensor
         shaped like the parameter) and, if given, the gradient of the features.  One backward per forward: it consumes the tape."""
         d = self.plan.device
         arr, n = self.plan._grad_table(named_grads)
-        with torch.cuda.device(d):
+        with self.plan._on_stream() as st:
             gf = _ptr(grad_features, torch.float32, d) if grad_features is not None else _vp()
-            _check(self.lib.gw_train_backward_tape(self._plan_handle(), self.handle, _ptr(grad_out, torch.float32, d), gf, arr, n, _stream(d)))
+            _check(self.lib.gw_train_backward_tape(self._plan_handle(), self.handle, _ptr(grad_out, torch.float32, d), gf, arr, n, st))
 
     def bytes(self) -> int:
         """gw_tape_bytes: what the tape holds now (between its forward and backward, the forward's saved tensors)."""
@@ -394,8 +411,8 @@ class Tape:
 
     def close(self):
         if getattr(self, "handle", None) is not None and self.handle.value:
-            with torch.cuda.device(self.plan.device):
-                self.lib.gw_tape_destroy(self.handle, _stream(self.plan.device))
+            with self.plan._on_stream() as st:
+                self.lib.gw_tape_destroy(self.handle, st)
             self.handle = _vp()
 
     def __del__(self):

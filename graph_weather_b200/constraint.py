@@ -83,7 +83,6 @@ class PhysicalConstraintLayer(nn.Module):
         self.upsampling_factor = upsampling_factor
         if upsampling_factor != 1:
             raise NotImplementedError("upsampling_factor != 1: GraphWeatherForecaster only ever uses 1 (forecast.py:166)")
-        self._ws = {}
 
     def _prepare(self, hr: torch.Tensor, lr: torch.Tensor):
         """The float32 rows the kernels read: hr contiguous, lr with unit column stride and rows of one stride."""
@@ -108,15 +107,13 @@ class PhysicalConstraintLayer(nn.Module):
         lib = _capi.load()
         B, N, C = hr.shape
         out = torch.empty_like(hr)
-        key = (str(hr.device), B, C)
-        if key not in self._ws:
-            self._ws = {key: torch.empty(int(lib.gw_constraint_workspace_bytes(B, C)), dtype=torch.uint8, device=hr.device)}
+        ws = torch.empty(int(lib.gw_constraint_workspace_bytes(B, C)), dtype=torch.uint8, device=hr.device)  # (per call: stream-ordered)
         with torch.cuda.device(hr.device):
             st = torch.cuda.current_stream().cuda_stream
             _capi._check(lib.gw_constraint_apply(
                 CONSTRAINT_TYPES[self.constraint_type], ctypes.c_void_p(hr.data_ptr()), ctypes.c_void_p(lr.data_ptr()), int(lr.stride(1)),
                 int(lr_channels), ctypes.c_void_p(src.data_ptr()), ctypes.c_void_p(out.data_ptr()), B, N, C, float(self.exp_factor),
-                ctypes.c_void_p(self._ws[key].data_ptr()), ctypes.c_void_p(st)))  # fmt: skip
+                ctypes.c_void_p(ws.data_ptr()), ctypes.c_void_p(st)))  # fmt: skip
         return out
 
     def _backward(self, dy, hr, lr, src, need_lr):

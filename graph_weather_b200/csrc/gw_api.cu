@@ -145,8 +145,16 @@ static int plan_create(const gw_dims* dims, gw_plan** out_plan, bool train_only)
   rc |= p->zeros_h3.alloc((size_t)d.n_mesh * d.in_dim);
   if (!train_only) rc |= alloc_inference_scratch(p.get(), chunk);
   GW_TRY(rc);
-  GW_CUDA(cudaMemset(p->zeros_h3.p, 0, p->zeros_h3.bytes()));
-  GW_CUDA(cudaMemset(p->bounds.p, 0, p->bounds.bytes()));
+  {  // zeroed on a private non-blocking stream and complete on return: the plan's first call may come from any stream, also one
+     // not ordered against the legacy default stream (cudaDeviceSynchronize would instead wait for whatever the caller queued there)
+    cudaStream_t zs = nullptr;
+    GW_CUDA(cudaStreamCreateWithFlags(&zs, cudaStreamNonBlocking));
+    cudaError_t e = cudaMemsetAsync(p->zeros_h3.p, 0, p->zeros_h3.bytes(), zs);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p->bounds.p, 0, p->bounds.bytes(), zs);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(zs);
+    cudaStreamDestroy(zs);
+    GW_CUDA(e);
+  }
   GW_CUDA(cudaHostAlloc((void**)&p->tc_status_host, 64 * sizeof(int32_t), cudaHostAllocMapped));
   std::memset(p->tc_status_host, 0, 64 * sizeof(int32_t));
   GW_CUDA(cudaHostGetDevicePointer((void**)&p->tc_status_dev, p->tc_status_host, 0));

@@ -619,6 +619,8 @@ static void apply_out_peers(gw_plan* p, TcChain& ch) {
 // e' rows of the decoder block are only materialised by the CUDA-core path and by the unfused fallback: allocated on demand
 static int ensure_rows_e(gw_plan* p, size_t floats) {
   if (p->rows_e.n >= floats) return 0;
+  // the buffer being replaced may still be read by work of this plan queued on any stream (the caller orders its calls, not
+  // their completion): wait for all of it before the buffer is freed
   GW_CUDA(cudaDeviceSynchronize());
   return p->rows_e.alloc(floats);
 }

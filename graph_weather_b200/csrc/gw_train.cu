@@ -348,7 +348,8 @@ static int build_chunks(gw_plan* p, TrainState* T, int batch) {
     for (int s = 0; s < H; ++s)
       for (int j = eptr[s]; j < eptr[s + 1]; ++j) slot[j] = s;
     if (T->enc_slot_sorted.n < slot.size()) GW_TRY(T->enc_slot_sorted.alloc(slot.size()));
-    GW_CUDA(cudaMemcpy(T->enc_slot_sorted.p, slot.data(), slot.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    GW_CUDA(cudaMemcpyAsync(T->enc_slot_sorted.p, slot.data(), slot.size() * sizeof(int32_t), cudaMemcpyHostToDevice, T->st));
+    GW_CUDA(cudaStreamSynchronize(T->st));  // (the copy reads `slot`, which goes out of scope with this block)
     long long most = 0;  // most rows (samples x rows) of one chunk's row op
     T->enc_chunks.clear();
     const int pe = chunk_points(p, batch, 1.0);
@@ -376,7 +377,8 @@ static int build_chunks(gw_plan* p, TrainState* T, int batch) {
     GW_CUDA(cudaStreamSynchronize(T->st));
     for (size_t i = 0; i < iota.size(); ++i) iota[i] = (int32_t)i;
     if (T->iota.n < iota.size()) GW_TRY(T->iota.alloc(iota.size()));
-    GW_CUDA(cudaMemcpy(T->iota.p, iota.data(), iota.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    GW_CUDA(cudaMemcpyAsync(T->iota.p, iota.data(), iota.size() * sizeof(int32_t), cudaMemcpyHostToDevice, T->st));
+    GW_CUDA(cudaStreamSynchronize(T->st));  // (the copy reads `iota`, which goes out of scope with this block)
     long long most = 0;
     T->dec_chunks.clear();
     const int pd = chunk_points(p, batch, (double)Ed / std::max(No, 1));

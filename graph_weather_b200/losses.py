@@ -67,7 +67,7 @@ class NormalizedMSELoss(torch.nn.Module):
         self.weights = torch.tensor([np.cos(lat * np.pi / 180.0) for lat in unique_lats], dtype=torch.float)
         self.normalize = normalize
         assert not torch.isnan(self.weights).any()
-        self._dev = {}  # per device: (inv_variance, node_weight, workspace, sum)
+        self._dev = {}  # per device and shape: (inv_variance, node_weight), constant tables
 
     def _device_state(self, device, num_nodes, num_features):
         key = (str(device), num_nodes, num_features)
@@ -75,13 +75,12 @@ class NormalizedMSELoss(torch.nn.Module):
             lib = _capi.load()
             inv = (1.0 / self.feature_variance.to(torch.float32)).reshape(-1).expand(num_features).to(device).contiguous()
             w = torch.from_numpy(node_weights(self.lat_lons, num_nodes)).to(device)
-            ws = torch.empty(int(lib.gw_loss_workspace_bytes()), dtype=torch.uint8, device=device)
-            s = torch.zeros(1, dtype=torch.float64, device=device)
-            self._dev[key] = (inv, w, ws, s)
+            self._dev[key] = (inv, w)
         return self._dev[key]
 
     def local_sum(self, pred: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
-        """sum over the local rows of w(n) * mean_f(...): a 1-element float64 device tensor (valid until the next call)."""
+        """sum over the local rows of w(n) * mean_f(...): a new 1-element float64 device tensor.  The result and the kernel's
+        workspace come from torch's allocator on the current stream, so calls on several streams do not share them."""
         if not (pred.is_cuda and target.is_cuda):
             raise RuntimeError("graph_weather_b200.NormalizedMSELoss runs on CUDA tensors only (no CPU fallback)")
         if pred.shape != target.shape:
@@ -94,10 +93,11 @@ class NormalizedMSELoss(torch.nn.Module):
             raise RuntimeError("feature_variance does not match the feature dimension")
         p = pred.detach().to(torch.float32).contiguous()
         t = target.detach().to(torch.float32).contiguous()
-        inv, w, ws, s = self._device_state(pred.device, num_nodes, F)
+        inv, w = self._device_state(pred.device, num_nodes, F)
         if B == 0:  # an empty batch shard (total_batch < world size) contributes nothing; the kernel is not launched
-            s.zero_()
-            return s
+            return torch.zeros(1, dtype=torch.float64, device=pred.device)
+        s = torch.empty(1, dtype=torch.float64, device=pred.device)
+        ws = torch.empty(int(lib.gw_loss_workspace_bytes()), dtype=torch.uint8, device=pred.device)
         with torch.cuda.device(pred.device):
             st = torch.cuda.current_stream().cuda_stream
             _capi._check(lib.gw_normalized_mse_loss_sum(
@@ -113,7 +113,7 @@ class NormalizedMSELoss(torch.nn.Module):
         num_nodes = int(np.prod(pred.shape[1:-1]))
         p = pred.detach().to(torch.float32).contiguous()
         t = target.detach().to(torch.float32).contiguous()
-        inv, w, _, _ = self._device_state(pred.device, num_nodes, F)
+        inv, w = self._device_state(pred.device, num_nodes, F)
         up = upstream.detach().to(device=pred.device, dtype=torch.float32).reshape(1).contiguous()
         g = torch.empty_like(p)
         if B == 0:

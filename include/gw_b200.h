@@ -11,9 +11,12 @@
  *     (thread-local).  Nothing throws across the ABI.  There is NO CPU fallback: every compute entry point
  *     fails if no CUDA device / kernel image is available.
  *   - the caller owns every buffer it passes.  The plan owns only its scratch, packed weights and the
- *     weight-constant tensors it precomputes.  One plan per device and stream; no global state; plans are
- *     independent (one per GPU rank).
- *   - `stream` is a cudaStream_t passed as void*.
+ *     weight-constant tensors it precomputes.  No global state; plans are independent (one per GPU rank).
+ *   - `stream` is a cudaStream_t passed as void*, and may be any stream of the plan's device, also a non-blocking one.  A call
+ *     does all its device work on that stream; the only exception is gw_plan_create, which zeroes the new plan's buffers on a
+ *     private stream and waits for that before it returns.  Calls on one plan share its scratch: when they come from
+ *     different streams, the caller orders each after the previous one (graph_weather_b200/_capi.py does, with an event per
+ *     plan).
  */
 #ifndef GW_B200_H
 #define GW_B200_H
@@ -145,8 +148,10 @@ int gw_forward_strided(gw_plan* plan, const float* features, float* out, int32_t
  * per-weight work -- transposed weights and, on tensor cores, the weight images -- is done once per gw_plan_set_weights, by the
  * first step after it (tag train_weights).
  * Several tapes keep several forwards alive at once (a loss summed over a multi-step rollout, back-propagated once).  Tapes of one
- * plan share its weights, graphs and gradient buffer, and run on the plan's stream.  Batches may differ between tapes.
- *   gw_tape_destroy releases the tape's memory stream-ordered on `stream` and frees the handle.
+ * plan share its weights, graphs and gradient buffer; their calls are ordered like every other call on the plan (Conventions).
+ * Batches may differ between tapes.
+ *   gw_tape_destroy releases the tape's memory stream-ordered on `stream` and frees the handle: from another stream than the
+ *   tape's last forward or backward, the caller orders it after that call as it orders any call on the plan.
  *   gw_plan_destroy releases the memory of every tape of the plan and leaves them dead: a forward or backward on a dead tape
  *   fails (gw_tape_destroy still frees the handle).
  *   A backward fails when gw_plan_set_weights ran after the tape's forward (its gradient would be taken at other weights).
