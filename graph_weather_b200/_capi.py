@@ -81,6 +81,7 @@ _SIGNATURES = {
     "gw_train_forward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp]),
     "gw_train_backward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
     "gw_tape_bytes": (_i64, [_vp]),
+    "gw_train_set_processor_segments": (ctypes.c_int, [_vp, _i32]),
     "gw_launch_count": (_i64, []),
     "gw_launch_count_reset": (None, []),
 }
@@ -195,6 +196,11 @@ class Plan:
     def train_peak_bytes(self) -> int:
         """High-water mark of the training step's working allocations over the last train_forward + train_backward."""
         return int(self.lib.gw_train_peak_bytes(self.handle))
+
+    def set_processor_segments(self, segments: int):
+        """gw_train_set_processor_segments: processor segments of the training forwards that follow (0 none, N > 0 blocks per
+        segment, -1 one segment); their backward recomputes each segment instead of keeping the processor's tape."""
+        _check(self.lib.gw_train_set_processor_segments(self.handle, int(segments)))
 
     def _dev(self, arr, dtype):
         t = torch.as_tensor(arr).to(dtype=dtype).contiguous().to(self.device)

@@ -25,7 +25,9 @@
 // Memory: the grid-sized phases (the encoder's lat/lon side, the decoder) are written once over a GridRange.  The taped step runs
 // each on one whole range and keeps its tape from the forward.  A training-only plan (gw_plan_create_train, use_checkpointing=True)
 // runs them chunk by chunk: the forward keeps only agg_m and the output rows, and the backward recomputes each chunk's tape with the
-// same ops (and, in fp32 mode, the same per-chunk operand bounds) just before that chunk's backward, then frees it.
+// same ops (and, in fp32 mode, the same per-chunk operand bounds) just before that chunk's backward, then frees it.  Processor
+// segments (gw_train_set_processor_segments, either step) do the same for the mesh-sized processor: the forward keeps x and e at the
+// start of every segment, and the backward recomputes a segment's blocks with block_fwd right before their block_bwd.
 //
 // Arithmetic (the plan's precision):
 //   fp32_simt   every product on CUDA cores in exact fp32 (gw_simt.cu).
@@ -81,10 +83,13 @@ struct gw_tape {
   size_t bytes = 0;                              // bytes they hold now
   unsigned wgen = 0;                             // gw_plan::wgen of the weights the forward ran with
   int batch = 0;
+  int segments = 0;        // processor segments its forward ran with (gw_plan::train_segments; its backward follows them)
   bool have_tape = false;  // a forward's activations, not yet consumed by a backward
   const float* features = nullptr;
   float *xm0 = nullptr, *agg_m = nullptr, *e_lat = nullptr, *Pm = nullptr, *Pd = nullptr;  // (Pm, Pd: the grid phases' mesh-side addends)
-  std::vector<float*> x, e, agg;  // x[k] k = 0..nb, e[k] k = 1..nb (e[0] = e_lat broadcast), agg[k]
+  // x[k] k = 0..nb, e[k] k = 1..nb (e[0] = e_lat broadcast), agg[k].  With processor segments only x[k], e[k] at the start of
+  // each segment and x[nb] are kept; agg, t_pe and t_pn stay empty.
+  std::vector<float*> x, e, agg;
   gw::MlpTape t_enc_node_h, t_enc_mnode, t_lat_enc;
   gw::EncTape enc;  // taped step: the grid-sized tapes (the chunked step recomputes them chunk by chunk)
   gw::DecTape dec;
@@ -143,6 +148,36 @@ static void tape_free_to(TrainState* t, gw_tape* k, size_t mark, cudaStream_t st
   }
 }
 static void tfree_to(TrainState* t, size_t mark) { tape_free_to(t, t->tp, mark, t->st); }
+// releases every allocation of the running tape made since its allocs.size() was `mark`, except the buffers in `keep` (which stay,
+// in their order, at the end of the list)
+static void tfree_except(TrainState* t, size_t mark, std::initializer_list<const void*> keep) {
+  gw_tape* k = t->tp;
+  size_t w = mark;
+  for (size_t r = mark; r < k->allocs.size(); ++r) {
+    const auto a = k->allocs[r];
+    if (std::find(keep.begin(), keep.end(), a.first) != keep.end()) {
+      k->allocs[w++] = a;
+    } else {
+      cudaFreeAsync(a.first, t->st);
+      k->bytes -= a.second;
+      t->cur_bytes -= a.second;
+    }
+  }
+  k->allocs.resize(w);
+}
+// releases one allocation of the running tape (null: none).  It may lie below a mark, so no mark may be pending across this call.
+static void tfree_one(TrainState* t, const void* q) {
+  if (!q) return;
+  gw_tape* k = t->tp;
+  for (size_t r = k->allocs.size(); r-- > 0;)
+    if (k->allocs[r].first == q) {
+      cudaFreeAsync(k->allocs[r].first, t->st);
+      k->bytes -= k->allocs[r].second;
+      t->cur_bytes -= k->allocs[r].second;
+      k->allocs.erase(k->allocs.begin() + r);
+      return;
+    }
+}
 static void tape_release(TrainState* t, gw_tape* k, cudaStream_t st) {
   tape_free_to(t, k, 0, st);
   k->have_tape = false;
@@ -676,6 +711,158 @@ static int dec_bwd(gw_plan* p, TrainState* T, const GridRange& r, const DecTape&
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
+// one processor block (the taped forward, the segmented forward and the segments' recompute in the backward all run these)
+// ---------------------------------------------------------------------------------------------------------------------------
+// the block's edge input e[k]: e_lat broadcast over the batch in block 0
+static RowSrc block_edge_src(TrainState* T, int k, const float* ek, int De, int El) {
+  return k == 0 ? src_bcast(T->tp->e_lat, De, De) : src_stream(ek, De, De, El);
+}
+
+// block k from x[k] (xk) and e[k] (ek; block 0 reads e_lat): P [B, H, 2 He] is the caller's scratch for the factored layer 1's node
+// terms.  Allocates e[k+1], agg[k] and x[k+1], in that order, on the running tape; tpe / tpn receive the edge and node MLP tapes.
+static int block_fwd(gw_plan* p, TrainState* T, int k, const float* xk, const float* ek, float* P, float** en_out, float** ag_out, float** xn_out,
+                     MlpTape* tpe, MlpTape* tpn) {
+  const gw_dims& d = p->d;
+  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, H = d.n_mesh, El = d.n_lat_edges, B = T->tp->batch;
+  RowSrc none;
+  const Mlp& me = p->proc_edge[k];
+  const Mlp& mn = p->proc_node[k];
+  for (int h = 0; h < 2; ++h) {
+    GemmOp t;
+    t.rows_per_sample = H, t.batch = B, t.a[0] = src_stream(xk, Dn, Dn, H), t.W = me.W[0] + h * Dn, t.K = Dn, t.ldw = me.in[0], t.N = He;
+    t.out = P + h * He, t.ldo = 2 * He;
+    GW_TRY(train_op(p, T, t, TAG_TRAIN_FWD));
+  }
+  const RowSrc e_src = block_edge_src(T, k, ek, De, El);
+  GW_TALLOC(en, (size_t)B * El * De);
+  {
+    GemmOp fo = first_op(El, B, e_src, none, me.W[0] + 2 * Dn, De, me.in[0], me.b[0]);
+    fo.add[0] = src_gather(P, 2 * He, He, p->lat_src.p, H, 0);
+    fo.add[1] = src_gather(P, 2 * He, He, p->lat_dst.p, H, He);
+    GW_TRY(mlp_fwd(p, T, me, fo, e_src, en, De, tpe));
+  }
+  GW_TALLOC(ag, (size_t)B * H * De);
+  GW_OTHER(launch_segsum(en, De, De, p->lat_ptr.p, nullptr, El, H, B, ag, De, T->st));
+  GW_TALLOC(xn, (size_t)B * H * Dn);
+  GW_TRY(mlp_fwd(p, T, mn, first_op(H, B, src_stream(xk, Dn, Dn, H), src_stream(ag, De, De, H), mn.W[0], mn.in[0], mn.in[0], mn.b[0]),
+                 src_stream(xk, Dn, Dn, H), xn, Dn, tpn));
+  *en_out = en, *ag_out = ag, *xn_out = xn;
+  return 0;
+}
+
+// backward of block k: dx / de are the gradients of x[k+1] / e[k+1] (de null: none flows into the last block's e'); xk, ek, agg,
+// tpe, tpn what block_fwd read and kept.  Returns the gradients of x[k] and e[k] (allocated on the running tape).
+static int block_bwd(gw_plan* p, TrainState* T, int k, const float* xk, const float* ek, const float* agg, const MlpTape& tpe, const MlpTape& tpn,
+                     const float* dx, const float* de, float** dx_out, float** de_out) {
+  const gw_dims& d = p->d;
+  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, H = d.n_mesh, El = d.n_lat_edges, B = T->tp->batch;
+  const cudaStream_t st = T->st;
+  const Mlp& me = p->proc_edge[k];
+  const Mlp& mn = p->proc_node[k];
+  float* dh = nullptr;
+  // node MLP: x[k+1] = LN(MLP([x[k] ; agg[k]])) + x[k]
+  GW_TRY(mlp_bwd(p, T, mn, tpn, dx, Dn, &dh));
+  GW_TRY(train_wgrad(p, T, dh, mn.out[0], mn.out[0], src_stream(xk, Dn, Dn, H), Dn, H, B, grad_of(p, T, mn.W[0]), mn.in[0], grad_of(p, T, mn.b[0])));
+  GW_TRY(train_wgrad(p, T, dh, mn.out[0], mn.out[0], src_stream(agg, De, De, H), De, H, B, grad_of(p, T, mn.W[0]) + Dn, mn.in[0], nullptr));
+  GW_TALLOC(dxk, (size_t)B * H * Dn);
+  GW_TRY(dgrad(p, T, dh, mn.out[0], mn.out[0], H, B, mn.W[0], mn.out[0], 0, Dn, nullptr, 0, dx, Dn, dxk, Dn));  // + residual path
+  GW_TALLOC(d_agg, (size_t)B * H * De);
+  GW_TRY(dgrad(p, T, dh, mn.out[0], mn.out[0], H, B, mn.W[0], mn.out[0], Dn, De, nullptr, 0, nullptr, 0, d_agg, De));
+  // e[k+1] receives its target's aggregate gradient (+ what the next block sent back)
+  GW_TALLOC(d_en, (size_t)B * El * De);
+  if (de) {
+    GW_CUDA(cudaMemcpyAsync(d_en, de, (size_t)B * El * De * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    GW_OTHER(launch_gather_rows(d_agg, De, H, p->lat_dst.p, El, De, B, d_en, De, true, st));
+  } else {
+    GW_OTHER(launch_gather_rows(d_agg, De, H, p->lat_dst.p, El, De, B, d_en, De, false, st));
+  }
+  // edge MLP: e[k+1] = LN(...) + e[k];  h1 = relu(e[k] W1e^T + P_s[src] + P_d[dst] + b1)
+  GW_TRY(mlp_bwd(p, T, me, tpe, d_en, De, &dh));
+  const RowSrc e_src = block_edge_src(T, k, ek, De, El);
+  GW_TRY(train_wgrad(p, T, dh, He, He, e_src, De, El, B, grad_of(p, T, me.W[0]) + 2 * Dn, me.in[0], grad_of(p, T, me.b[0])));
+  GW_TALLOC(d_ek, (size_t)B * El * De);
+  GW_TRY(dgrad(p, T, dh, He, He, El, B, me.W[0], me.out[0], 2 * Dn, De, nullptr, 0, d_en, De, d_ek, De));  // + residual path
+  GW_TALLOC(dPs, (size_t)B * H * He);
+  GW_TALLOC(dPt, (size_t)B * H * He);
+  GW_OTHER(launch_segsum(dh, He, He, T->lat_ptr_src.p, T->lat_perm_src.p, El, H, B, dPs, He, st));
+  GW_OTHER(launch_segsum(dh, He, He, p->lat_ptr.p, nullptr, El, H, B, dPt, He, st));
+  GW_TRY(train_wgrad(p, T, dPs, He, He, src_stream(xk, Dn, Dn, H), Dn, H, B, grad_of(p, T, me.W[0]), me.in[0], nullptr));
+  GW_TRY(train_wgrad(p, T, dPt, He, He, src_stream(xk, Dn, Dn, H), Dn, H, B, grad_of(p, T, me.W[0]) + Dn, me.in[0], nullptr));
+  GW_TALLOC(dx1, (size_t)B * H * Dn);
+  GW_TRY(dgrad(p, T, dPs, He, He, H, B, me.W[0], me.out[0], 0, Dn, nullptr, 0, dxk, Dn, dx1, Dn));
+  GW_TALLOC(dx2, (size_t)B * H * Dn);
+  GW_TRY(dgrad(p, T, dPt, He, He, H, B, me.W[0], me.out[0], Dn, Dn, nullptr, 0, dx1, Dn, dx2, Dn));
+  *dx_out = dx2, *de_out = d_ek;
+  return 0;
+}
+
+// blocks per processor segment of a tape recorded with `segments` (0: no segments; -1 or >= num_blocks: one segment)
+static int segment_blocks(int segments, int nb) { return (segments < 0 || segments >= nb) ? nb : segments; }
+
+// the processor of a forward with segments: every block runs as in the taped step, but the tape keeps only x[k0], e[k0] at the
+// start of each segment and the output x[nb]; a block's tapes and sums, and its inputs unless they start a segment, are released
+// as soon as the block has run
+static int proc_fwd_segmented(gw_plan* p, TrainState* T, gw_tape* K) {
+  const gw_dims& d = p->d;
+  const int He = d.hidden_edge, H = d.n_mesh, nb = d.num_blocks, B = K->batch, S = segment_blocks(K->segments, nb);
+  GW_TALLOC(P, (size_t)B * H * 2 * He);
+  float *x = K->x[0], *e = nullptr;
+  for (int k = 0; k < nb; ++k) {
+    const size_t mark = K->allocs.size();
+    float *en = nullptr, *ag = nullptr, *xn = nullptr;
+    MlpTape tpe, tpn;
+    GW_TRY(block_fwd(p, T, k, x, e, P, &en, &ag, &xn, &tpe, &tpn));
+    tfree_except(T, mark, {en, xn});
+    if (k % S != 0) tfree_one(T, x), tfree_one(T, e);
+    x = xn, e = en;
+    if ((k + 1) % S == 0 && k + 1 < nb) K->x[k + 1] = xn, K->e[k + 1] = en;
+  }
+  K->x[nb] = x;
+  tfree_one(T, e);  // (no block reads e[nb])
+  tfree_one(T, P);
+  return 0;
+}
+
+// the processor's backward on a tape with segments, last segment first: each segment's blocks are recomputed from its kept x[k0],
+// e[k0] with block_fwd, then differentiated last block first; a block's recomputed tape and backward temporaries are released once
+// its backward has run.  Every recomputed row op measures its operand bound as the forward did (fp32), from fresh bound slots per
+// block, so the recompute reproduces the forward's values and any segment length fits the slots.  dx: gradient of x[nb] in,
+// x[0] out; de: gradient of e[0] out.
+static int proc_bwd_segmented(gw_plan* p, TrainState* T, gw_tape* K, float** dx, float** de) {
+  const gw_dims& d = p->d;
+  const int He = d.hidden_edge, H = d.n_mesh, nb = d.num_blocks, B = K->batch, S = segment_blocks(K->segments, nb);
+  float *gx = *dx, *ge = nullptr;
+  for (int k1 = nb; k1 > 0;) {
+    const int k0 = (k1 - 1) / S * S, n = k1 - k0;
+    const float* gx_in = gx;
+    const float* ge_in = ge;
+    const size_t mark = K->allocs.size();
+    std::vector<float*> xs(n + 1), es(n + 1), ags(n);
+    std::vector<MlpTape> tpe(n), tpn(n);
+    std::vector<size_t> bmark(n);
+    GW_TALLOC(P, (size_t)B * H * 2 * He);
+    xs[0] = K->x[k0], es[0] = K->e[k0];
+    for (int j = 0; j < n; ++j) {
+      bmark[j] = K->allocs.size();
+      GW_TRY(reset_bounds(T));
+      GW_TRY(block_fwd(p, T, k0 + j, xs[j], es[j], P, &es[j + 1], &ags[j], &xs[j + 1], &tpe[j], &tpn[j]));
+    }
+    for (int j = n - 1; j >= 0; --j) {
+      GW_TRY(reset_bounds(T));
+      float *gxn = nullptr, *gen = nullptr;
+      GW_TRY(block_bwd(p, T, k0 + j, xs[j], es[j], ags[j], tpe[j], tpn[j], gx, ge, &gxn, &gen));
+      tfree_except(T, bmark[j], {gxn, gen});  // block j's recompute, its temporaries, and the gradients block j + 1 sent it
+      gx = gxn, ge = gen;
+    }
+    tfree_except(T, mark, {gx, ge});  // (P)
+    tfree_one(T, gx_in), tfree_one(T, ge_in);
+    k1 = k0;
+  }
+  *dx = gx, *de = ge;
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
 // forward (keeps activations; the chunked step keeps only the mesh-sized ones, the agg_m rows and the output)
 // ---------------------------------------------------------------------------------------------------------------------------
 static int train_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* features, float* out, int B, cudaStream_t st) {
@@ -687,7 +874,7 @@ static int train_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* fea
   GW_TRY(train_prepare(p, T, B, st));
   GW_TRY(reset_bounds(T));
   RowSrc none;
-  K->features = features, K->batch = B, K->wgen = p->wgen;
+  K->features = features, K->batch = B, K->wgen = p->wgen, K->segments = p->train_segments;
   const bool chunked = p->train_only;
   // ---- encoder ------------------------------------------------------------------------------------------------------------
   // mesh rows: xm0 = node_encoder(h3_nodes), Pm = xm0 W1d^T (the mesh end of every encoder edge)
@@ -727,32 +914,13 @@ static int train_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* fea
                  &K->t_lat_enc));
   K->xm0 = xm0, K->agg_m = agg_m, K->e_lat = e_lat, K->Pm = Pm;
   // ---- processor ----------------------------------------------------------------------------------------------------------
-  GW_TALLOC(P, (size_t)B * H * 2 * He);
-  for (int k = 0; k < nb; ++k) {
-    const Mlp& me = p->proc_edge[k];
-    const Mlp& mn = p->proc_node[k];
-    for (int h = 0; h < 2; ++h) {
-      GemmOp t;
-      t.rows_per_sample = H, t.batch = B, t.a[0] = src_stream(K->x[k], Dn, Dn, H), t.W = me.W[0] + h * Dn, t.K = Dn, t.ldw = me.in[0], t.N = He;
-      t.out = P + h * He, t.ldo = 2 * He;
-      GW_TRY(train_op(p, T, t, TAG_TRAIN_FWD));
-    }
-    const RowSrc e_src = k == 0 ? src_bcast(e_lat, De, De) : src_stream(K->e[k], De, De, El);
-    GW_TALLOC(en, (size_t)B * El * De);
-    {
-      GemmOp fo = first_op(El, B, e_src, none, me.W[0] + 2 * Dn, De, me.in[0], me.b[0]);
-      fo.add[0] = src_gather(P, 2 * He, He, p->lat_src.p, H, 0);
-      fo.add[1] = src_gather(P, 2 * He, He, p->lat_dst.p, H, He);
-      GW_TRY(mlp_fwd(p, T, me, fo, e_src, en, De, &K->t_pe[k]));
-    }
-    K->e[k + 1] = en;
-    GW_TALLOC(ag, (size_t)B * H * De);
-    GW_OTHER(launch_segsum(en, De, De, p->lat_ptr.p, nullptr, El, H, B, ag, De, st));
-    K->agg[k] = ag;
-    GW_TALLOC(xn, (size_t)B * H * Dn);
-    GW_TRY(mlp_fwd(p, T, mn, first_op(H, B, src_stream(K->x[k], Dn, Dn, H), src_stream(ag, De, De, H), mn.W[0], mn.in[0], mn.in[0], mn.b[0]),
-                   src_stream(K->x[k], Dn, Dn, H), xn, Dn, &K->t_pn[k]));
-    K->x[k + 1] = xn;
+  if (K->segments == 0) {
+    GW_TALLOC(P, (size_t)B * H * 2 * He);
+    for (int k = 0; k < nb; ++k)
+      GW_TRY(block_fwd(p, T, k, K->x[k], K->e[k], P, &K->e[k + 1], &K->agg[k], &K->x[k + 1], &K->t_pe[k], &K->t_pn[k]));
+  } else {
+    K->agg.clear(), K->t_pe.clear(), K->t_pn.clear();
+    GW_TRY(proc_fwd_segmented(p, T, K));
   }
   // ---- decoder ------------------------------------------------------------------------------------------------------------
   const Mlp& mdb = p->dec_blk_edge;
@@ -816,42 +984,11 @@ static int train_backward(gw_plan* p, TrainState* T, gw_tape* K, const float* dO
   float* dx = dx_last;  // gradient of x[nb]
   // ---- processor blocks, last to first ------------------------------------------------------------------------------------------
   float* de = nullptr;  // gradient of e[k+1] (none flows into the last block's e')
-  for (int k = nb - 1; k >= 0; --k) {
-    const Mlp& me = p->proc_edge[k];
-    const Mlp& mn = p->proc_node[k];
-    // node MLP: x[k+1] = LN(MLP([x[k] ; agg[k]])) + x[k]
-    GW_TRY(mlp_bwd(p, T, mn, K->t_pn[k], dx, Dn, &dh));
-    GW_TRY(train_wgrad(p, T, dh, mn.out[0], mn.out[0], src_stream(K->x[k], Dn, Dn, H), Dn, H, B, grad_of(p, T, mn.W[0]), mn.in[0], grad_of(p, T, mn.b[0])));
-    GW_TRY(train_wgrad(p, T, dh, mn.out[0], mn.out[0], src_stream(K->agg[k], De, De, H), De, H, B, grad_of(p, T, mn.W[0]) + Dn, mn.in[0], nullptr));
-    GW_TALLOC(dxk, (size_t)B * H * Dn);
-    GW_TRY(dgrad(p, T, dh, mn.out[0], mn.out[0], H, B, mn.W[0], mn.out[0], 0, Dn, nullptr, 0, dx, Dn, dxk, Dn));  // + residual path
-    GW_TALLOC(d_agg, (size_t)B * H * De);
-    GW_TRY(dgrad(p, T, dh, mn.out[0], mn.out[0], H, B, mn.W[0], mn.out[0], Dn, De, nullptr, 0, nullptr, 0, d_agg, De));
-    // e[k+1] receives its target's aggregate gradient (+ what the next block sent back)
-    GW_TALLOC(d_en, (size_t)B * El * De);
-    if (de) {
-      GW_CUDA(cudaMemcpyAsync(d_en, de, (size_t)B * El * De * sizeof(float), cudaMemcpyDeviceToDevice, st));
-      GW_OTHER(launch_gather_rows(d_agg, De, H, p->lat_dst.p, El, De, B, d_en, De, true, st));
-    } else {
-      GW_OTHER(launch_gather_rows(d_agg, De, H, p->lat_dst.p, El, De, B, d_en, De, false, st));
-    }
-    // edge MLP: e[k+1] = LN(...) + e[k];  h1 = relu(e[k] W1e^T + P_s[src] + P_d[dst] + b1)
-    GW_TRY(mlp_bwd(p, T, me, K->t_pe[k], d_en, De, &dh));
-    const RowSrc e_src = k == 0 ? src_bcast(K->e_lat, De, De) : src_stream(K->e[k], De, De, El);
-    GW_TRY(train_wgrad(p, T, dh, He, He, e_src, De, El, B, grad_of(p, T, me.W[0]) + 2 * Dn, me.in[0], grad_of(p, T, me.b[0])));
-    GW_TALLOC(d_ek, (size_t)B * El * De);
-    GW_TRY(dgrad(p, T, dh, He, He, El, B, me.W[0], me.out[0], 2 * Dn, De, nullptr, 0, d_en, De, d_ek, De));  // + residual path
-    GW_TALLOC(dPs, (size_t)B * H * He);
-    GW_TALLOC(dPt, (size_t)B * H * He);
-    GW_OTHER(launch_segsum(dh, He, He, T->lat_ptr_src.p, T->lat_perm_src.p, El, H, B, dPs, He, st));
-    GW_OTHER(launch_segsum(dh, He, He, p->lat_ptr.p, nullptr, El, H, B, dPt, He, st));
-    GW_TRY(train_wgrad(p, T, dPs, He, He, src_stream(K->x[k], Dn, Dn, H), Dn, H, B, grad_of(p, T, me.W[0]), me.in[0], nullptr));
-    GW_TRY(train_wgrad(p, T, dPt, He, He, src_stream(K->x[k], Dn, Dn, H), Dn, H, B, grad_of(p, T, me.W[0]) + Dn, me.in[0], nullptr));
-    GW_TALLOC(dx1, (size_t)B * H * Dn);
-    GW_TRY(dgrad(p, T, dPs, He, He, H, B, me.W[0], me.out[0], 0, Dn, nullptr, 0, dxk, Dn, dx1, Dn));
-    GW_TALLOC(dx2, (size_t)B * H * Dn);
-    GW_TRY(dgrad(p, T, dPt, He, He, H, B, me.W[0], me.out[0], Dn, Dn, nullptr, 0, dx1, Dn, dx2, Dn));
-    dx = dx2, de = d_ek;
+  if (K->segments == 0) {
+    for (int k = nb - 1; k >= 0; --k)
+      GW_TRY(block_bwd(p, T, k, K->x[k], K->e[k], K->agg[k], K->t_pe[k], K->t_pn[k], dx, de, &dx, &de));
+  } else {
+    GW_TRY(proc_bwd_segmented(p, T, K, &dx, &de));
   }
   // e[0] = e_lat broadcast: reduce over the batch, back through latent_edge_encoder
   {
@@ -988,5 +1125,12 @@ int gw_train_backward_tape(gw_plan* p, gw_tape* k, const float* grad_out, float*
 }
 
 int64_t gw_train_peak_bytes(const gw_plan* p) { return (p && p->train) ? (int64_t)p->train->peak_bytes : 0; }
+
+int gw_train_set_processor_segments(gw_plan* p, int32_t segments) {
+  GW_CHECK(p != nullptr, "null plan");
+  GW_CHECK(segments >= -1, "processor segments must be -1 (the whole processor), 0 (none) or a positive number of blocks");
+  p->train_segments = segments;
+  return 0;
+}
 
 }  // extern "C"

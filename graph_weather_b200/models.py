@@ -268,6 +268,7 @@ class _TrainFn(torch.autograd.Function):
         if not in_window and eng.last_tape is not None:
             eng.last_tape.close()  # stream-ordered, ahead of this forward's allocations
             eng.last_tape = None
+        plan.set_processor_segments(model._processor_segments())
         tape = plan.tape()
         try:
             tape.forward(f, out)
@@ -332,6 +333,13 @@ def _switch_training_engine(engines: dict, bounded: bool, make) -> _Engine:
 def _wants_grad(model, features):
     """A wrapper's forward takes the training step in train mode with autograd on and something to differentiate."""
     return torch.is_grad_enabled() and model.training and (features.requires_grad or any(q.requires_grad for q in model.parameters()))
+
+
+def _check_segments(segments):
+    """A processor segment count is -1 (the whole processor), 0 (none) or a number of blocks: refused where it is set, not at the next
+    training forward."""
+    if segments < -1:
+        raise ValueError(f"checkpoint segments must be -1 (the whole processor), 0 (none) or a positive number of blocks, got {segments}")
 
 
 def _prefixed(prefix, module):
@@ -446,6 +454,11 @@ class Processor(nn.Module):
         self._engine = None
 
     def set_checkpoint_segments(self, checkpoint_segments: int):
+        """processor.py:70-81.  The training step of the wrapper this processor belongs to recomputes the processor in its backward:
+        0 (the default) keeps the processor's whole tape; N > 0 recomputes segments of N blocks, keeping only each segment's first
+        node and edge rows; -1 recomputes the whole processor as one segment.  Outputs and gradients do not change, only the memory a
+        training forward keeps and the time of its backward (gw_train_set_processor_segments).  Read at every training forward."""
+        _check_segments(checkpoint_segments)
         self.checkpoint_segments = checkpoint_segments
 
     def _sorted_graph(self, edge_index, n_nodes):
@@ -652,6 +665,10 @@ class _Wrapper(nn.Module):
 
     def _bounded_step(self) -> bool:
         return bool(self.use_checkpointing)
+
+    def _processor_segments(self) -> int:
+        """Processor segments of a training forward (`Processor.set_checkpoint_segments`), read at every training forward."""
+        return self.processor.checkpoint_segments
 
     def _training_engine(self):
         """The plan the training step runs on, of precision `train_precision`; the inference engine stays as it is.  A
@@ -986,8 +1003,10 @@ class GraphCast(_Wrapper):
         use_checkpointing, set_checkpoint_model(True), set_checkpoint_encoder(True) or set_checkpoint_decoder(True) is set --
         GraphCastConfig.full_checkpointing and balanced_checkpointing;
       * the taped step otherwise.
-    set_checkpoint_processor(segments) on its own keeps the processor's tape: the CUDA step has no processor-segment recompute
-    (DESIGN.md section 9).  Checkpointing never changes the forward's result, in the reference or here."""
+    set_checkpoint_processor(segments) combines with either step: a non-zero value makes the backward recompute the processor in
+    segments of that many blocks (-1: the whole processor as one) instead of keeping its tape -- GraphCastConfig.balanced_checkpointing
+    and processor_only_checkpointing; 0 leaves the choice to processor.set_checkpoint_segments.  Checkpointing never changes the
+    forward's result or the gradients, in the reference or here."""
 
     def __init__(self, lat_lons: list, resolution: int = 2, input_dim: int = 78, output_dim: int = 78, hidden_dim: int = 256,
                  num_processor_blocks: int = 9, hidden_layers: int = 2, mlp_norm_type: str = "LayerNorm",
@@ -1023,6 +1042,9 @@ class GraphCast(_Wrapper):
     def _bounded_step(self) -> bool:
         return bool(self.use_checkpointing or self._checkpoint_model or self._checkpoint_encoder or self._checkpoint_decoder)
 
+    def _processor_segments(self) -> int:
+        return self._checkpoint_processor_segments or self.processor.checkpoint_segments
+
     # hierarchical checkpointing controls (model.py:118-174)
     def set_checkpoint_model(self, checkpoint_flag: bool):
         self._checkpoint_model = checkpoint_flag
@@ -1035,6 +1057,7 @@ class GraphCast(_Wrapper):
         self._checkpoint_encoder = checkpoint_flag
 
     def set_checkpoint_processor(self, checkpoint_segments: int):
+        _check_segments(checkpoint_segments)
         self._checkpoint_processor_segments = checkpoint_segments
 
     def set_checkpoint_decoder(self, checkpoint_flag: bool):

@@ -230,6 +230,10 @@ class RegionalForecaster(nn.Module):
         self.__dict__["_train_engine"] = eng
         return eng
 
+    def _processor_segments(self) -> int:
+        """Processor segments of a training forward (`processor.set_checkpoint_segments`)."""
+        return self.processor.checkpoint_segments
+
     def _grad_bindings(self):
         """The plan's parameters; `encoder.h3_nodes` (the region's rows of h3_embeddings) differentiates the table: the rows'
         gradients go to the region's cells (unique, so a copy), every other row is zero.  The nudging layer is not bound: its

@@ -164,6 +164,16 @@ int gw_train_forward_tape(gw_plan* plan, gw_tape* tape, const float* features, f
 int gw_train_backward_tape(gw_plan* plan, gw_tape* tape, const float* grad_out, float* grad_features, const gw_param* grads,
                            int32_t n, void* stream);
 int64_t gw_tape_bytes(const gw_tape* tape);
+/* Replaces: Processor.set_checkpoint_segments (processor.py:70-81) and GraphCast.set_checkpoint_processor (graphcast/model.py:149-163,
+ * 230-250).  Processor segments of the training forwards that start after this call, on either training step: 0 (the default) keeps
+ * the processor's whole tape; N > 0 cuts segments of N blocks (0..N-1, N..2N-1, ..., a shorter last one); -1, or any N >=
+ * num_blocks, makes the processor one segment.  A forward with segments keeps only each segment's first x and e rows and the
+ * processor's output, and its backward recomputes one segment at a time with the forward's own ops before differentiating it:
+ * outputs and gradients are those of segments = 0 bit for bit (GW_PREC_FP32_SIMT weight gradients up to its float atomics), at
+ * the cost of one more processor forward.  Each tape records the value its forward ran with, and its backward follows that, so
+ * changing it between a forward and its backward is harmless.  gw_tape_bytes and gw_train_peak_bytes depend on the shapes and
+ * this value only.  Values below -1 fail. */
+int gw_train_set_processor_segments(gw_plan* plan, int32_t segments);
 /* High-water mark, in bytes, of the training step's stream-ordered working allocations -- every live tape plus the running step's
  * temporaries -- since a training forward last began while no other tape held memory (0 before the first step).  For one tape at
  * a time: over the last gw_train_forward_tape and the gw_train_backward_tape after it.  It depends on the shapes only, unlike device-wide

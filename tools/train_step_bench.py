@@ -4,7 +4,7 @@ GraphWeatherAssimilator or RegionalForecaster.
                                      [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16] [--feature-dim F] [--aux-dim A]
                                      [--num-blocks NB] [--width W] [--constraint-type none|additive|multiplicative|softmax]
                                      [--use-checkpointing] [--fit-batch] [--n-obs N] [--rollout K [--compare-plain]]
-                                     [--extent DEG] [--max-points N] [--moving-region]
+                                     [--extent DEG] [--max-points N] [--moving-region] [--processor-segments S]
 The model defaults to the README's 78 + 24 features, 9 blocks, 256-wide.  --model graphcast: GraphCast(input_dim = output_dim =
 --feature-dim, hidden_dim = --width or 256); its bounded step is selected by --use-checkpointing (the same step
 GraphCastConfig.balanced_checkpointing / full_checkpointing select).  --model assimilator: GraphWeatherAssimilator(output_lat_lons =
@@ -31,6 +31,9 @@ synthetic regions shaped like the reference's RegionalDataset samples: a square 
 centre on the 0.25-degree grid, --max-points of its points drawn without replacement (--grid is not used).  One box is reused for
 every step, or with --moving-region a new box is drawn for every step, as the dataset does: that step also builds the region's
 graphs on the host, creates its plans and uploads the graphs and weights, so the difference of the two is the per-region set-up cost.
+--processor-segments S: processor.set_checkpoint_segments(S) -- the backward recomputes the processor in segments of S blocks
+(-1: one segment) instead of keeping its tape; "tape_bytes" (gw_tape_bytes of every tape of the last step, read before its backward)
+shows what that saves.
 With --constraint-type the step includes PhysicalConstraintLayer; the constraint backward
 (gw_constraint_backward, no timing tag of the plan) is also timed on its own with CUDA events around it, on the step's shapes."""
 import argparse
@@ -46,14 +49,14 @@ sys.path.insert(0, ROOT)
 
 
 def card():
-    """Name and enforced power limit of cuda:0 (read-only query; None where nvidia-smi is unavailable)."""
-    info = {"name": torch.cuda.get_device_name(0), "power_limit_w": None}
+    """Name, enforced power limit and SM clocks (now and at most) of cuda:0 (read-only query; None where nvidia-smi is unavailable)."""
+    info = {"name": torch.cuda.get_device_name(0), "power_limit_w": None, "sm_clock_mhz": None, "sm_clock_max_mhz": None}
     try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", "0"], capture_output=True,
-                           text=True, timeout=30)  # fmt: skip
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader,nounits", "-i", "0"],
+                           capture_output=True, text=True, timeout=30)  # fmt: skip
         if r.returncode == 0 and r.stdout.strip():
-            name, pl = [v.strip() for v in r.stdout.strip().splitlines()[0].split(",")]
-            info["name"], info["power_limit_w"] = name, float(pl)
+            name, pl, clk, clk_max = [v.strip() for v in r.stdout.strip().splitlines()[0].split(",")]
+            info["name"], info["power_limit_w"], info["sm_clock_mhz"], info["sm_clock_max_mhz"] = name, float(pl), float(clk), float(clk_max)
     except (OSError, ValueError, subprocess.SubprocessError):
         pass
     return info
@@ -103,6 +106,7 @@ def main():
     ap.add_argument("--extent", type=float, default=20.0, help="side of the square region in degrees (--model regional)")
     ap.add_argument("--max-points", type=int, default=2000, help="points per region (--model regional)")
     ap.add_argument("--moving-region", action="store_true", help="a new region for every step (--model regional)")
+    ap.add_argument("--processor-segments", type=int, default=0, help="processor.set_checkpoint_segments(S): 0 none, N blocks, -1 one")
     a = ap.parse_args()
     if a.model == "regional" and (a.rollout or a.fit_batch):
         ap.error("--model regional: no --rollout or --fit-batch")
@@ -169,9 +173,10 @@ def main():
         model = GraphWeatherForecaster(ll, train_precision=a.train_precision, constraint_type=a.constraint_type,
                                        use_checkpointing=a.use_checkpointing, **dims).cuda().train()  # fmt: skip
         n_in, f_in = len(ll), F + a.aux_dim
+    model.processor.set_checkpoint_segments(a.processor_segments)
     crit = torch.nn.functional.mse_loss if a.model == "regional" else NormalizedMSELoss([1.0] * F, ll, normalize=True)
     opt = torch.optim.SGD(model.parameters(), lr=1e-3)
-    tape_bytes = []  # gw_tape_bytes of every tape of the last --rollout step, read before its backward
+    tape_bytes = []  # gw_tape_bytes of every tape of the last step, read before its backward
 
     def measure(batch, steps):
         """(ms/step, losses, torch peak bytes, train_peak_bytes, plan device_bytes, step function, inputs) of `steps` timed steps."""
@@ -193,11 +198,11 @@ def main():
                         loss = loss + crit(out, y)
                         if t + 1 < rollout:
                             inp = torch.cat([out, x[..., F:]], -1) if f_in > F else out
-                tape_bytes[:] = [t.bytes() for t in model._train_engine.plan.live_tapes()]
             elif a.model == "regional":  # (every box has max_points points: the inputs keep their shapes)
                 loss = crit(model(x, box() if a.moving_region else fixed), y)
             else:
                 loss = crit(model(x, obs()) if a.model == "assimilator" else model(x), y)
+            tape_bytes[:] = [t.bytes() for t in model._train_engine.plan.live_tapes()]
             loss.backward()
             opt.step()
             return loss.detach()
@@ -260,7 +265,8 @@ def main():
     plan.status()
     cbwd = constraint_backward_time(model, x, F) if a.constraint_type != "none" else None
     print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "model": a.model, "train_precision": a.train_precision, "grid": None if a.model == "regional" else a.grid, "batch": a.batch,
-                      "use_checkpointing": a.use_checkpointing, "rollout": rollout, "train_peak_gib": round(train_peak / 2**30, 3),
+                      "use_checkpointing": a.use_checkpointing, "processor_segments": a.processor_segments,
+                      "tape_bytes": list(tape_bytes), "rollout": rollout, "train_peak_gib": round(train_peak / 2**30, 3),
                       "plan_device_gib": round(plan_bytes / 2**30, 3),
                       "dims": dims, "constraint_type": a.constraint_type, "constraint_backward": cbwd,
                       "n_params": sum(q.numel() for q in model.parameters()),
