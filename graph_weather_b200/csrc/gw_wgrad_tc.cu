@@ -35,6 +35,10 @@ namespace wgt {
 constexpr int RC = 64;                      // rows per chunk (the K of four m64nNk16 steps)
 constexpr int OB = 128;                     // o rows per CTA
 constexpr int THREADS = 256;
+// Rows one wgmma accumulator sums before it is added into the CTA's partial (round-to-nearest fp32, in row order): the wgmma
+// accumulator's additions do not round to nearest, so its error grows with the rows it sums faster than fp32 summation's.  The
+// bound keeps a long row range (~55 000 rows per CTA at 3.6 M rows, N = 256) as accurate as a short one.
+constexpr int FLUSH_CHUNKS = 32;            // 2048 rows
 constexpr int Y_HALF = OB * 128;            // [128 o][64 r] 16-bit
 constexpr int A_HALF = 256 * 128;           // [256 k][64 r] 16-bit
 constexpr int STAGE = 2 * (Y_HALF + A_HALF);  // hi | lo of both images
@@ -161,6 +165,26 @@ __global__ void __launch_bounds__(THREADS, 1) gw_wgrad_tc_kernel(const __grid_co
 #pragma unroll
   for (int i = 0; i < 128; ++i) d[i] = 0.f;
   const int wg = warp >> 2;
+  // accumulator -> this CTA's partial block (the first flush stores, later ones add): thread t of warp q4 holds
+  // (o = 16 q4 + t/4 + 8 m, k = 8 j + 2 (t % 4) + e) of its warpgroup's 64 rows
+  const float inv = (1.f / sy) * (1.f / sa);
+  const int q4 = warp & 3;
+  float* part = a.part + (size_t)blockIdx.x * a.N * a.K;
+  auto flush = [&](bool first) {
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+      const int o = o0 + 64 * wg + 16 * q4 + (lane >> 2) + 8 * m;
+      if (o < a.N) {
+#pragma unroll
+        for (int j = 0; j < NW / 8; ++j) {
+          const int k = 8 * j + 2 * (lane & 3);
+          float* p = part + (size_t)o * a.K + k;
+          if (k < a.K) p[0] = first ? d[4 * j + 2 * m] * inv : p[0] + d[4 * j + 2 * m] * inv;
+          if (k + 1 < a.K) p[1] = first ? d[4 * j + 2 * m + 1] * inv : p[1] + d[4 * j + 2 * m + 1] * inv;
+        }
+      }
+    }
+  };
   if (nchunks > 0) stage(0, 0);
   __syncthreads();
   for (int c = 0; c < nchunks; ++c) {
@@ -180,24 +204,14 @@ __global__ void __launch_bounds__(THREADS, 1) gw_wgrad_tc_kernel(const __grid_co
     if (c + 1 < nchunks) stage(c + 1, (c + 1) & 1);  // overlaps the wgmma of chunk c
     wgmma_wait<0>();
     fence_operand(d);
+    if ((c + 1) % FLUSH_CHUNKS == 0 && c + 1 < nchunks) {  // (the next wgmma_fence orders the cleared registers)
+      flush(c + 1 == FLUSH_CHUNKS);
+#pragma unroll
+      for (int i = 0; i < 128; ++i) d[i] = 0.f;
+    }
     __syncthreads();  // both warpgroups are done with stage c & 1 before it is refilled
   }
-  // partial block -> workspace: thread t of warp q4 holds (o = 16 q4 + t/4 + 8 m, k = 8 j + 2 (t % 4) + e) of its warpgroup's 64 rows
-  const float inv = (1.f / sy) * (1.f / sa);
-  const int q4 = warp & 3;
-  float* part = a.part + (size_t)blockIdx.x * a.N * a.K;
-#pragma unroll
-  for (int m = 0; m < 2; ++m) {
-    const int o = o0 + 64 * wg + 16 * q4 + (lane >> 2) + 8 * m;
-    if (o < a.N) {
-#pragma unroll
-      for (int j = 0; j < NW / 8; ++j) {
-        const int k = 8 * j + 2 * (lane & 3);
-        if (k < a.K) part[(size_t)o * a.K + k] = d[4 * j + 2 * m] * inv;
-        if (k + 1 < a.K) part[(size_t)o * a.K + k + 1] = d[4 * j + 2 * m + 1] * inv;
-      }
-    }
-  }
+  flush(nchunks <= FLUSH_CHUNKS);
   // bias: the 8 lanes of a column quad hold the 8 row groups
 #pragma unroll
   for (int i = 0; i < 4; ++i) {

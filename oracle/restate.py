@@ -122,7 +122,7 @@ def gnn_block(sd, prefix, x, edge_index, edge_attr, hl_node=2, hl_edge=2):
     out = mlp(sd, f"{prefix}.edge_model.edge_mlp", out, hl_edge)
     out += edge_attr
     edge_attr = out
-    agg = torch.zeros((x.size(0), edge_attr.size(1)), dtype=x.dtype).scatter_add_(
+    agg = torch.zeros((x.size(0), edge_attr.size(1)), dtype=x.dtype, device=x.device).scatter_add_(
         0, col.view(-1, 1).expand_as(edge_attr), edge_attr
     )
     out = torch.cat([x, agg], dim=-1)
@@ -174,7 +174,7 @@ def assimilator_decoder_forward(sd, g, processor_features, batch_size, prefix="d
     edge_attr = edge_attr.repeat(batch_size, 1)
     edge_index = _replicate(g["dec_edge_index"], batch_size)
     feats = processor_features.reshape(batch_size, -1, processor_features.shape[-1])
-    latlon_nodes = torch.zeros((batch_size, g["num_latlons"], feats.shape[-1]), dtype=feats.dtype)
+    latlon_nodes = torch.zeros((batch_size, g["num_latlons"], feats.shape[-1]), dtype=feats.dtype, device=feats.device)
     feats = torch.cat([feats, latlon_nodes], dim=1).reshape(-1, feats.shape[-1])
     out, _ = graph_processor(sd, f"{prefix}.graph_processor", feats, edge_index, edge_attr, 1, hl_node, hl_edge)
     out = mlp(sd, f"{prefix}.node_decoder", out, hl_dec, norm=False)

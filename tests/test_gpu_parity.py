@@ -266,39 +266,6 @@ def test_1deg_batch8_two_samples_against_oracle():
         assert err < TOL
 
 
-def _quarter_deg():
-    lat = -90.0 + 0.25 * np.arange(721)
-    lon = 0.25 * np.arange(1440)
-    return np.stack(np.meshgrid(lat, lon, indexing="ij"), axis=-1).reshape(-1, 2)
-
-
-def test_quarter_degree_tensor_core_vs_exact_fp32():
-    """BASELINE configs[2] grid (0.25 degree ERA5, 1 038 240 points).  No CPU oracle fits (22 GB/sample), so the wgmma path is
-    checked against the exact-fp32 CUDA-core path -- itself pinned to the reference fixtures and the oracle above -- on one
-    sample (< 1e-4), and bf16 against the fp32-faithful path at its own tolerance."""
-    from graph_weather_b200 import GraphWeatherForecaster
-    from oracle import weights
-
-    ll = _quarter_deg()
-    assert len(ll) == 1038240
-    sd = weights.make_state_dict(weights.forecaster_shapes(), 10)
-    x = weights.make_features(1, len(ll), 102, 10).cuda()
-    outs = {}
-    for precision in ("fp32_simt", "fp32", "bf16"):
-        model = GraphWeatherForecaster(ll, precision=precision).cuda().eval()
-        model.load_state_dict(sd)
-        outs[precision] = model(x).clone()
-        assert outs[precision].shape == (1, 1038240, 78) and torch.isfinite(outs[precision]).all()
-        model._engine.plan.status()
-        del model
-        torch.cuda.empty_cache()
-    e32 = float((outs["fp32"] - outs["fp32_simt"]).abs().max())
-    e16 = float((outs["bf16"] - outs["fp32"]).abs().max())
-    print(f"0.25deg: max|tc - simt| = {e32:.3e}, max|bf16 - tc| = {e16:.3e}")
-    assert e32 < TOL
-    assert e16 < BF16_TOL
-
-
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 def test_quarter_degree_regional_crop_against_oracle(precision):
     """0.25 degree spacing against the reference arithmetic: a 40 x 80 degree crop of the ERA5 grid (51 681 points, up to ~40

@@ -12,9 +12,18 @@ def _grid(step):
     return [(float(lat), float(lon)) for lat in range(-90, 90, step) for lon in range(0, 360, step)]
 
 
-@pytest.mark.parametrize("step", [10, 30])
+def _quarter_degree():
+    """The ERA5 0.25-degree grid as bench.py builds it: 721 x 1440 points, lat = -90 + 0.25 i (both poles), lon = 0.25 j."""
+    lat = -90.0 + 0.25 * np.arange(721)
+    lon = 0.25 * np.arange(1440)
+    return np.stack(np.meshgrid(lat, lon, indexing="ij"), axis=-1).reshape(-1, 2)
+
+
+# 10 and 30 degrees; 1 degree (64 800 points); 0.25 degrees (1 038 240 points, up to 9 142 in one mesh cell, 7.27 M decoder edges:
+# the loops take about 2 minutes there)
+@pytest.mark.parametrize("step", [10, 30, 1, 0.25])
 def test_vectorised_equals_loops(step):
-    ll = _grid(step)
+    ll = _quarter_degree() if step == 0.25 else _grid(step)
     g = restate.build_forecaster_graphs(ll)
     e = graphs.build_encoder_graph(ll)
     m = graphs.build_mesh_graph()
