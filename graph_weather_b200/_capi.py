@@ -81,6 +81,12 @@ _SIGNATURES = {
     "gw_train_forward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp]),
     "gw_train_backward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
     "gw_tape_bytes": (_i64, [_vp]),
+    "gw_train_encoder_forward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _vp]),
+    "gw_train_encoder_backward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
+    "gw_train_processor_forward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "gw_train_processor_backward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
+    "gw_train_decoder_forward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _i32, _vp]),
+    "gw_train_decoder_backward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
     "gw_train_set_processor_segments": (ctypes.c_int, [_vp, _i32]),
     "gw_launch_count": (_i64, []),
     "gw_launch_count_reset": (None, []),
@@ -130,6 +136,11 @@ def _ptr(t, dtype, device):
     if t.dtype != dtype or not t.is_contiguous() or t.device != device:
         raise RuntimeError(f"expected a contiguous {dtype} tensor on {device}, got {t.dtype} on {t.device}")
     return ctypes.c_void_p(t.data_ptr())
+
+
+def _opt_ptr(t, device):
+    """An optional float32 tensor argument: NULL for None."""
+    return _vp() if t is None else _ptr(t, torch.float32, device)
 
 
 def launch_count() -> int:
@@ -410,6 +421,50 @@ class Tape:
         with self.plan._on_stream() as st:
             gf = _ptr(grad_features, torch.float32, d) if grad_features is not None else _vp()
             _check(self.lib.gw_train_backward_tape(self._plan_handle(), self.handle, _ptr(grad_out, torch.float32, d), gf, arr, n, st))
+
+    # one stage alone (gw_train_{encoder,processor,decoder}_{forward,backward}_tape); None gradients pass NULL
+    def encoder_forward(self, features, x_out, e_lat_out):
+        d = self.plan.device
+        with self.plan._on_stream() as st:
+            _check(self.lib.gw_train_encoder_forward_tape(self._plan_handle(), self.handle, _ptr(features, torch.float32, d),
+                                                          _ptr(x_out, torch.float32, d), _ptr(e_lat_out, torch.float32, d),
+                                                          int(features.shape[0]), st))  # fmt: skip
+
+    def encoder_backward(self, grad_x, grad_e_lat, grad_features, named_grads):
+        d = self.plan.device
+        arr, n = self.plan._grad_table(named_grads)
+        with self.plan._on_stream() as st:
+            _check(self.lib.gw_train_encoder_backward_tape(self._plan_handle(), self.handle, _ptr(grad_x, torch.float32, d),
+                                                           _opt_ptr(grad_e_lat, d), _opt_ptr(grad_features, d), arr, n, st))  # fmt: skip
+
+    def processor_forward(self, x_in, x_out, edge_attr, src, dst, ptr):
+        d = self.plan.device
+        with self.plan._on_stream() as st:
+            _check(self.lib.gw_train_processor_forward_tape(
+                self._plan_handle(), self.handle, _ptr(x_in, torch.float32, d), _ptr(x_out, torch.float32, d),
+                _ptr(edge_attr, torch.float32, d), int(x_in.shape[0]), int(src.numel()), _ptr(src, torch.int32, d),
+                _ptr(dst, torch.int32, d), _ptr(ptr, torch.int32, d), st))  # fmt: skip
+
+    def processor_backward(self, grad_x_out, grad_x_in, grad_edge_attr, named_grads):
+        d = self.plan.device
+        arr, n = self.plan._grad_table(named_grads)
+        with self.plan._on_stream() as st:
+            _check(self.lib.gw_train_processor_backward_tape(self._plan_handle(), self.handle, _ptr(grad_x_out, torch.float32, d),
+                                                             _opt_ptr(grad_x_in, d), _opt_ptr(grad_edge_attr, d), arr, n, st))  # fmt: skip
+
+    def decoder_forward(self, x_in, start, out, batch):
+        d = self.plan.device
+        with self.plan._on_stream() as st:
+            ld = int(start.shape[-1]) if start is not None else 0
+            _check(self.lib.gw_train_decoder_forward_tape(self._plan_handle(), self.handle, _ptr(x_in, torch.float32, d), _opt_ptr(start, d),
+                                                          ld, _ptr(out, torch.float32, d), int(batch), st))  # fmt: skip
+
+    def decoder_backward(self, grad_out, grad_x_in, named_grads):
+        d = self.plan.device
+        arr, n = self.plan._grad_table(named_grads)
+        with self.plan._on_stream() as st:
+            _check(self.lib.gw_train_decoder_backward_tape(self._plan_handle(), self.handle, _ptr(grad_out, torch.float32, d),
+                                                           _opt_ptr(grad_x_in, d), arr, n, st))  # fmt: skip
 
     def bytes(self) -> int:
         """gw_tape_bytes: what the tape holds now (between its forward and backward, the forward's saved tensors)."""

@@ -258,6 +258,7 @@ int gw_plan_set_latent_graph(gw_plan* p, const int32_t* src, const int32_t* dst,
   GW_CUDA(cudaMemcpyAsync(p->lat_attr.p, attr, El * 2 * 4, cudaMemcpyDeviceToDevice, st));
   GW_TRY(gw::csr_stats(p, p->lat_ptr.p, p->d.n_mesh, nullptr, &p->lat_maxdeg, &p->lat_mindeg, st));
   p->have_lat = true;
+  ++p->graph_gen;
   p->w_enc = p->w_proc = p->w_dec = false;  // constants depend on the graphs: weights must be (re)uploaded after
   return 0;
 }
@@ -272,6 +273,7 @@ int gw_plan_set_decoder_graph(gw_plan* p, const int32_t* src, const int32_t* ptr
   GW_CUDA(cudaMemcpyAsync(p->dec_attr.p, attr, Ed * 2 * 4, cudaMemcpyDeviceToDevice, st));
   GW_TRY(gw::csr_stats(p, p->dec_ptr.p, p->d.n_out, p->dec_dst.p, &p->dec_maxdeg, &p->dec_mindeg, st));
   p->have_dec = true;
+  ++p->graph_gen;
   p->w_enc = p->w_proc = p->w_dec = false;
   return 0;
 }

@@ -105,6 +105,7 @@ struct gw_plan {
   int device = 0;
   int n_in_cur = 0;
   unsigned enc_graph_gen = 0;  // bumped whenever the encoder graph is replaced (the training step's chunk tables are built per graph)
+  unsigned graph_gen = 0;      // bumped whenever the latent or decoder graph is replaced (the training step's source-sorted copies follow it)
   unsigned wgen = 0;           // bumped by every gw_plan_set_weights (the training step's per-weight work and its tapes key on it)
   // graphs
   DevBuf<int32_t> enc_mesh, enc_perm, enc_ptr, lat_src, lat_dst, lat_ptr, dec_src, dec_ptr;

@@ -22,6 +22,10 @@
 // Tapes: what a forward saves for its backward is a gw_tape.  Every forward runs on a tape gw_tape_create made -- one per training
 // step, or one per forward of a multi-step rollout -- and its own backward consumes it.
 //
+// Stages: the step is three stage functions (enc_stage_* / proc_stage_* / dec_stage_*) with explicit boundary tensors; the whole
+// network's forward and backward compose them, and the reference's standalone Encoder / Processor / Decoder train on one stage
+// alone (gw_train_{encoder,processor,decoder}_{forward,backward}_tape).
+//
 // Memory: the grid-sized phases (the encoder's lat/lon side, the decoder) are written once over a GridRange.  The taped step runs
 // each on one whole range and keeps its tape from the forward.  A training-only plan (gw_plan_create_train, use_checkpointing=True)
 // runs them chunk by chunk: the forward keeps only agg_m and the output rows, and the backward recomputes each chunk's tape with the
@@ -69,6 +73,16 @@ struct DecTape {
   float *e_dec = nullptr, *agg_g = nullptr, *xg2 = nullptr;
   MlpTape edge_enc, edge, node, out;
 };
+// the graph a tape's processor runs on: the plan's latent graph (the whole network), or a standalone processor's per-call graph
+// copied onto the tape with its source-sorted CSR (gw_train_processor_forward_tape)
+struct LatGraph {
+  int H = 0, El = 0;                                              // nodes per sample, edges per sample
+  const int32_t *src = nullptr, *dst = nullptr, *ptr = nullptr;   // edges sorted by target, CSR over targets
+  const int32_t *perm_src = nullptr, *ptr_src = nullptr;          // the same edges grouped by source
+  bool e0_bcast = true;  // block 0 reads e[0] as one sample's rows broadcast over the batch (the encoder's e_lat), else per edge
+};
+// what a tape's forward ran, so that only the matching backward consumes it
+enum TapeStage { TAPE_NET = 0, TAPE_ENC, TAPE_PROC, TAPE_DEC };
 
 }  // namespace gw
 
@@ -85,11 +99,18 @@ struct gw_tape {
   int batch = 0;
   int segments = 0;        // processor segments its forward ran with (gw_plan::train_segments; its backward follows them)
   bool have_tape = false;  // a forward's activations, not yet consumed by a backward
+  int stage = gw::TAPE_NET;        // the forward that made it: the whole network or one stage
+  unsigned enc_gen = 0;            // gw_plan::enc_graph_gen its encoder ran on
+  bool caller_input = false;       // the processor's / decoder's input rows are the caller's: their stage-0 ops bound them (train_op)
   const float* features = nullptr;
+  const float* start = nullptr;    // the decoder's residual rows (the features in the whole network), row stride start_ld
+  int start_ld = 0;
+  const float* xd = nullptr;       // the decoder's input x [B, H, Dn]
   float *xm0 = nullptr, *agg_m = nullptr, *e_lat = nullptr, *Pm = nullptr, *Pd = nullptr;  // (Pm, Pd: the grid phases' mesh-side addends)
-  // x[k] k = 0..nb, e[k] k = 1..nb (e[0] = e_lat broadcast), agg[k].  With processor segments only x[k], e[k] at the start of
-  // each segment and x[nb] are kept; agg, t_pe and t_pn stay empty.
+  // x[k] k = 0..nb, e[k] k = 0..nb (e[0]: e_lat broadcast, or a standalone processor's per-edge input), agg[k].  With processor
+  // segments only x[k], e[k] at the start of each segment and x[nb] are kept; agg, t_pe and t_pn stay empty.
   std::vector<float*> x, e, agg;
+  gw::LatGraph g;
   gw::MlpTape t_enc_node_h, t_enc_mnode, t_lat_enc;
   gw::EncTape enc;  // taped step: the grid-sized tapes (the chunked step recomputes them chunk by chunk)
   gw::DecTape dec;
@@ -109,7 +130,8 @@ struct TrainState {
   unsigned wgen = 0;          // gw_plan::wgen that wT and the weight images were made for (per-weight work runs once per upload)
   DevBuf<int32_t> lat_perm_src, lat_ptr_src, dec_perm_src, dec_ptr_src, iota;
   DevBuf<unsigned char> sort_ws;
-  bool graphs_ready = false;
+  bool pool_kept = false;   // the stream-ordered pool keeps its memory between steps
+  unsigned graphs_gen = 0;  // gw_plan::graph_gen the source-sorted graphs were built for
   // chunked step (training-only plans): chunk tables for a batch size (and, for the encoder, an encoder graph), built by the forward
   // and, when a tape of another batch size ran since, again by the backward
   int enc_chunks_batch = 0, dec_chunks_batch = 0;
@@ -437,10 +459,11 @@ static int build_chunks(gw_plan* p, TrainState* T, int batch) {
   return 0;
 }
 
-static int train_prepare(gw_plan* p, TrainState* T, int batch, cudaStream_t st) {
+// need: the stages the forward runs (check_ready's NEED_ENC / NEED_PROC / NEED_DEC)
+static int train_prepare(gw_plan* p, TrainState* T, int batch, int need, cudaStream_t st) {
   const gw_dims& d = p->d;
   GW_CHECK(d.precision == GW_PREC_FP32_SIMT || d.precision == GW_PREC_FP32_TC || d.precision == GW_PREC_BF16_TC, "unknown training precision");
-  GW_CHECK(p->w_enc && p->w_proc && p->w_dec && p->have_enc && p->have_lat && p->have_dec, "training needs the full forecaster (graphs + weights)");
+  GW_TRY(check_ready(p, batch, need));
   // the LayerNorm'd widths are node_dim and edge_dim (every other width, feature and hidden, is a plain Linear of any size)
   GW_CHECK(d.node_dim <= LN_BWD_MAX_N && d.edge_dim <= LN_BWD_MAX_N, "training kernels cover node / edge dims <= 1024 (LayerNorm backward)");
   GW_CHECK(!is_tc(p) || (d.node_dim <= 256 && d.edge_dim <= 256 && d.hidden_node <= 256 && d.hidden_edge <= 256),
@@ -470,22 +493,29 @@ static int train_prepare(gw_plan* p, TrainState* T, int batch, cudaStream_t st) 
     T->wgen = p->wgen;
   }
   if (is_tc(p) && T->bslots.n == 0) GW_TRY(T->bslots.alloc(4096));
-  if (!T->graphs_ready) {  // keep the stream-ordered pool's memory between steps (the default returns it to the driver at every sync)
+  if (!T->pool_kept) {  // keep the stream-ordered pool's memory between steps (the default returns it to the driver at every sync)
     cudaMemPool_t pool = nullptr;
     int dev = 0;
     if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
       unsigned long long keep = ~0ull;
       cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
     }
+    T->pool_kept = true;
   }
-  if (!T->graphs_ready) {  // edges grouped by SOURCE (the x[src] gathers become per-source sums going backward)
+  if (T->graphs_gen != p->graph_gen) {  // edges grouped by SOURCE (the x[src] gathers become per-source sums going backward), for
+                                        // the graphs the plan holds, rebuilt whenever an upload replaced them
     const int El = d.n_lat_edges, Ed = d.n_dec_edges, H = d.n_mesh;
     const size_t ws = std::max(sort_csr_workspace_bytes(El), sort_csr_workspace_bytes(Ed));
-    GW_TRY(T->sort_ws.alloc(ws));
-    GW_TRY(T->lat_perm_src.alloc(El) | T->lat_ptr_src.alloc(H + 1) | T->dec_perm_src.alloc(Ed) | T->dec_ptr_src.alloc(H + 1));
-    GW_CUDA(launch_sort_csr(p->lat_src.p, El, H, T->lat_perm_src.p, T->lat_ptr_src.p, T->sort_ws.p, T->sort_ws.n, st));
-    GW_CUDA(launch_sort_csr(p->dec_src.p, Ed, H, T->dec_perm_src.p, T->dec_ptr_src.p, T->sort_ws.p, T->sort_ws.n, st));
-    T->graphs_ready = true;
+    if (T->sort_ws.n < ws) GW_TRY(T->sort_ws.alloc(ws));
+    if (p->have_lat) {
+      GW_TRY(T->lat_perm_src.alloc(El) | T->lat_ptr_src.alloc(H + 1));
+      GW_CUDA(launch_sort_csr(p->lat_src.p, El, H, T->lat_perm_src.p, T->lat_ptr_src.p, T->sort_ws.p, T->sort_ws.n, st));
+    }
+    if (p->have_dec) {
+      GW_TRY(T->dec_perm_src.alloc(Ed) | T->dec_ptr_src.alloc(H + 1));
+      GW_CUDA(launch_sort_csr(p->dec_src.p, Ed, H, T->dec_perm_src.p, T->dec_ptr_src.p, T->sort_ws.p, T->sort_ws.n, st));
+    }
+    T->graphs_gen = p->graph_gen;
   }
   if (p->train_only) GW_TRY(build_chunks(p, T, batch));
   return 0;
@@ -642,12 +672,13 @@ static int dec_fwd(gw_plan* p, TrainState* T, const GridRange& r, const float* P
   const Mlp& mdo = p->dec_node_dec;
   RowSrc res;
   float* o = out;
+  const gw_tape* K = T->tp;
   if (r.whole) {
-    if (d.residual_dim > 0) res = src_stream(T->tp->features, d.in_dim, d.out_dim, No);
+    if (d.residual_dim > 0) res = src_stream(K->start, K->start_ld, d.out_dim, No);
   } else {
     if (d.residual_dim > 0) {
       GW_TALLOC(fr, (size_t)B * n * d.out_dim);
-      GW_OTHER(launch_permute_rows(T->tp->features, d.in_dim, T->iota.p + r0, n, No, d.out_dim, B, fr, d.out_dim, false, T->st));
+      GW_OTHER(launch_permute_rows(K->start, K->start_ld, T->iota.p + r0, n, No, d.out_dim, B, fr, d.out_dim, false, T->st));
       res = src_stream(fr, d.out_dim, d.out_dim, n);
     }
     GW_TALLOC(oc, (size_t)B * n * d.out_dim);
@@ -713,17 +744,20 @@ static int dec_bwd(gw_plan* p, TrainState* T, const GridRange& r, const DecTape&
 // ---------------------------------------------------------------------------------------------------------------------------
 // one processor block (the taped forward, the segmented forward and the segments' recompute in the backward all run these)
 // ---------------------------------------------------------------------------------------------------------------------------
-// the block's edge input e[k]: e_lat broadcast over the batch in block 0
+// the block's edge input e[k]: in block 0 of the whole network, e_lat broadcast over the batch
 static RowSrc block_edge_src(TrainState* T, int k, const float* ek, int De, int El) {
-  return k == 0 ? src_bcast(T->tp->e_lat, De, De) : src_stream(ek, De, De, El);
+  return (k == 0 && T->tp->g.e0_bcast) ? src_bcast(ek, De, De) : src_stream(ek, De, De, El);
 }
 
-// block k from x[k] (xk) and e[k] (ek; block 0 reads e_lat): P [B, H, 2 He] is the caller's scratch for the factored layer 1's node
-// terms.  Allocates e[k+1], agg[k] and x[k+1], in that order, on the running tape; tpe / tpn receive the edge and node MLP tapes.
+// block k from x[k] (xk) and e[k] (ek), on the running tape's graph: P [B, H, 2 He] is the caller's scratch for the factored layer
+// 1's node terms.  Allocates e[k+1], agg[k] and x[k+1], in that order, on the running tape; tpe / tpn receive the edge and node MLP
+// tapes.  Block 0 of a standalone processor reads the caller's rows, and bounds them (train_op's reads_input).
 static int block_fwd(gw_plan* p, TrainState* T, int k, const float* xk, const float* ek, float* P, float** en_out, float** ag_out, float** xn_out,
                      MlpTape* tpe, MlpTape* tpn) {
   const gw_dims& d = p->d;
-  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, H = d.n_mesh, El = d.n_lat_edges, B = T->tp->batch;
+  const LatGraph& g = T->tp->g;
+  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, H = g.H, El = g.El, B = T->tp->batch;
+  const bool in = k == 0 && T->tp->caller_input;
   RowSrc none;
   const Mlp& me = p->proc_edge[k];
   const Mlp& mn = p->proc_node[k];
@@ -731,21 +765,21 @@ static int block_fwd(gw_plan* p, TrainState* T, int k, const float* xk, const fl
     GemmOp t;
     t.rows_per_sample = H, t.batch = B, t.a[0] = src_stream(xk, Dn, Dn, H), t.W = me.W[0] + h * Dn, t.K = Dn, t.ldw = me.in[0], t.N = He;
     t.out = P + h * He, t.ldo = 2 * He;
-    GW_TRY(train_op(p, T, t, TAG_TRAIN_FWD));
+    GW_TRY(train_op(p, T, t, TAG_TRAIN_FWD, in));
   }
   const RowSrc e_src = block_edge_src(T, k, ek, De, El);
   GW_TALLOC(en, (size_t)B * El * De);
   {
     GemmOp fo = first_op(El, B, e_src, none, me.W[0] + 2 * Dn, De, me.in[0], me.b[0]);
-    fo.add[0] = src_gather(P, 2 * He, He, p->lat_src.p, H, 0);
-    fo.add[1] = src_gather(P, 2 * He, He, p->lat_dst.p, H, He);
-    GW_TRY(mlp_fwd(p, T, me, fo, e_src, en, De, tpe));
+    fo.add[0] = src_gather(P, 2 * He, He, g.src, H, 0);
+    fo.add[1] = src_gather(P, 2 * He, He, g.dst, H, He);
+    GW_TRY(mlp_fwd(p, T, me, fo, e_src, en, De, tpe, in));
   }
   GW_TALLOC(ag, (size_t)B * H * De);
-  GW_OTHER(launch_segsum(en, De, De, p->lat_ptr.p, nullptr, El, H, B, ag, De, T->st));
+  GW_OTHER(launch_segsum(en, De, De, g.ptr, nullptr, El, H, B, ag, De, T->st));
   GW_TALLOC(xn, (size_t)B * H * Dn);
   GW_TRY(mlp_fwd(p, T, mn, first_op(H, B, src_stream(xk, Dn, Dn, H), src_stream(ag, De, De, H), mn.W[0], mn.in[0], mn.in[0], mn.b[0]),
-                 src_stream(xk, Dn, Dn, H), xn, Dn, tpn));
+                 src_stream(xk, Dn, Dn, H), xn, Dn, tpn, in));
   *en_out = en, *ag_out = ag, *xn_out = xn;
   return 0;
 }
@@ -755,7 +789,8 @@ static int block_fwd(gw_plan* p, TrainState* T, int k, const float* xk, const fl
 static int block_bwd(gw_plan* p, TrainState* T, int k, const float* xk, const float* ek, const float* agg, const MlpTape& tpe, const MlpTape& tpn,
                      const float* dx, const float* de, float** dx_out, float** de_out) {
   const gw_dims& d = p->d;
-  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, H = d.n_mesh, El = d.n_lat_edges, B = T->tp->batch;
+  const LatGraph& g = T->tp->g;
+  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, H = g.H, El = g.El, B = T->tp->batch;
   const cudaStream_t st = T->st;
   const Mlp& me = p->proc_edge[k];
   const Mlp& mn = p->proc_node[k];
@@ -772,9 +807,9 @@ static int block_bwd(gw_plan* p, TrainState* T, int k, const float* xk, const fl
   GW_TALLOC(d_en, (size_t)B * El * De);
   if (de) {
     GW_CUDA(cudaMemcpyAsync(d_en, de, (size_t)B * El * De * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    GW_OTHER(launch_gather_rows(d_agg, De, H, p->lat_dst.p, El, De, B, d_en, De, true, st));
+    GW_OTHER(launch_gather_rows(d_agg, De, H, g.dst, El, De, B, d_en, De, true, st));
   } else {
-    GW_OTHER(launch_gather_rows(d_agg, De, H, p->lat_dst.p, El, De, B, d_en, De, false, st));
+    GW_OTHER(launch_gather_rows(d_agg, De, H, g.dst, El, De, B, d_en, De, false, st));
   }
   // edge MLP: e[k+1] = LN(...) + e[k];  h1 = relu(e[k] W1e^T + P_s[src] + P_d[dst] + b1)
   GW_TRY(mlp_bwd(p, T, me, tpe, d_en, De, &dh));
@@ -784,8 +819,8 @@ static int block_bwd(gw_plan* p, TrainState* T, int k, const float* xk, const fl
   GW_TRY(dgrad(p, T, dh, He, He, El, B, me.W[0], me.out[0], 2 * Dn, De, nullptr, 0, d_en, De, d_ek, De));  // + residual path
   GW_TALLOC(dPs, (size_t)B * H * He);
   GW_TALLOC(dPt, (size_t)B * H * He);
-  GW_OTHER(launch_segsum(dh, He, He, T->lat_ptr_src.p, T->lat_perm_src.p, El, H, B, dPs, He, st));
-  GW_OTHER(launch_segsum(dh, He, He, p->lat_ptr.p, nullptr, El, H, B, dPt, He, st));
+  GW_OTHER(launch_segsum(dh, He, He, g.ptr_src, g.perm_src, El, H, B, dPs, He, st));
+  GW_OTHER(launch_segsum(dh, He, He, g.ptr, nullptr, El, H, B, dPt, He, st));
   GW_TRY(train_wgrad(p, T, dPs, He, He, src_stream(xk, Dn, Dn, H), Dn, H, B, grad_of(p, T, me.W[0]), me.in[0], nullptr));
   GW_TRY(train_wgrad(p, T, dPt, He, He, src_stream(xk, Dn, Dn, H), Dn, H, B, grad_of(p, T, me.W[0]) + Dn, me.in[0], nullptr));
   GW_TALLOC(dx1, (size_t)B * H * Dn);
@@ -804,9 +839,9 @@ static int segment_blocks(int segments, int nb) { return (segments < 0 || segmen
 // as soon as the block has run
 static int proc_fwd_segmented(gw_plan* p, TrainState* T, gw_tape* K) {
   const gw_dims& d = p->d;
-  const int He = d.hidden_edge, H = d.n_mesh, nb = d.num_blocks, B = K->batch, S = segment_blocks(K->segments, nb);
+  const int He = d.hidden_edge, H = K->g.H, nb = d.num_blocks, B = K->batch, S = segment_blocks(K->segments, nb);
   GW_TALLOC(P, (size_t)B * H * 2 * He);
-  float *x = K->x[0], *e = nullptr;
+  float *x = K->x[0], *e = K->e[0];
   for (int k = 0; k < nb; ++k) {
     const size_t mark = K->allocs.size();
     float *en = nullptr, *ag = nullptr, *xn = nullptr;
@@ -830,7 +865,7 @@ static int proc_fwd_segmented(gw_plan* p, TrainState* T, gw_tape* K) {
 // x[0] out; de: gradient of e[0] out.
 static int proc_bwd_segmented(gw_plan* p, TrainState* T, gw_tape* K, float** dx, float** de) {
   const gw_dims& d = p->d;
-  const int He = d.hidden_edge, H = d.n_mesh, nb = d.num_blocks, B = K->batch, S = segment_blocks(K->segments, nb);
+  const int He = d.hidden_edge, H = K->g.H, nb = d.num_blocks, B = K->batch, S = segment_blocks(K->segments, nb);
   float *gx = *dx, *ge = nullptr;
   for (int k1 = nb; k1 > 0;) {
     const int k0 = (k1 - 1) / S * S, n = k1 - k0;
@@ -863,20 +898,36 @@ static int proc_bwd_segmented(gw_plan* p, TrainState* T, gw_tape* K, float** dx,
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// forward (keeps activations; the chunked step keeps only the mesh-sized ones, the agg_m rows and the output)
+// the three stages of the step.  The whole network's forward and backward are their composition; each stage also runs alone, on a
+// tape of its own, for the reference's standalone Encoder / Processor / Decoder (gw_train_{encoder,processor,decoder}_*_tape).
+// A stage's forward keeps its activations on the running tape; the chunked step (training-only plans) keeps only the mesh-sized
+// ones, the agg_m rows and the output.
 // ---------------------------------------------------------------------------------------------------------------------------
-static int train_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* features, float* out, int B, cudaStream_t st) {
-  const gw_dims& d = p->d;
-  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, H = d.n_mesh, El = d.n_lat_edges, nb = d.num_blocks;
-  tape_release(T, K, st);  // a second forward on a tape replaces the first's activations
+// the start of a forward on tape K: its previous activations released (a second forward on a tape replaces the first's), the
+// training state ready for the stages in `need`, the tape's processor on the plan's latent graph
+static int forward_begin(gw_plan* p, TrainState* T, gw_tape* K, int stage, int need, int B, cudaStream_t st) {
+  tape_release(T, K, st);
   if (T->cur_bytes == 0) T->peak_bytes = 0;  // no other tape holds memory: the high-water mark starts over
   T->tp = K;
-  GW_TRY(train_prepare(p, T, B, st));
+  GW_TRY(train_prepare(p, T, B, need, st));
   GW_TRY(reset_bounds(T));
+  K->batch = B, K->wgen = p->wgen, K->segments = p->train_segments, K->stage = stage, K->enc_gen = p->enc_graph_gen;
+  K->features = nullptr, K->start = nullptr, K->start_ld = 0, K->xd = nullptr, K->caller_input = false;
+  K->g = LatGraph();
+  if (p->have_lat) {
+    K->g.H = p->d.n_mesh, K->g.El = p->d.n_lat_edges;
+    K->g.src = p->lat_src.p, K->g.dst = p->lat_dst.p, K->g.ptr = p->lat_ptr.p, K->g.perm_src = T->lat_perm_src.p, K->g.ptr_src = T->lat_ptr_src.p;
+  }
+  return 0;
+}
+
+// encoder: the features (K->features) -> x[0] [B, H, Dn] (*x0_out, on the tape) and e_lat [El, De] (K->e_lat: one sample's latent
+// edge features, shared by the batch)
+static int enc_stage_fwd(gw_plan* p, TrainState* T, gw_tape* K, float** x0_out) {
+  const gw_dims& d = p->d;
+  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, H = d.n_mesh, El = d.n_lat_edges, B = K->batch;
   RowSrc none;
-  K->features = features, K->batch = B, K->wgen = p->wgen, K->segments = p->train_segments;
   const bool chunked = p->train_only;
-  // ---- encoder ------------------------------------------------------------------------------------------------------------
   // mesh rows: xm0 = node_encoder(h3_nodes), Pm = xm0 W1d^T (the mesh end of every encoder edge)
   const Mlp& mne = p->enc_node;
   GW_TALLOC(xm0, (size_t)H * Dn);
@@ -902,18 +953,25 @@ static int train_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* fea
     }
   }
   const Mlp& mnb = p->enc_blk_node;
-  K->x.assign(nb + 1, nullptr), K->e.assign(nb + 1, nullptr), K->agg.assign(nb, nullptr);
-  K->t_pe.assign(nb, MlpTape()), K->t_pn.assign(nb, MlpTape());
   GW_TALLOC(x0, (size_t)B * H * Dn);
   GW_TRY(mlp_fwd(p, T, mnb, first_op(H, B, src_bcast(xm0, Dn, Dn), src_stream(agg_m, De, De, H), mnb.W[0], mnb.in[0], mnb.in[0], mnb.b[0]),
                  src_bcast(xm0, Dn, Dn), x0, Dn, &K->t_enc_mnode));
-  K->x[0] = x0;
   const Mlp& mle = p->enc_lat_edge_enc;
   GW_TALLOC(e_lat, (size_t)El * De);
   GW_TRY(mlp_fwd(p, T, mle, first_op(El, 1, src_stream(p->lat_attr.p, 2, 2, El), none, mle.W[0], mle.in[0], mle.in[0], mle.b[0]), none, e_lat, De,
                  &K->t_lat_enc));
   K->xm0 = xm0, K->agg_m = agg_m, K->e_lat = e_lat, K->Pm = Pm;
-  // ---- processor ----------------------------------------------------------------------------------------------------------
+  *x0_out = x0;
+  return 0;
+}
+
+// processor: x[0] [B, H, Dn] and e[0] (e_lat broadcast over the batch, or [B, El, De] per edge: K->g.e0_bcast) -> x[nb] (K->x[nb],
+// on the tape), on the tape's graph K->g.  x0 and e0 stay the caller's: the backward reads them again.
+static int proc_stage_fwd(gw_plan* p, TrainState* T, gw_tape* K, const float* x0, const float* e0) {
+  const int He = p->d.hidden_edge, H = K->g.H, nb = p->d.num_blocks, B = K->batch;
+  K->x.assign(nb + 1, nullptr), K->e.assign(nb + 1, nullptr), K->agg.assign(nb, nullptr);
+  K->t_pe.assign(nb, MlpTape()), K->t_pn.assign(nb, MlpTape());
+  K->x[0] = const_cast<float*>(x0), K->e[0] = const_cast<float*>(e0);
   if (K->segments == 0) {
     GW_TALLOC(P, (size_t)B * H * 2 * He);
     for (int k = 0; k < nb; ++k)
@@ -922,16 +980,23 @@ static int train_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* fea
     K->agg.clear(), K->t_pe.clear(), K->t_pn.clear();
     GW_TRY(proc_fwd_segmented(p, T, K));
   }
-  // ---- decoder ------------------------------------------------------------------------------------------------------------
+  return 0;
+}
+
+// decoder: x [B, H, Dn] (K->xd, read again by the backward) -> out [B, n_out, out_dim] (+ the first out_dim columns of K->start
+// when the plan has a residual)
+static int dec_stage_fwd(gw_plan* p, TrainState* T, gw_tape* K, float* out) {
+  const gw_dims& d = p->d;
+  const int Dn = d.node_dim, He = d.hidden_edge, H = d.n_mesh, B = K->batch;
   const Mlp& mdb = p->dec_blk_edge;
   GW_TALLOC(Pd, (size_t)B * H * He);
   {
     GemmOp t;
-    t.rows_per_sample = H, t.batch = B, t.a[0] = src_stream(K->x[nb], Dn, Dn, H), t.W = mdb.W[0], t.K = Dn, t.ldw = mdb.in[0], t.N = He, t.out = Pd, t.ldo = He;
-    GW_TRY(train_op(p, T, t, TAG_TRAIN_FWD));
+    t.rows_per_sample = H, t.batch = B, t.a[0] = src_stream(K->xd, Dn, Dn, H), t.W = mdb.W[0], t.K = Dn, t.ldw = mdb.in[0], t.N = He, t.out = Pd, t.ldo = He;
+    GW_TRY(train_op(p, T, t, TAG_TRAIN_FWD, K->caller_input));
   }
   K->Pd = Pd;
-  if (!chunked) {
+  if (!p->train_only) {
     GW_TRY(dec_fwd(p, T, GridRange(), Pd, out, &K->dec));
   } else {
     for (const GridRange& r : T->dec_chunks) {
@@ -942,30 +1007,47 @@ static int train_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* fea
       tfree_to(T, mark);
     }
   }
+  return 0;
+}
+
+// the whole network: encoder -> processor (block 0 reads e_lat broadcast) -> decoder with the features as the residual
+static int train_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* features, float* out, int B, cudaStream_t st) {
+  GW_TRY(forward_begin(p, T, K, TAPE_NET, NEED_ENC | NEED_PROC | NEED_DEC, B, st));
+  K->features = features, K->start = features, K->start_ld = p->d.in_dim;
+  float* x0 = nullptr;
+  GW_TRY(enc_stage_fwd(p, T, K, &x0));
+  GW_TRY(proc_stage_fwd(p, T, K, x0, K->e_lat));
+  K->xd = K->x[p->d.num_blocks];
+  GW_TRY(dec_stage_fwd(p, T, K, out));
   K->have_tape = true;
   return 0;
 }
 
-// ---------------------------------------------------------------------------------------------------------------------------
-// backward
-// ---------------------------------------------------------------------------------------------------------------------------
-static int train_backward(gw_plan* p, TrainState* T, gw_tape* K, const float* dOut, float* dFeatures, cudaStream_t st) {
-  const gw_dims& d = p->d;
-  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, N = p->n_in_cur, H = d.n_mesh, El = d.n_lat_edges, nb = d.num_blocks, B = K->batch;
-  GW_CHECK(K->have_tape, "gw_train_backward_tape needs the activations of a preceding gw_train_forward_tape (one backward per forward)");
+// the start of a backward on tape K: it holds the activations of a forward of `stage`, taken at the plan's current weights (and,
+// for a standalone encoder, on its current encoder graph); the gradient buffer is cleared
+static int backward_begin(gw_plan* p, TrainState* T, gw_tape* K, int stage, cudaStream_t st) {
+  GW_CHECK(K->have_tape, "a training backward needs the activations of a preceding training forward on its tape (one backward per forward)");
+  GW_CHECK(K->stage == stage, "this tape holds the activations of another kind of training forward (the whole network or another stage)");
   GW_CHECK(K->wgen == p->wgen, "training backward: the plan's weights were replaced (gw_plan_set_weights) after this tape's forward; "
                                "its gradient would be taken at other weights");
+  GW_CHECK(stage != TAPE_ENC || K->enc_gen == p->enc_graph_gen,
+           "encoder backward: the plan's encoder graph was replaced after this tape's forward; its gradient would be taken on another graph");
   T->st = st;
   T->tp = K;
-  if (p->train_only) GW_TRY(build_chunks(p, T, B));  // (a tape of another batch size may have run since this one's forward)
+  if (p->train_only) GW_TRY(build_chunks(p, T, K->batch));  // (a tape of another batch size may have run since this one's forward)
   GW_TRY(reset_bounds(T));
   GW_CUDA(cudaMemsetAsync(T->gbuf.p, 0, T->gbuf.bytes(), st));
-  if (dFeatures) GW_CUDA(cudaMemsetAsync(dFeatures, 0, (size_t)B * N * d.in_dim * sizeof(float), st));
-  const bool chunked = p->train_only;
-  float* dh = nullptr;
-  // ---- decoder: lat/lon side, then the mesh end of its edges (dPd: gradient of Pd = x[nb] W1s^T) ---------------------------------
+  return 0;
+}
+
+// decoder backward: dOut [B, n_out, out_dim] -> its weight gradients and the gradient of its input x (*dx_out [B, H, Dn], on the
+// tape).  The residual's share of the start features' gradient is dOut itself, added by the caller.
+static int dec_stage_bwd(gw_plan* p, TrainState* T, gw_tape* K, const float* dOut, float** dx_out) {
+  const gw_dims& d = p->d;
+  const int Dn = d.node_dim, He = d.hidden_edge, H = d.n_mesh, B = K->batch;
+  // lat/lon side, then the mesh end of its edges (dPd: gradient of Pd = x W1s^T)
   GW_TALLOC(dPd, (size_t)B * H * He);
-  if (!chunked) {
+  if (!p->train_only) {
     GW_TRY(dec_bwd(p, T, GridRange(), K->dec, dOut, dPd));
   } else {
     for (const GridRange& r : T->dec_chunks) {
@@ -978,23 +1060,39 @@ static int train_backward(gw_plan* p, TrainState* T, gw_tape* K, const float* dO
     }
   }
   const Mlp& mdb = p->dec_blk_edge;
-  GW_TRY(train_wgrad(p, T, dPd, He, He, src_stream(K->x[nb], Dn, Dn, H), Dn, H, B, grad_of(p, T, mdb.W[0]), mdb.in[0], nullptr));
-  GW_TALLOC(dx_last, (size_t)B * H * Dn);
-  GW_TRY(dgrad(p, T, dPd, He, He, H, B, mdb.W[0], mdb.out[0], 0, Dn, nullptr, 0, nullptr, 0, dx_last, Dn));
-  float* dx = dx_last;  // gradient of x[nb]
-  // ---- processor blocks, last to first ------------------------------------------------------------------------------------------
-  float* de = nullptr;  // gradient of e[k+1] (none flows into the last block's e')
+  GW_TRY(train_wgrad(p, T, dPd, He, He, src_stream(K->xd, Dn, Dn, H), Dn, H, B, grad_of(p, T, mdb.W[0]), mdb.in[0], nullptr));
+  GW_TALLOC(dx, (size_t)B * H * Dn);
+  GW_TRY(dgrad(p, T, dPd, He, He, H, B, mdb.W[0], mdb.out[0], 0, Dn, nullptr, 0, nullptr, 0, dx, Dn));
+  *dx_out = dx;
+  return 0;
+}
+
+// processor backward, blocks last to first: dx (the gradient of x[nb]) -> its weight gradients and the gradients of x[0] (*dx0)
+// and of e[0] (*de0, per sample and edge [B, El, De]), on the tape
+static int proc_stage_bwd(gw_plan* p, TrainState* T, gw_tape* K, const float* dx_in, float** dx0, float** de0) {
+  float* dx = const_cast<float*>(dx_in);  // (read only; the segmented backward releases it when it is the tape's)
+  float* de = nullptr;                    // gradient of e[k+1] (none flows into the last block's e')
   if (K->segments == 0) {
-    for (int k = nb - 1; k >= 0; --k)
+    for (int k = p->d.num_blocks - 1; k >= 0; --k)
       GW_TRY(block_bwd(p, T, k, K->x[k], K->e[k], K->agg[k], K->t_pe[k], K->t_pn[k], dx, de, &dx, &de));
   } else {
     GW_TRY(proc_bwd_segmented(p, T, K, &dx, &de));
   }
-  // e[0] = e_lat broadcast: reduce over the batch, back through latent_edge_encoder
-  {
+  *dx0 = dx, *de0 = de;
+  return 0;
+}
+
+// encoder backward: the gradients of x[0] (dx0 [B, H, Dn]) and of e_lat (d_elat [El, De], summed over the batch; null: none) ->
+// its weight gradients and, if dFeatures is not null, the gradient of the features [B, n_in, in_dim]
+static int enc_stage_bwd(gw_plan* p, TrainState* T, gw_tape* K, const float* dx0, const float* d_elat, float* dFeatures) {
+  const gw_dims& d = p->d;
+  const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, N = p->n_in_cur, H = d.n_mesh, El = d.n_lat_edges, B = K->batch;
+  const cudaStream_t st = T->st;
+  const bool chunked = p->train_only;
+  if (dFeatures) GW_CUDA(cudaMemsetAsync(dFeatures, 0, (size_t)B * N * d.in_dim * sizeof(float), st));
+  float* dh = nullptr;
+  if (d_elat) {  // back through latent_edge_encoder
     const Mlp& mle = p->enc_lat_edge_enc;
-    GW_TALLOC(d_elat, (size_t)El * De);
-    GW_OTHER(launch_batch_reduce(de, De, El, De, B, d_elat, De, false, st));
     float* g0 = nullptr;
     GW_TRY(mlp_bwd(p, T, mle, K->t_lat_enc, d_elat, De, &g0));
     GW_TRY(train_wgrad(p, T, g0, mle.out[0], mle.out[0], src_stream(p->lat_attr.p, 2, 2, El), 2, El, 1, grad_of(p, T, mle.W[0]), mle.in[0], grad_of(p, T, mle.b[0])));
@@ -1002,8 +1100,8 @@ static int train_backward(gw_plan* p, TrainState* T, gw_tape* K, const float* dO
   // ---- encoder block, node MLP (mesh rows): x[0] = LN(MLP([xm0 ; agg_m])) + xm0 ------------------------------------------------
   const Mlp& mnb = p->enc_blk_node;
   GW_TALLOC(d_xm0, (size_t)H * Dn);
-  GW_OTHER(launch_batch_reduce(dx, Dn, H, Dn, B, d_xm0, Dn, false, st));  // residual: xm0 is shared by the batch
-  GW_TRY(mlp_bwd(p, T, mnb, K->t_enc_mnode, dx, Dn, &dh));
+  GW_OTHER(launch_batch_reduce(dx0, Dn, H, Dn, B, d_xm0, Dn, false, st));  // residual: xm0 is shared by the batch
+  GW_TRY(mlp_bwd(p, T, mnb, K->t_enc_mnode, dx0, Dn, &dh));
   GW_TRY(train_wgrad(p, T, dh, mnb.out[0], mnb.out[0], src_bcast(K->xm0, Dn, Dn), Dn, H, B, grad_of(p, T, mnb.W[0]), mnb.in[0], grad_of(p, T, mnb.b[0])));
   GW_TRY(train_wgrad(p, T, dh, mnb.out[0], mnb.out[0], src_stream(K->agg_m, De, De, H), De, H, B, grad_of(p, T, mnb.W[0]) + Dn, mnb.in[0], nullptr));
   {
@@ -1044,9 +1142,110 @@ static int train_backward(gw_plan* p, TrainState* T, gw_tape* K, const float* dO
                    grad_of(p, T, p->h3_nodes), d.in_dim));
   }
   if (!chunked) GW_TRY(enc_node_bwd(p, T, GridRange(), K->enc, d_xg, dFeatures));
+  return 0;
+}
+
+// the whole network's backward: decoder, processor, then the encoder with e[0]'s gradient summed over the batch (e_lat is
+// broadcast), and the residual's share of the features' gradient
+static int train_backward(gw_plan* p, TrainState* T, gw_tape* K, const float* dOut, float* dFeatures, cudaStream_t st) {
+  const gw_dims& d = p->d;
+  const int De = d.edge_dim, N = p->n_in_cur, El = d.n_lat_edges, B = K->batch;
+  GW_TRY(backward_begin(p, T, K, TAPE_NET, st));
+  float *dx = nullptr, *dx0 = nullptr, *de0 = nullptr;
+  GW_TRY(dec_stage_bwd(p, T, K, dOut, &dx));
+  GW_TRY(proc_stage_bwd(p, T, K, dx, &dx0, &de0));
+  GW_TALLOC(d_elat, (size_t)El * De);
+  GW_OTHER(launch_batch_reduce(de0, De, El, De, B, d_elat, De, false, st));
+  GW_TRY(enc_stage_bwd(p, T, K, dx0, d_elat, dFeatures));
   if (dFeatures && d.residual_dim > 0)  // out = node_decoder(...) + features[..., :out]: the residual passes dOut straight through
     GW_OTHER(launch_strided_add(dOut, d.out_dim, dFeatures, d.in_dim, (long long)B * N, d.out_dim, st));
   tape_release(T, K, st);  // the backward consumes its tape
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// one stage alone (the reference's sub-modules, each trained on its own tape)
+// ---------------------------------------------------------------------------------------------------------------------------
+static int copy_rows(float* dst, const float* src, size_t floats, cudaStream_t st) {
+  GW_CUDA(cudaMemcpyAsync(dst, src, floats * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+static int encoder_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* features, float* x_out, float* e_lat_out, int B, cudaStream_t st) {
+  const gw_dims& d = p->d;
+  GW_TRY(forward_begin(p, T, K, TAPE_ENC, NEED_ENC, B, st));
+  K->features = features;
+  float* x0 = nullptr;
+  GW_TRY(enc_stage_fwd(p, T, K, &x0));
+  GW_TRY(copy_rows(x_out, x0, (size_t)B * d.n_mesh * d.node_dim, st));
+  GW_TRY(copy_rows(e_lat_out, K->e_lat, (size_t)d.n_lat_edges * d.edge_dim, st));
+  tfree_one(T, x0), tfree_one(T, K->e_lat);  // (the encoder's backward reads neither)
+  K->e_lat = nullptr;
+  K->have_tape = true;
+  return 0;
+}
+
+static int encoder_backward(gw_plan* p, TrainState* T, gw_tape* K, const float* dx, const float* d_elat, float* dFeatures, cudaStream_t st) {
+  GW_TRY(backward_begin(p, T, K, TAPE_ENC, st));
+  GW_TRY(enc_stage_bwd(p, T, K, dx, d_elat, dFeatures));
+  tape_release(T, K, st);
+  return 0;
+}
+
+// the caller's graph is copied onto the tape, with its edges grouped by source: it may change from call to call, and several
+// tapes may hold forwards on different graphs
+static int processor_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* x_in, float* x_out, const float* edge_attr, int n_nodes, int n_edges,
+                             const int32_t* src, const int32_t* dst, const int32_t* ptr, cudaStream_t st) {
+  const gw_dims& d = p->d;
+  GW_TRY(forward_begin(p, T, K, TAPE_PROC, NEED_PROC, 1, st));
+  const size_t E = n_edges, V = (size_t)n_nodes + 1;
+  float* gbuf = talloc(T, 3 * E + 2 * V);
+  GW_CHECK(gbuf != nullptr, "training step: out of device memory");
+  int32_t* s = reinterpret_cast<int32_t*>(gbuf);
+  int32_t *t = s + E, *pt = t + E, *perm = pt + V, *ps = perm + E;
+  GW_CUDA(cudaMemcpyAsync(s, src, E * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  GW_CUDA(cudaMemcpyAsync(t, dst, E * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  GW_CUDA(cudaMemcpyAsync(pt, ptr, V * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  const size_t ws = sort_csr_workspace_bytes(n_edges);
+  if (T->sort_ws.n < ws) GW_TRY(T->sort_ws.alloc(ws));
+  GW_CUDA(launch_sort_csr(s, n_edges, n_nodes, perm, ps, T->sort_ws.p, T->sort_ws.n, st));
+  K->g.H = n_nodes, K->g.El = n_edges, K->g.src = s, K->g.dst = t, K->g.ptr = pt, K->g.perm_src = perm, K->g.ptr_src = ps, K->g.e0_bcast = false;
+  K->caller_input = true;
+  GW_TRY(proc_stage_fwd(p, T, K, x_in, edge_attr));
+  float* xo = K->x[d.num_blocks];
+  GW_TRY(copy_rows(x_out, xo, (size_t)n_nodes * d.node_dim, st));
+  tfree_one(T, xo);  // (no block's backward reads the output)
+  K->x[d.num_blocks] = nullptr;
+  K->have_tape = true;
+  return 0;
+}
+
+static int processor_backward(gw_plan* p, TrainState* T, gw_tape* K, const float* grad_x_out, float* grad_x_in, float* grad_edge_attr, cudaStream_t st) {
+  const gw_dims& d = p->d;
+  GW_TRY(backward_begin(p, T, K, TAPE_PROC, st));
+  float *dx0 = nullptr, *de0 = nullptr;
+  GW_TRY(proc_stage_bwd(p, T, K, grad_x_out, &dx0, &de0));
+  if (grad_x_in) GW_TRY(copy_rows(grad_x_in, dx0, (size_t)K->g.H * d.node_dim, st));
+  if (grad_edge_attr) GW_TRY(copy_rows(grad_edge_attr, de0, (size_t)K->g.El * d.edge_dim, st));
+  tape_release(T, K, st);
+  return 0;
+}
+
+static int decoder_forward(gw_plan* p, TrainState* T, gw_tape* K, const float* x_in, const float* start, int start_ld, float* out, int B, cudaStream_t st) {
+  GW_TRY(forward_begin(p, T, K, TAPE_DEC, NEED_DEC, B, st));
+  K->xd = x_in, K->start = start, K->start_ld = start_ld, K->caller_input = true;
+  GW_TRY(dec_stage_fwd(p, T, K, out));
+  K->have_tape = true;
+  return 0;
+}
+
+static int decoder_backward(gw_plan* p, TrainState* T, gw_tape* K, const float* grad_out, float* grad_x_in, cudaStream_t st) {
+  const gw_dims& d = p->d;
+  GW_TRY(backward_begin(p, T, K, TAPE_DEC, st));
+  float* dx = nullptr;
+  GW_TRY(dec_stage_bwd(p, T, K, grad_out, &dx));
+  if (grad_x_in) GW_TRY(copy_rows(grad_x_in, dx, (size_t)K->batch * d.n_mesh * d.node_dim, st));
+  tape_release(T, K, st);
   return 0;
 }
 
@@ -1106,22 +1305,97 @@ int gw_train_forward_tape(gw_plan* p, gw_tape* k, const float* features, float* 
   return rc;
 }
 
+// gradients are handed out under the reference's parameter names, shaped like the parameters
+static int hand_out_grads(gw_plan* p, const gw_param* grads, int32_t n, const char* what, cudaStream_t st) {
+  for (int i = 0; i < n; ++i) {
+    GW_CHECK(grads[i].name && grads[i].data, "malformed gw_param entry");
+    auto it = p->params.find(grads[i].name);
+    GW_CHECK(it != p->params.end(), std::string(what) + ": unknown parameter '" + grads[i].name + "'");
+    const size_t cnt = (size_t)it->second.second.first * it->second.second.second;
+    GW_CHECK((size_t)grads[i].rows * grads[i].cols == cnt, std::string(what) + ": shape of '" + grads[i].name + "' differs");
+    GW_CUDA(cudaMemcpyAsync(const_cast<float*>(grads[i].data), p->train->gbuf.p + (it->second.first - p->wbuf.p), cnt * sizeof(float),
+                            cudaMemcpyDeviceToDevice, st));
+  }
+  return 0;
+}
+
 int gw_train_backward_tape(gw_plan* p, gw_tape* k, const float* grad_out, float* grad_features, const gw_param* grads, int32_t n, void* stream) {
   GW_TRY(check_tape(p, k));
   GW_CHECK(grad_out && (n == 0 || grads), "null argument");
   GW_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
   GW_TRY(gw::train_backward(p, p->train, k, grad_out, grad_features, st));
-  for (int i = 0; i < n; ++i) {  // gradients are handed out under the reference's parameter names, shaped like the parameters
-    GW_CHECK(grads[i].name && grads[i].data, "malformed gw_param entry");
-    auto it = p->params.find(grads[i].name);
-    GW_CHECK(it != p->params.end(), std::string("gw_train_backward_tape: unknown parameter '") + grads[i].name + "'");
-    const size_t cnt = (size_t)it->second.second.first * it->second.second.second;
-    GW_CHECK((size_t)grads[i].rows * grads[i].cols == cnt, std::string("gw_train_backward_tape: shape of '") + grads[i].name + "' differs");
-    GW_CUDA(cudaMemcpyAsync(const_cast<float*>(grads[i].data), p->train->gbuf.p + (it->second.first - p->wbuf.p), cnt * sizeof(float),
-                            cudaMemcpyDeviceToDevice, st));
-  }
-  return 0;
+  return hand_out_grads(p, grads, n, "gw_train_backward_tape", st);
+}
+
+// the stages alone: the taped step of a gw_plan_create plan
+static const char* const kStagePlan = "the stage training calls run the taped step: they need a gw_plan_create plan, not a training-only one";
+
+int gw_train_encoder_forward_tape(gw_plan* p, gw_tape* k, const float* features, float* x_out, float* e_lat_out, int32_t batch, void* stream) {
+  GW_TRY(check_tape(p, k));
+  GW_TRY(gw::check_ready(p, batch, gw::NEED_ENC));
+  GW_CHECK(features && x_out && e_lat_out, "null argument");
+  GW_CHECK(!p->train_only, kStagePlan);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rc = gw::encoder_forward(p, p->train, k, features, x_out, e_lat_out, batch, st);
+  if (rc) gw::tape_release(p->train, k, st);
+  return rc;
+}
+
+int gw_train_encoder_backward_tape(gw_plan* p, gw_tape* k, const float* grad_x, const float* grad_e_lat, float* grad_features, const gw_param* grads,
+                                   int32_t n, void* stream) {
+  GW_TRY(check_tape(p, k));
+  GW_CHECK(grad_x && (n == 0 || grads), "null argument");
+  GW_CUDA(cudaSetDevice(p->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  GW_TRY(gw::encoder_backward(p, p->train, k, grad_x, grad_e_lat, grad_features, st));
+  return hand_out_grads(p, grads, n, "gw_train_encoder_backward_tape", st);
+}
+
+int gw_train_processor_forward_tape(gw_plan* p, gw_tape* k, const float* x_in, float* x_out, const float* edge_attr, int32_t n_nodes, int32_t n_edges,
+                                    const int32_t* src, const int32_t* dst, const int32_t* ptr, void* stream) {
+  GW_TRY(check_tape(p, k));
+  GW_TRY(gw::check_ready(p, 1, gw::NEED_PROC));
+  GW_CHECK(x_in && x_out && edge_attr && src && dst && ptr, "null argument");
+  GW_CHECK(x_out != x_in, "the training forward reads x_in again in its backward: x_out must be another buffer");
+  GW_CHECK(!p->train_only, kStagePlan);
+  GW_CHECK(n_nodes >= 1 && n_edges >= 1, "the graph needs at least one node and one edge");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rc = gw::processor_forward(p, p->train, k, x_in, x_out, edge_attr, n_nodes, n_edges, src, dst, ptr, st);
+  if (rc) gw::tape_release(p->train, k, st);
+  return rc;
+}
+
+int gw_train_processor_backward_tape(gw_plan* p, gw_tape* k, const float* grad_x_out, float* grad_x_in, float* grad_edge_attr, const gw_param* grads,
+                                     int32_t n, void* stream) {
+  GW_TRY(check_tape(p, k));
+  GW_CHECK(grad_x_out && (n == 0 || grads), "null argument");
+  GW_CUDA(cudaSetDevice(p->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  GW_TRY(gw::processor_backward(p, p->train, k, grad_x_out, grad_x_in, grad_edge_attr, st));
+  return hand_out_grads(p, grads, n, "gw_train_processor_backward_tape", st);
+}
+
+int gw_train_decoder_forward_tape(gw_plan* p, gw_tape* k, const float* x_in, const float* start_features, int32_t start_ld, float* out, int32_t batch,
+                                  void* stream) {
+  GW_TRY(check_tape(p, k));
+  GW_TRY(gw::check_ready(p, batch, gw::NEED_DEC));
+  GW_CHECK(x_in && out, "null argument");
+  GW_CHECK(p->d.residual_dim == 0 || (start_features && start_ld >= p->d.residual_dim), "start features required (decoder.py:93)");
+  GW_CHECK(!p->train_only, kStagePlan);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rc = gw::decoder_forward(p, p->train, k, x_in, start_features, start_ld, out, batch, st);
+  if (rc) gw::tape_release(p->train, k, st);
+  return rc;
+}
+
+int gw_train_decoder_backward_tape(gw_plan* p, gw_tape* k, const float* grad_out, float* grad_x_in, const gw_param* grads, int32_t n, void* stream) {
+  GW_TRY(check_tape(p, k));
+  GW_CHECK(grad_out && (n == 0 || grads), "null argument");
+  GW_CUDA(cudaSetDevice(p->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  GW_TRY(gw::decoder_backward(p, p->train, k, grad_out, grad_x_in, st));
+  return hand_out_grads(p, grads, n, "gw_train_decoder_backward_tape", st);
 }
 
 int64_t gw_train_peak_bytes(const gw_plan* p) { return (p && p->train) ? (int64_t)p->train->peak_bytes : 0; }

@@ -311,6 +311,91 @@ class _TrainFn(torch.autograd.Function):
                                                  for gr, to_param, need in zip(grads, ctx.maps, ctx.pgrad))
 
 
+class _Stage:
+    """What `_StageFn` runs for one training forward of a standalone sub-module: its training engine and plan, the parameters it
+    differentiates (bound names and shapes), and the sub-module's two calls on a tape -- forward(tape, *inputs) -> outputs and
+    backward(tape, grad_outputs, named_grads) -> the inputs' gradients."""
+
+    def __init__(self, eng, plan, named_params, forward, backward):
+        self.eng, self.plan = eng, plan
+        self.names = [k for k, _ in named_params]
+        self.shapes = [tuple(q.shape) for _, q in named_params]
+        self.forward, self.backward = forward, backward
+
+
+class _StageFn(torch.autograd.Function):
+    """autograd node of one training forward of a standalone Encoder, AssimilatorEncoder, Processor, Decoder or AssimilatorDecoder:
+    forward = the stage's gw_train_*_forward_tape on a tape of its own, backward = its gw_train_*_backward_tape (gradients of the
+    stage's inputs and of every parameter).  The node owns its tape until the backward consumes it or the graph is dropped (which
+    frees it): the semantics of `multi_step()` without the window, so a stage applied twice in one graph back-propagates through
+    both calls.  One backward per forward.  The first `n_in` tensors are the stage's inputs (the tape reads them again in the
+    backward, so the node keeps them), the rest its parameters."""
+
+    @staticmethod
+    def forward(ctx, stage, n_in, *tensors):
+        inputs = tuple(t.detach() for t in tensors[:n_in])
+        tape = stage.plan.tape()
+        try:
+            outs = stage.forward(tape, *inputs)
+            _maybe_check(stage.plan)
+        except BaseException:
+            tape.close()  # a refused forward leaves no tape
+            raise
+        tape.node = weakref.ref(ctx)  # alive while the graph that will run this backward is (`_pending_tape`)
+        ctx.tape, ctx.stage, ctx.n_in, ctx.keep = tape, stage, n_in, inputs
+        return outs
+
+    @staticmethod
+    def backward(ctx, *grad_outs):
+        stage = ctx.stage
+        if ctx.tape is None or not ctx.tape.handle.value:
+            raise RuntimeError("graph_weather_b200: backward of a sub-module's training forward whose activations were consumed by an "
+                               "earlier backward (one backward per forward)")
+        if stage.eng.plan is not stage.plan:
+            raise RuntimeError("graph_weather_b200: backward of a sub-module's training forward whose plan was replaced (a larger batch "
+                               "or graph, or .to()): its activations are gone (one backward per forward)")
+        g = [x.detach().to(torch.float32).contiguous() for x in grad_outs]
+        grads = [torch.empty(s, dtype=torch.float32, device=g[0].device) for s in stage.shapes]
+        try:
+            gin = stage.backward(ctx.tape, g, list(zip(stage.names, grads)))
+        finally:  # consumed, or refused: either way the tape is done
+            ctx.tape.close()
+            ctx.tape = None
+        _maybe_check(stage.plan)
+        need = ctx.needs_input_grad[2:]
+        return (None, None) + tuple(gr if nd else None for gr, nd in zip(tuple(gin) + tuple(grads), need))
+
+
+def _stage_wants_grad(module, *inputs):
+    """A sub-module built with a `train_precision` takes its training step in train mode with autograd on and something to
+    differentiate (an input or a parameter); without one it stays inference-only."""
+    return (module.train_precision is not None and torch.is_grad_enabled() and module.training
+            and (any(t is not None and t.requires_grad for t in inputs) or any(q.requires_grad for q in module.parameters())))  # fmt: skip
+
+
+def _stage_engine(module, dims, uploaders) -> _Engine:
+    """The training engine of a standalone sub-module, of precision `train_precision` (created on first use; its inference engine
+    stays as it is).  It runs the taped step: the bounded-memory step of use_checkpointing=True is the wrappers' alone."""
+    eng = module.__dict__.get("_train_engine")
+    if eng is None:
+        eng = _new_engine(dims, module.train_precision, uploaders)
+        module.__dict__["_train_engine"] = eng
+    return eng
+
+
+def _run_stage(eng, plan, prefix, module, inputs, forward, backward):
+    """One training forward of `module` through `_StageFn`, differentiating its inputs and every parameter (bound as `prefix.name`)."""
+    named = [(f"{prefix}.{k}", q) for k, q in module.named_parameters()]
+    stage = _Stage(eng, plan, named, forward, backward)
+    return _StageFn.apply(stage, len(inputs), *inputs, *[q for _, q in named])
+
+
+def _check_train_precision(train_precision, dims):
+    """`train_precision` of a sub-module: None (the default) keeps it inference-only; a value is checked as for the wrappers."""
+    if train_precision is not None:
+        _validate_train_precision(train_precision, dims)
+
+
 def _pending_tape(engine) -> bool:
     """The engine's plan holds a tape that a backward still needs: made by a forward whose backward has not run, and whose autograd
     graph is still alive (a dropped graph's tape is only waiting to be closed)."""
@@ -357,7 +442,11 @@ class Encoder(nn.Module):
     def __init__(self, lat_lons: list, resolution: int = 2, input_dim: int = 78, output_dim: int = 256, output_edge_dim: int = 256,
                  hidden_dim_processor_node=256, hidden_dim_processor_edge=256, hidden_layers_processor_node=2,
                  hidden_layers_processor_edge=2, mlp_norm_type="LayerNorm", use_checkpointing: bool = False,
-                 efficient_batching: bool = False, precision: str = "auto"):  # fmt: skip
+                 efficient_batching: bool = False, precision: str = "auto", train_precision: Optional[str] = None):  # fmt: skip
+        """encoder.py:36-151.  train_precision=None (the default) keeps the module inference-only: its output has no autograd graph.
+        'fp32_simt' | 'fp32' | 'bf16' (as for GraphWeatherForecaster) make a train-mode call with autograd on run the encoder's
+        training step, so that `x` and `edge_attr` carry gradients to the features and every parameter.  That is the taped step;
+        use_checkpointing does not bound it here."""
         super().__init__()
         self.use_checkpointing = use_checkpointing  # accepted for API parity; GraphWeatherForecaster(use_checkpointing=True) selects its bounded-memory training step
         self.efficient_batching = efficient_batching
@@ -383,6 +472,8 @@ class Encoder(nn.Module):
         self._engine = None
         _validate_precision(precision, self._dims)
         self._precision = precision
+        _check_train_precision(train_precision, self._dims)
+        self.train_precision = train_precision
         self._lat_edge_index_t = {}
 
     # graph uploads shared with the wrappers
@@ -391,26 +482,66 @@ class Encoder(nn.Module):
         plan.set_encoder_graph(g.mesh_local, g.perm, g.ptr, g.edge_attr)
         plan.set_latent_graph(m.src, m.dst, m.ptr, m.edge_attr[m.perm])
 
-    def _latent_outputs(self, plan, batch, device):
-        """(edge_index [2,B*El] int64, edge_attr [B*El,De]) in the reference's order and replication (encoder.py:224-242)."""
+    def _latent_edge_index(self, batch, device):
+        """edge_index [2,B*El] int64 in the reference's order and replication (encoder.py:224-242)."""
         m = self._g_lat
-        El = m.edge_index.shape[1]
         key = (str(device), batch)
         if key not in self._lat_edge_index_t:
             ei = graphs.replicate_edge_index(m.edge_index, batch) if not self.efficient_batching else m.edge_index
             self._lat_edge_index_t = {key: torch.from_numpy(ei).to(device)}
+        return self._lat_edge_index_t[key]
+
+    def _latent_outputs(self, plan, batch, device):
+        """(edge_index [2,B*El] int64, edge_attr [B*El,De]) in the reference's order and replication (encoder.py:224-242)."""
+        m = self._g_lat
+        El = m.edge_index.shape[1]
+        ei = self._latent_edge_index(batch, device)
         sorted_attr = torch.empty((El, self._dims["edge_dim"]), dtype=torch.float32, device=device)
         plan.latent_edge_features(sorted_attr)
         ref_attr = torch.empty_like(sorted_attr)
         ref_attr[torch.from_numpy(m.perm).to(device)] = sorted_attr
         if not self.efficient_batching:
             ref_attr = ref_attr.repeat(batch, 1)
-        return self._lat_edge_index_t[key], ref_attr
+        return ei, ref_attr
+
+    def _train_encode(self, features, lat_lon_heights):
+        """The training step of Encoder.forward / AssimilatorEncoder.forward (`_StageFn`): x [B*H, Dn] and edge_attr as in inference,
+        both differentiable.  edge_attr is formed from the sorted latent edge features by torch ops (the inverse of the plan's
+        edge order, then one copy per sample), so autograd sums the copies' gradients.  lat_lon_heights gets no gradient."""
+        B = features.shape[0]
+        eng = _stage_engine(self, self._dims, [self._upload_graphs])
+        grow = None if lat_lon_heights is None else dict(n_in=lat_lon_heights.shape[0])
+        plan = eng.ensure(features.device, B, _prefixed("encoder", self), grow=grow)
+        if lat_lon_heights is not None:
+            self._upload_obs(eng, plan, lat_lon_heights)
+        m = self._g_lat
+        El, f_shape = m.edge_index.shape[1], tuple(features.shape)
+
+        def forward(tape, f):
+            x = torch.empty((B * self.num_h3, self.output_dim), dtype=torch.float32, device=f.device)
+            e = torch.empty((El, self._dims["edge_dim"]), dtype=torch.float32, device=f.device)
+            tape.encoder_forward(f, x, e)
+            return x, e
+
+        def backward(tape, g, named):
+            gf = torch.empty(f_shape, dtype=torch.float32, device=g[0].device)
+            tape.encoder_backward(g[0], g[1], gf, named)
+            return (gf,)
+
+        f = features.to(torch.float32).contiguous()
+        x, sorted_attr = _run_stage(eng, plan, "encoder", self, (f,), forward, backward)
+        inv = torch.from_numpy(np.argsort(m.perm)).to(f.device)  # ref_attr[perm] = sorted_attr, as a gather autograd can reverse
+        ref_attr = sorted_attr[inv]
+        if not self.efficient_batching:
+            ref_attr = ref_attr.repeat(B, 1)
+        return x, self._latent_edge_index(B, f.device), ref_attr
 
     def _encode(self, features, what, lat_lon_heights=None):
         """Encoder.forward and AssimilatorEncoder.forward; the assimilator's observation graph is uploaded for every call."""
         if features.device.type != "cuda":
             _no_host_path(what)
+        if _stage_wants_grad(self, features):
+            return self._train_encode(features, lat_lon_heights)
         B = features.shape[0]
         eng = _own_engine(self)
         if lat_lon_heights is None:
@@ -436,7 +567,12 @@ class Processor(nn.Module):
     def __init__(self, input_dim: int = 256, edge_dim: int = 256, num_blocks: int = 9, hidden_dim_processor_node: int = 256,
                  hidden_dim_processor_edge: int = 256, hidden_layers_processor_node: int = 2, hidden_layers_processor_edge: int = 2,
                  mlp_norm_type: str = "LayerNorm", use_thermalizer: bool = False, use_checkpointing: bool = False,
-                 precision: str = "auto"):  # fmt: skip
+                 precision: str = "auto", train_precision: Optional[str] = None):  # fmt: skip
+        """processor.py:17-68.  train_precision=None (the default) keeps the module inference-only.  'fp32_simt' | 'fp32' | 'bf16'
+        make a train-mode call with autograd on run the processor's training step on the call's graph: `x`, `edge_attr` (in the
+        caller's edge order) and every parameter get gradients, with `checkpoint_segments` read at every call.  Each call keeps its
+        own tape, so a processor applied several times in one graph back-propagates through every call.  That is the taped step;
+        use_checkpointing does not bound it here."""
         super().__init__()
         if use_thermalizer:
             raise NotImplementedError("use_thermalizer=True: the stochastic ThermalizerLayer is outside the accelerated path")
@@ -451,10 +587,13 @@ class Processor(nn.Module):
                          hidden_layers_edge=hidden_layers_processor_edge, num_blocks=num_blocks)  # fmt: skip
         _validate_precision(precision, self._cfg)
         self._precision = precision
+        _check_train_precision(train_precision, self._cfg)
+        self.train_precision = train_precision
         self._engine = None
 
     def set_checkpoint_segments(self, checkpoint_segments: int):
-        """processor.py:70-81.  The training step of the wrapper this processor belongs to recomputes the processor in its backward:
+        """processor.py:70-81.  The training step of the wrapper this processor belongs to, or of this processor alone (a
+        `train_precision`), recomputes the processor in its backward:
         0 (the default) keeps the processor's whole tape; N > 0 recomputes segments of N blocks, keeping only each segment's first
         node and edge rows; -1 recomputes the whole processor as one segment.  Outputs and gradients do not change, only the memory a
         training forward keeps and the time of its backward (gw_train_set_processor_segments).  Read at every training forward."""
@@ -470,10 +609,15 @@ class Processor(nn.Module):
         ptr = torch.searchsorted(dst_sorted, torch.arange(n_nodes + 1, device=edge_index.device, dtype=dst_sorted.dtype)).to(torch.int32)
         return src, dst_sorted.to(torch.int32).contiguous(), ptr.contiguous(), order
 
+    def _plan_dims(self, n_nodes, n_edges):
+        return dict(n_in=0, n_out=0, n_mesh=n_nodes, n_lat_edges=n_edges, n_dec_edges=0, in_dim=1, enc_edge_attr_dim=2, out_dim=1,
+                    residual_dim=0, hidden_dec=1, hidden_layers_dec=1, **self._cfg)  # fmt: skip
+
     def forward(self, x: torch.Tensor, edge_index, edge_attr, t: int = 0, batch_size: int = None, efficient_batching: bool = False):
         if x.device.type != "cuda":
             _no_host_path("Processor.forward")
-        x = x.detach().to(torch.float32).contiguous()
+        train = _stage_wants_grad(self, x, edge_attr)
+        x = x.to(torch.float32).contiguous() if train else x.detach().to(torch.float32).contiguous()
         n_nodes = x.shape[0]
         if efficient_batching and batch_size is not None and batch_size > 1:
             # shared graph, per-sample loop in the reference (processor.py:106-122) == block-diagonal replication
@@ -481,16 +625,38 @@ class Processor(nn.Module):
             edge_index = torch.cat([edge_index + i * per for i in range(batch_size)], dim=1)
             edge_attr = edge_attr.repeat(batch_size, 1)
         src, dst, ptr, order = self._sorted_graph(edge_index, n_nodes)
+        if train:
+            return self._train_forward(x, edge_attr.to(torch.float32)[order].contiguous(), src, dst, ptr)
         ea = edge_attr.detach().to(torch.float32)[order].contiguous()
         if self._engine is None:
-            dims = dict(n_in=0, n_out=0, n_mesh=n_nodes, n_lat_edges=int(src.numel()), n_dec_edges=0, in_dim=1,
-                        enc_edge_attr_dim=2, out_dim=1, residual_dim=0, hidden_dec=1, hidden_layers_dec=1, **self._cfg)  # fmt: skip
-            self._engine = _Engine(dims, self._precision)
+            self._engine = _Engine(self._plan_dims(n_nodes, int(src.numel())), self._precision)
         plan = self._engine.ensure(x.device, 1, _prefixed("processor", self), grow=dict(n_mesh=n_nodes, n_lat_edges=int(src.numel())))
         out = torch.empty_like(x)
         plan.processor_forward_graph(x, out, ea, src, dst, ptr)
         _maybe_check(plan)
         return out
+
+    def _train_forward(self, x, ea, src, dst, ptr):
+        """The training step of Processor.forward (`_StageFn`) on the target-sorted graph; ea is edge_attr in that order, gathered by
+        a torch op so that autograd returns its gradient in the caller's order."""
+        n_nodes, n_edges = x.shape[0], int(src.numel())
+        eng = _stage_engine(self, self._plan_dims(n_nodes, n_edges), [])
+        plan = eng.ensure(x.device, 1, _prefixed("processor", self), grow=dict(n_mesh=n_nodes, n_lat_edges=n_edges))
+        plan.set_processor_segments(self.checkpoint_segments)
+        x_shape, e_shape = tuple(x.shape), tuple(ea.shape)
+
+        def forward(tape, xi, e):
+            out = torch.empty_like(xi)
+            tape.processor_forward(xi, out, e, src, dst, ptr)
+            return out
+
+        def backward(tape, g, named):
+            gx = torch.empty(x_shape, dtype=torch.float32, device=g[0].device)
+            ge = torch.empty(e_shape, dtype=torch.float32, device=g[0].device)
+            tape.processor_backward(g[0], gx, ge, named)
+            return gx, ge
+
+        return _run_stage(eng, plan, "processor", self, (x, ea), forward, backward)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -501,7 +667,11 @@ class AssimilatorDecoder(nn.Module):
                  hidden_dim_processor_node: int = 256, hidden_dim_processor_edge: int = 256, hidden_layers_processor_node: int = 2,
                  hidden_layers_processor_edge: int = 2, mlp_norm_type: str = "LayerNorm", hidden_dim_decoder: int = 128,
                  hidden_layers_decoder: int = 2, use_checkpointing: bool = False, efficient_batching: bool = False,
-                 precision: str = "auto"):  # fmt: skip
+                 precision: str = "auto", train_precision: Optional[str] = None):  # fmt: skip
+        """assimilator_decoder.py:36-129 (Decoder: decoder.py:24-77).  train_precision=None (the default) keeps the module
+        inference-only.  'fp32_simt' | 'fp32' | 'bf16' make a train-mode call with autograd on run the decoder's training step:
+        processor_features, start_features (the Decoder's residual) and every parameter get gradients.  That is the taped step;
+        use_checkpointing does not bound it here."""
         super().__init__()
         self.use_checkpointing = use_checkpointing
         self.efficient_batching = efficient_batching
@@ -524,22 +694,50 @@ class AssimilatorDecoder(nn.Module):
         )  # fmt: skip
         _validate_precision(precision, self._dims)
         self._precision = precision
+        _check_train_precision(train_precision, self._dims)
+        self.train_precision = train_precision
         self._engine = None
 
     def _upload_graphs(self, plan):
         g = self._g_dec
         plan.set_decoder_graph(g.src, g.ptr, g.edge_attr)
 
-    def _run(self, processor_features, batch_size, start):
+    def _run(self, processor_features, batch_size, start_features):
         if processor_features.device.type != "cuda":
             _no_host_path("Decoder.forward")
+        if _stage_wants_grad(self, processor_features, start_features):
+            return self._train_run(processor_features, batch_size, start_features)
         x = processor_features.detach().to(torch.float32).contiguous()
+        start = None if start_features is None else start_features.detach().to(torch.float32).contiguous()
         eng = _own_engine(self, dict(self._dims, residual_dim=self.output_dim if self._residual else 0))
         plan = eng.ensure(x.device, batch_size, _prefixed("decoder", self))
         out = torch.empty((batch_size, self.num_latlons, self.output_dim), dtype=torch.float32, device=x.device)
         plan.decoder_forward(x, start, out, batch_size)
         _maybe_check(plan)
         return out
+
+    def _train_run(self, processor_features, batch_size, start_features):
+        """The training step of the decoder's forward (`_StageFn`).  The residual's gradient is the output's gradient itself."""
+        x = processor_features.to(torch.float32).contiguous()
+        if x.numel() != batch_size * self.num_h3 * self._dims["node_dim"]:
+            raise RuntimeError(f"processor_features: expected {batch_size} x {self.num_h3} mesh rows of width {self._dims['node_dim']}, "
+                               f"got {tuple(processor_features.shape)}")  # fmt: skip
+        eng = _stage_engine(self, dict(self._dims, residual_dim=self.output_dim if self._residual else 0), [self._upload_graphs])
+        plan = eng.ensure(x.device, batch_size, _prefixed("decoder", self))
+        out_shape, x_shape = (batch_size, self.num_latlons, self.output_dim), tuple(x.shape)
+
+        def forward(tape, xi, *start):
+            out = torch.empty(out_shape, dtype=torch.float32, device=xi.device)
+            tape.decoder_forward(xi, start[0] if start else None, out, batch_size)
+            return out
+
+        def backward(tape, g, named):
+            gx = torch.empty(x_shape, dtype=torch.float32, device=g[0].device)
+            tape.decoder_backward(g[0], gx, named)
+            return (gx, g[0]) if start_features is not None else (gx,)
+
+        inputs = (x,) if start_features is None else (x, start_features.to(torch.float32).contiguous())
+        return _run_stage(eng, plan, "decoder", self, inputs, forward, backward)
 
     def forward(self, processor_features: torch.Tensor, batch_size: int) -> torch.Tensor:
         return self._run(processor_features, batch_size, None)
@@ -550,10 +748,11 @@ class Decoder(AssimilatorDecoder):
                  hidden_dim_processor_node: int = 256, hidden_dim_processor_edge: int = 256, hidden_layers_processor_node: int = 2,
                  hidden_layers_processor_edge: int = 2, mlp_norm_type: str = "LayerNorm", hidden_dim_decoder: int = 128,
                  hidden_layers_decoder: int = 2, use_checkpointing: bool = False, efficient_batching: bool = False,
-                 precision: str = "auto"):  # fmt: skip
+                 precision: str = "auto", train_precision: Optional[str] = None):  # fmt: skip
         super().__init__(lat_lons, resolution, input_dim, output_dim, output_edge_dim, hidden_dim_processor_node,
                          hidden_dim_processor_edge, hidden_layers_processor_node, hidden_layers_processor_edge, mlp_norm_type,
-                         hidden_dim_decoder, hidden_layers_decoder, use_checkpointing, efficient_batching, precision)  # fmt: skip
+                         hidden_dim_decoder, hidden_layers_decoder, use_checkpointing, efficient_batching, precision,
+                         train_precision)  # fmt: skip
         self._residual = True
 
     def forward(self, processor_features: torch.Tensor, start_features: torch.Tensor, t: int = 0) -> torch.Tensor:
@@ -562,8 +761,7 @@ class Decoder(AssimilatorDecoder):
                 f"The size of tensor a ({self.output_dim}) must match the size of tensor b ({start_features.shape[-1]}) "
                 "at non-singleton dimension 2"
             )
-        start = start_features.detach().to(torch.float32).contiguous()
-        return self._run(processor_features, start_features.shape[0], start)
+        return self._run(processor_features, start_features.shape[0], start_features)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -573,7 +771,11 @@ class AssimilatorEncoder(nn.Module):
     def __init__(self, resolution: int = 2, input_dim: int = 2, output_dim: int = 256, output_edge_dim: int = 256,
                  hidden_dim_processor_node: int = 256, hidden_dim_processor_edge: int = 256, hidden_layers_processor_node: int = 2,
                  hidden_layers_processor_edge: int = 2, mlp_norm_type: str = "LayerNorm", use_checkpointing: bool = False,
-                 precision: str = "auto"):  # fmt: skip
+                 precision: str = "auto", train_precision: Optional[str] = None):  # fmt: skip
+        """assimilator_encoder.py:36-168.  train_precision as for Encoder: None keeps the module inference-only; a value makes a
+        train-mode call with autograd on differentiable in the observation values and every parameter (not in lat_lon_heights).
+        The observation graph belongs to the plan, so of two training forwards alive at once only the later one can run its
+        backward (the earlier one's raises)."""
         super().__init__()
         self.use_checkpointing = use_checkpointing
         self.output_dim = output_dim
@@ -596,6 +798,8 @@ class AssimilatorEncoder(nn.Module):
         )  # fmt: skip
         _validate_precision(precision, self._dims)
         self._precision = precision
+        _check_train_precision(train_precision, self._dims)
+        self.train_precision = train_precision
         self._engine = None
         self.efficient_batching = False
         self._lat_edge_index_t = {}
@@ -623,7 +827,9 @@ class AssimilatorEncoder(nn.Module):
             plan.set_encoder_graph(g.mesh_local, g.perm, g.ptr, g.edge_attr)
             engine.obs_key = key
 
+    _latent_edge_index = Encoder._latent_edge_index
     _latent_outputs = Encoder._latent_outputs
+    _train_encode = Encoder._train_encode
     _encode = Encoder._encode
 
     def forward(self, features: torch.Tensor, lat_lon_heights: torch.Tensor):

@@ -164,6 +164,39 @@ int gw_train_forward_tape(gw_plan* plan, gw_tape* tape, const float* features, f
 int gw_train_backward_tape(gw_plan* plan, gw_tape* tape, const float* grad_out, float* grad_features, const gw_param* grads,
                            int32_t n, void* stream);
 int64_t gw_tape_bytes(const gw_tape* tape);
+/* The training step of one stage alone, on a tape of a gw_plan_create plan that holds that stage (the reference's sub-modules are
+ * ordinary differentiable modules, tests/test_model.py:20-119).  Replaces the autograd backward of Encoder.forward (encoder.py:153-242)
+ * and AssimilatorEncoder.forward (assimilator_encoder.py:118-168), Processor.forward (processor.py:83-128), Decoder.forward
+ * (decoder.py:79-94) and AssimilatorDecoder.forward (assimilator_decoder.py:131-200).  The whole-network step above is these three
+ * stages composed.  Conventions as for gw_train_forward_tape / gw_train_backward_tape: one backward per forward, on the tape of a
+ * forward of the same stage; a backward after gw_plan_set_weights fails; gradients are copied into `grads` under the reference's
+ * state_dict names; gw_tape_bytes and gw_train_peak_bytes keep their meaning; the processor calls follow
+ * gw_train_set_processor_segments; GW_PREC_FP32_TC / GW_PREC_BF16_TC bound the caller's x_in and edge_attr as they bound features
+ * (status bit 3 on an inf / NaN).  Inputs a forward reads (features, x_in, edge_attr, start_features) are read again by its
+ * backward: the caller keeps them unchanged until it has run.  Mesh rows are in slot order, as for the stage entry points below.
+ *   encoder    features [batch, n_in, in_dim] -> x_out [batch*n_mesh, node_dim] and e_lat_out [n_lat_edges, edge_dim]: one sample's
+ *              latent edge features in the plan's target-sorted order, as gw_latent_edge_features returns them (the reference
+ *              repeats them per sample).  Backward: grad_x, grad_e_lat (summed over the samples; NULL: zero) -> parameter gradients
+ *              and, unless grad_features is NULL, the features' gradient.  A backward fails once the encoder graph was replaced
+ *              after its forward (the assimilator's per-call observation graph).
+ *   processor  on a caller-supplied graph, as gw_processor_forward_graph (copied onto the tape with its source-sorted CSR, so it
+ *              may change on every call); x_out must not alias x_in.  Backward: grad_x_out [n_nodes, node_dim] -> parameter
+ *              gradients, grad_x_in [n_nodes, node_dim] and grad_edge_attr [n_edges, edge_dim] per edge (either may be NULL).
+ *   decoder    x_in [batch*n_mesh, node_dim] (+ start_features [batch, n_out, start_ld] when the plan has a residual) -> out.
+ *              Backward: grad_out [batch, n_out, out_dim] -> parameter gradients and grad_x_in (NULL: none).  The residual's
+ *              gradient, grad_out itself, is the caller's to add to start_features' gradient. */
+int gw_train_encoder_forward_tape(gw_plan* plan, gw_tape* tape, const float* features, float* x_out, float* e_lat_out, int32_t batch,
+                                  void* stream);
+int gw_train_encoder_backward_tape(gw_plan* plan, gw_tape* tape, const float* grad_x, const float* grad_e_lat, float* grad_features,
+                                   const gw_param* grads, int32_t n, void* stream);
+int gw_train_processor_forward_tape(gw_plan* plan, gw_tape* tape, const float* x_in, float* x_out, const float* edge_attr, int32_t n_nodes,
+                                    int32_t n_edges, const int32_t* src, const int32_t* dst, const int32_t* ptr, void* stream);
+int gw_train_processor_backward_tape(gw_plan* plan, gw_tape* tape, const float* grad_x_out, float* grad_x_in, float* grad_edge_attr,
+                                     const gw_param* grads, int32_t n, void* stream);
+int gw_train_decoder_forward_tape(gw_plan* plan, gw_tape* tape, const float* x_in, const float* start_features, int32_t start_ld, float* out,
+                                  int32_t batch, void* stream);
+int gw_train_decoder_backward_tape(gw_plan* plan, gw_tape* tape, const float* grad_out, float* grad_x_in, const gw_param* grads, int32_t n,
+                                   void* stream);
 /* Replaces: Processor.set_checkpoint_segments (processor.py:70-81) and GraphCast.set_checkpoint_processor (graphcast/model.py:149-163,
  * 230-250).  Processor segments of the training forwards that start after this call, on either training step: 0 (the default) keeps
  * the processor's whole tape; N > 0 cuts segments of N blocks (0..N-1, N..2N-1, ..., a shorter last one); -1, or any N >=
