@@ -88,6 +88,8 @@ _SIGNATURES = {
     "gw_train_decoder_forward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _i32, _vp]),
     "gw_train_decoder_backward_tape": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.POINTER(GwParam), _i32, _vp]),
     "gw_train_set_processor_segments": (ctypes.c_int, [_vp, _i32]),
+    "gw_train_set_deterministic": (ctypes.c_int, [_vp, _i32]),
+    "gw_train_deterministic_bytes": (_i64, [_vp]),
     "gw_launch_count": (_i64, []),
     "gw_launch_count_reset": (None, []),
 }
@@ -212,6 +214,14 @@ class Plan:
         """gw_train_set_processor_segments: processor segments of the training forwards that follow (0 none, N > 0 blocks per
         segment, -1 one segment); their backward recomputes each segment instead of keeping the processor's tape."""
         _check(self.lib.gw_train_set_processor_segments(self.handle, int(segments)))
+
+    def set_deterministic(self, on: bool):
+        """gw_train_set_deterministic: fixed-order (bit-repeatable) parameter gradients in the training backwards that follow."""
+        _check(self.lib.gw_train_set_deterministic(self.handle, 1 if on else 0))
+
+    def deterministic_bytes(self) -> int:
+        """Device bytes of the fixed-order gradients' workspace (gw_train_deterministic_bytes)."""
+        return int(self.lib.gw_train_deterministic_bytes(self.handle))
 
     def _dev(self, arr, dtype):
         t = torch.as_tensor(arr).to(dtype=dtype).contiguous().to(self.device)

@@ -28,6 +28,18 @@ cudaError_t launch_wgrad(const float* dY, int ldy, int N, const RowSrc& a, int K
 cudaError_t launch_ln_bwd(const float* dy, int ld_dy, const float* z, int ld_z, int N, const float* gamma, long long R, float* dz, int ld_dz,
                           float* dgamma, float* dbeta, cudaStream_t st);
 constexpr int LN_BWD_MAX_N = 1024;  // widest row launch_ln_bwd takes (rows of more than 256 columns run on a kernel of their own)
+// Fixed-order variants of the two (gw_train_set_deterministic): the same per-slab / per-CTA sums, stored as partials in a
+// workspace and added in an order that follows from the shapes alone, so that every run gives the same bits.  The workspace
+// stays within DET_WS_BYTES: launch_wgrad_det cuts fewer row slabs for wide weights (one slab's tile fits for K < 32767), and
+// launch_ln_bwd_det needs 2 x (its grid, at most 8 GRID_SMS) x N floats, 8.7 MB at N = 1024.  ws_floats below the
+// *_workspace_floats of the shapes: cudaErrorInvalidValue.
+constexpr size_t DET_WS_BYTES = size_t(32) << 20;
+size_t wgrad_det_workspace_floats(long long R, int N, int K);
+cudaError_t launch_wgrad_det(const float* dY, int ldy, int N, const RowSrc& a, int K, int rows_per_sample, int batch, float* dW, int ldw, float* db,
+                             float* ws, size_t ws_floats, cudaStream_t st);
+size_t ln_bwd_det_workspace_floats(long long R, int N);
+cudaError_t launch_ln_bwd_det(const float* dy, int ld_dy, const float* z, int ld_z, int N, const float* gamma, long long R, float* dz, int ld_dz,
+                              float* dgamma, float* dbeta, float* ws, size_t ws_floats, cudaStream_t st);
 cudaError_t launch_batch_reduce(const float* in, int ld_in, long long rows, int width, int batch, float* out, int ld_out, bool accumulate,
                                 cudaStream_t st);
 // idx_base: `in` holds the targets idx_base .. idx_base + src_rows - 1 only (a chunk of the training step's grid-sized stages).
@@ -116,6 +128,8 @@ __host__ __device__ inline float tc_weight_scale(float amax, int parts) {
 // product, power-of-two scaled from the operands' absmax), else bf16.  Any N (128-row output blocks); K > 256 runs as blocks of
 // 256 columns of A, one after the other through the same workspace.
 size_t wgrad_tc_workspace_floats(long long R, int N, int K);
+// dW[o, k] += sum_s part[s][o][k] (s ascending, part [S][N][K]), db[o] += sum_s part_b[s][o] (db null: none)
+cudaError_t launch_wgrad_sum(const float* part, const float* part_b, int S, int N, int K, float* dW, int ldw, float* db, cudaStream_t st);
 cudaError_t launch_wgrad_tc(const float* dY, int ldy, int N, const RowSrc& a, int K, int rows_per_sample, int batch, float* dW, int ldw, float* db,
                             bool split, float* ws, size_t ws_floats, int32_t* status, cudaStream_t st);
 

@@ -101,6 +101,7 @@ struct gw_plan {
   bool train_only = false;          // gw_plan_create_train: graphs, weights and the bounded-memory (chunked) training step only
   int train_chunk_pts = 0;          // GW_B200_TRAIN_CHUNK: points per chunk of that step (0: from the shapes, gw_train.cu)
   int train_segments = 0;           // processor segments of later training forwards (gw_train_set_processor_segments)
+  bool train_deterministic = false; // fixed-order weight and LayerNorm-parameter gradients in later backwards (gw_train_set_deterministic)
   gw_dims d;
   int device = 0;
   int n_in_cur = 0;

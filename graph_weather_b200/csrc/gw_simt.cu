@@ -339,11 +339,13 @@ cudaError_t launch_segsum_chunked(const float* base, int ld, const int32_t* ptr,
 // dW[n, k] += sum_r dY[r, n] * A[r, k]   (and db[n] += sum_r dY[r, n]) over R = rows_per_sample * batch rows, A assembled from a row
 // source like the forward kernel does (N > 256: one launch per block of 256 outputs).  Tile: all N <= 256 output rows x 32
 // k-columns per CTA column (blockIdx.y), the rows are
-// cut into gridDim.x slabs; every CTA accumulates its slab in registers (8 n x 4 k per thread) and adds it to dW with float
-// atomics (summation order across slabs is not fixed: gradients repeat to ~1e-7 relative, not bit for bit).
+// cut into gridDim.x slabs; every CTA accumulates its slab in registers (8 n x 4 k per thread).  gw_wgrad_kernel adds it to dW
+// with float atomics (summation order across slabs is not fixed: gradients repeat to ~1e-7 relative, not bit for bit);
+// gw_wgrad_det_kernel stores it as slab blockIdx.x's partial tile, and gw_wgrad_sum_kernel adds the slabs in slab order.
 constexpr int WG_KT = 32, WG_RT = 16;
-__global__ void __launch_bounds__(256) gw_wgrad_kernel(const float* __restrict__ dY, int ldy, int N, RowSrc a, int K, int rows_per_sample, int batch,
-                                                       float* __restrict__ dW, int ldw, float* __restrict__ db) {
+template <bool PARTIAL>  // PARTIAL: store the slab's sums at dW / db (a partial tile) instead of adding them with atomics
+__device__ __forceinline__ void wgrad_slab(const float* __restrict__ dY, int ldy, int N, RowSrc a, int K, int rows_per_sample, int batch,
+                                           float* __restrict__ dW, int ldw, float* __restrict__ db) {
   __shared__ float Ys[WG_RT][256 + 1];
   __shared__ float As[WG_RT][WG_KT + 1];
   const int tid = threadIdx.x, tn = tid & 31, tk = tid >> 5;  // thread: n = tn + 32 i (i < 8), k = 4 tk + j (j < 4)
@@ -398,10 +400,26 @@ __global__ void __launch_bounds__(256) gw_wgrad_kernel(const float* __restrict__
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int k = k0 + 4 * tk + j;
-      if (k < K) atomicAdd(dW + (size_t)n * ldw + k, acc[i][j]);
+      if (k < K) {
+        if (PARTIAL) dW[(size_t)n * ldw + k] = acc[i][j];
+        else atomicAdd(dW + (size_t)n * ldw + k, acc[i][j]);
+      }
     }
-    if (db && blockIdx.y == 0 && tk == 0) atomicAdd(db + n, bacc[i]);
+    if (db && blockIdx.y == 0 && tk == 0) {
+      if (PARTIAL) db[n] = bacc[i];
+      else atomicAdd(db + n, bacc[i]);
+    }
   }
+}
+__global__ void __launch_bounds__(256) gw_wgrad_kernel(const float* __restrict__ dY, int ldy, int N, RowSrc a, int K, int rows_per_sample, int batch,
+                                                       float* __restrict__ dW, int ldw, float* __restrict__ db) {
+  wgrad_slab<false>(dY, ldy, N, a, K, rows_per_sample, batch, dW, ldw, db);
+}
+// part [gridDim.x][N][K], part_b [gridDim.x][N] (null: no bias): every element of slab blockIdx.x's tile is written
+__global__ void __launch_bounds__(256) gw_wgrad_det_kernel(const float* __restrict__ dY, int ldy, int N, RowSrc a, int K, int rows_per_sample,
+                                                           int batch, float* __restrict__ part, float* __restrict__ part_b) {
+  wgrad_slab<true>(dY, ldy, N, a, K, rows_per_sample, batch, part + (size_t)blockIdx.x * N * K, K,
+                   part_b ? part_b + (size_t)blockIdx.x * N : nullptr);
 }
 cudaError_t launch_wgrad(const float* dY, int ldy, int N, const RowSrc& a, int K, int rows_per_sample, int batch, float* dW, int ldw, float* db,
                          cudaStream_t st) {
@@ -415,12 +433,43 @@ cudaError_t launch_wgrad(const float* dY, int ldy, int N, const RowSrc& a, int K
   }
   return cudaGetLastError();
 }
+// Slabs of the fixed-order weight gradient: those of launch_wgrad, fewer where the partial tiles of one output block of 256 would
+// not fit in DET_WS_BYTES (train/run.py's 1024 x 1024 weights: 31 slabs).  From the shapes alone, so the summation order is too.
+static int wgrad_det_slabs(long long R, int N, int K) {
+  const size_t tile = (size_t)std::min(N, 256) * K + std::min(N, 256);
+  const long long fit = (long long)(DET_WS_BYTES / sizeof(float) / tile);
+  return (int)std::max(1LL, std::min({296LL, (R + 255) / 256, fit}));
+}
+size_t wgrad_det_workspace_floats(long long R, int N, int K) {
+  if (R <= 0 || N <= 0 || K <= 0) return 0;
+  return (size_t)wgrad_det_slabs(R, N, K) * ((size_t)std::min(N, 256) * K + std::min(N, 256));
+}
+cudaError_t launch_wgrad_det(const float* dY, int ldy, int N, const RowSrc& a, int K, int rows_per_sample, int batch, float* dW, int ldw, float* db,
+                             float* ws, size_t ws_floats, cudaStream_t st) {
+  const long long R = (long long)rows_per_sample * batch;
+  if (R <= 0 || N <= 0 || K <= 0) return cudaSuccess;
+  if (ws_floats < wgrad_det_workspace_floats(R, N, K)) return cudaErrorInvalidValue;
+  const int slabs = wgrad_det_slabs(R, N, K);
+  for (int o0 = 0; o0 < N; o0 += 256) {  // the output blocks one after the other through the same workspace
+    const int nb = std::min(256, N - o0);
+    float* part_b = db ? ws + (size_t)slabs * nb * K : nullptr;
+    gw_wgrad_det_kernel<<<dim3(slabs, (K + WG_KT - 1) / WG_KT), 256, 0, st>>>(dY + o0, ldy, nb, a, K, rows_per_sample, batch, ws, part_b);
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    if ((e = launch_wgrad_sum(ws, part_b, slabs, nb, K, dW + (size_t)o0 * ldw, ldw, db ? db + o0 : nullptr, st)) != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
 
 // LayerNorm backward over rows of N <= 256 columns (one warp per row, rows grid-strided):
 //   zh = (z - mean) * rstd;  g = dy * gamma;  dz = rstd * (g - mean(g) - zh * mean(g * zh));  dgamma += dy * zh;  dbeta += dy
-__global__ void __launch_bounds__(256) gw_ln_bwd_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z, int N,
-                                                        const float* __restrict__ gamma, long long R, float* __restrict__ dz, int ld_dz,
-                                                        float* __restrict__ dgamma, float* __restrict__ dbeta) {
+// gw_ln_bwd_kernel adds each CTA's dgamma / dbeta sums with float atomics; gw_ln_bwd_det_kernel stores them as CTA blockIdx.x's
+// partial rows (part [2][gridDim.x][N]: dgamma rows, then dbeta rows) and gw_colsum_kernel adds the CTAs in a fixed order.
+template <bool PARTIAL>  // PARTIAL: store the CTA's sums at dgamma / dbeta (its partial rows) instead of adding them with atomics
+__device__ __forceinline__ void ln_bwd_rows(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z, int N,
+                                            const float* __restrict__ gamma, long long R, float* __restrict__ dz, int ld_dz,
+                                            float* __restrict__ dgamma, float* __restrict__ dbeta) {
   __shared__ float sg[8][256], sb[8][256];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   float ag[8], ab[8];
@@ -475,16 +524,27 @@ __global__ void __launch_bounds__(256) gw_ln_bwd_kernel(const float* __restrict_
     float g = 0.f, b = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) g += sg[k][c], b += sb[k][c];
-    atomicAdd(dgamma + c, g), atomicAdd(dbeta + c, b);
+    if (PARTIAL) dgamma[c] = g, dbeta[c] = b;
+    else atomicAdd(dgamma + c, g), atomicAdd(dbeta + c, b);
   }
+}
+__global__ void __launch_bounds__(256) gw_ln_bwd_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z, int N,
+                                                        const float* __restrict__ gamma, long long R, float* __restrict__ dz, int ld_dz,
+                                                        float* __restrict__ dgamma, float* __restrict__ dbeta) {
+  ln_bwd_rows<false>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, dgamma, dbeta);
+}
+__global__ void __launch_bounds__(256) gw_ln_bwd_det_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z, int N,
+                                                            const float* __restrict__ gamma, long long R, float* __restrict__ dz, int ld_dz,
+                                                            float* __restrict__ part) {
+  ln_bwd_rows<true>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, part + (size_t)blockIdx.x * N, part + ((size_t)gridDim.x + blockIdx.x) * N);
 }
 // The same for rows of 256 < N <= 32 J columns (LN_BWD_MAX_N = 1024: the 1024-wide models of train/run.py:491-501): one warp per
 // row with J values per lane (column lane + 32 j).  The per-CTA dgamma / dbeta partials of the 8 warps meet in one [8][1024]
 // shared array, dgamma first, then dbeta (two [8][1024] arrays would not fit in 48 KB of static shared memory).
-template <int J>
-__global__ void __launch_bounds__(256) gw_ln_bwd_wide_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z, int N,
-                                                             const float* __restrict__ gamma, long long R, float* __restrict__ dz, int ld_dz,
-                                                             float* __restrict__ dgamma, float* __restrict__ dbeta) {
+template <int J, bool PARTIAL>
+__device__ __forceinline__ void ln_bwd_wide_rows(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z, int N,
+                                                 const float* __restrict__ gamma, long long R, float* __restrict__ dz, int ld_dz,
+                                                 float* __restrict__ dgamma, float* __restrict__ dbeta) {
   __shared__ float sp[8][LN_BWD_MAX_N];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   float ag[J], ab[J];
@@ -539,7 +599,8 @@ __global__ void __launch_bounds__(256) gw_ln_bwd_wide_kernel(const float* __rest
     float g = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) g += sp[k][c];
-    atomicAdd(dgamma + c, g);
+    if (PARTIAL) dgamma[c] = g;
+    else atomicAdd(dgamma + c, g);
   }
   __syncthreads();
 #pragma unroll
@@ -550,8 +611,22 @@ __global__ void __launch_bounds__(256) gw_ln_bwd_wide_kernel(const float* __rest
     float b = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) b += sp[k][c];
-    atomicAdd(dbeta + c, b);
+    if (PARTIAL) dbeta[c] = b;
+    else atomicAdd(dbeta + c, b);
   }
+}
+template <int J>
+__global__ void __launch_bounds__(256) gw_ln_bwd_wide_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z, int N,
+                                                             const float* __restrict__ gamma, long long R, float* __restrict__ dz, int ld_dz,
+                                                             float* __restrict__ dgamma, float* __restrict__ dbeta) {
+  ln_bwd_wide_rows<J, false>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, dgamma, dbeta);
+}
+template <int J>
+__global__ void __launch_bounds__(256) gw_ln_bwd_wide_det_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ z, int ld_z,
+                                                                 int N, const float* __restrict__ gamma, long long R, float* __restrict__ dz,
+                                                                 int ld_dz, float* __restrict__ part) {
+  ln_bwd_wide_rows<J, true>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, part + (size_t)blockIdx.x * N,
+                            part + ((size_t)gridDim.x + blockIdx.x) * N);
 }
 cudaError_t launch_ln_bwd(const float* dy, int ld_dy, const float* z, int ld_z, int N, const float* gamma, long long R, float* dz, int ld_dz,
                           float* dgamma, float* dbeta, cudaStream_t st) {
@@ -565,6 +640,46 @@ cudaError_t launch_ln_bwd(const float* dy, int ld_dy, const float* z, int ld_z, 
   else
     gw_ln_bwd_wide_kernel<32><<<grid, 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, dgamma, dbeta);
   count_launch();
+  return cudaGetLastError();
+}
+
+// out0[c] += sum_s part[0][s][c],  out1[c] += sum_s part[1][s][c]  (s < S, c < N): thread row ty sums s = ty, ty + 32, ...
+// ascending, then the 32 row sums are added in ty order -- an order fixed by S and N.
+__global__ void __launch_bounds__(1024) gw_colsum_kernel(const float* __restrict__ part, int S, int N, float* __restrict__ out0,
+                                                         float* __restrict__ out1) {
+  __shared__ float sm[32][33];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5, c = blockIdx.x * 32 + tx;
+  const float* p = part + (size_t)blockIdx.y * S * N;
+  float acc = 0.f;
+  if (c < N)
+    for (int s = ty; s < S; s += 32) acc += __ldg(p + (size_t)s * N + c);
+  sm[ty][tx] = acc;
+  __syncthreads();
+  if (ty == 0 && c < N) {
+    float t = 0.f;
+#pragma unroll
+    for (int k = 0; k < 32; ++k) t += sm[k][tx];
+    float* out = blockIdx.y ? out1 : out0;
+    out[c] += t;
+  }
+}
+size_t ln_bwd_det_workspace_floats(long long R, int N) {
+  if (R <= 0 || N <= 0) return 0;
+  return 2 * (size_t)std::min<long long>(GRID_SMS * 8, (R + 7) / 8) * N;
+}
+cudaError_t launch_ln_bwd_det(const float* dy, int ld_dy, const float* z, int ld_z, int N, const float* gamma, long long R, float* dz, int ld_dz,
+                              float* dgamma, float* dbeta, float* ws, size_t ws_floats, cudaStream_t st) {
+  if (R <= 0) return cudaSuccess;
+  if (N > LN_BWD_MAX_N || ws_floats < ln_bwd_det_workspace_floats(R, N)) return cudaErrorInvalidValue;
+  const unsigned grid = (unsigned)std::min<long long>(GRID_SMS * 8, (R + 7) / 8);  // the grid of launch_ln_bwd
+  if (N <= 256)
+    gw_ln_bwd_det_kernel<<<grid, 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, ws);
+  else if (N <= 512)
+    gw_ln_bwd_wide_det_kernel<16><<<grid, 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, ws);
+  else
+    gw_ln_bwd_wide_det_kernel<32><<<grid, 256, 0, st>>>(dy, ld_dy, z, ld_z, N, gamma, R, dz, ld_dz, ws);
+  gw_colsum_kernel<<<dim3((N + 31) / 32, 2), 1024, 0, st>>>(ws, (int)grid, N, dgamma, dbeta);
+  count_launch(2);
   return cudaGetLastError();
 }
 

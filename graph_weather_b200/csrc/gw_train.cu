@@ -11,6 +11,8 @@
 //     LayerNorm       gw_ln_bwd_kernel                     dz, dgamma, dbeta
 //     gathers         backward of x[src] / x[dst] / per-target sums: per-source / per-target segment sums and row gathers
 //     broadcasts      tensors shared by the batch (encoded edge attributes, h3 node rows): gw_batch_reduce_kernel
+// The weight gradient and the LayerNorm backward add their CTAs' sums with float atomics; gw_train_set_deterministic swaps in
+// their fixed-order variants (gw_wgrad_det_kernel, gw_ln_bwd_det_kernel), and every other sum of the step has a fixed order.
 // Gradients of the factored layer 1,  h1 = relu(e W1e^T + P_s[src] + P_d[dst] + b1),  P = x [W1s ; W1d]^T :
 //     dP_s = per-source sum of dh1, dP_d = per-target sum of dh1;  dW1s += dP_s^T x, dW1d += dP_d^T x, dW1e += dh1^T e;
 //     dx += dP_s W1s + dP_d W1d, de += dh1 W1e   -- two thirds of the K = 768 weight gradient are formed per NODE, not per edge.
@@ -147,6 +149,7 @@ struct TrainState {
   DevBuf<float> bslots;  // operand magnitude bounds of the current phase (reset at the start of the forward and of the backward)
   size_t bslot_used = 0;
   DevBuf<float> wg_ws;   // gw_wgrad_tc.cu partial sums
+  DevBuf<float> det_ws;  // partial sums of the fixed-order CUDA-core weight gradient and LayerNorm backward (gw_plan::train_deterministic)
 };
 
 // an allocation of the running tape (stream-ordered on the step's stream)
@@ -276,13 +279,24 @@ static int train_op(gw_plan* p, TrainState* T, GemmOp op, int tag, bool reads_in
   return 0;
 }
 
-// dW += dY^T A, db += colsum(dY): gw_wgrad_tc.cu on tensor-core plans (K > 16), else the CUDA-core kernel
+static int det_workspace(TrainState* T, size_t floats) {
+  if (T->det_ws.n < floats) GW_TRY(T->det_ws.alloc(floats));
+  return 0;
+}
+
+// dW += dY^T A, db += colsum(dY): gw_wgrad_tc.cu on tensor-core plans (K > 16), else the CUDA-core kernel (its fixed-order
+// variant under gw_train_set_deterministic)
 static int train_wgrad(gw_plan* p, TrainState* T, const float* dY, int ldy, int N, const RowSrc& a, int K, int rows, int batch, float* dW, int ldw,
                        float* db) {
   p->cur_tag = TAG_TRAIN_WGRAD;
   TimedLaunch tl(p, T->st);
   if (!is_tc(p) || K <= 16) {  // (the edge encoders' 2- and 3-wide inputs: too narrow for a tensor-core product)
-    GW_CUDA(launch_wgrad(dY, ldy, N, a, K, rows, batch, dW, ldw, db, T->st));
+    if (p->train_deterministic) {
+      GW_TRY(det_workspace(T, wgrad_det_workspace_floats((long long)rows * batch, N, K)));
+      GW_CUDA(launch_wgrad_det(dY, ldy, N, a, K, rows, batch, dW, ldw, db, T->det_ws.p, T->det_ws.n, T->st));
+    } else {
+      GW_CUDA(launch_wgrad(dY, ldy, N, a, K, rows, batch, dW, ldw, db, T->st));
+    }
     return 0;
   }
   const size_t need = wgrad_tc_workspace_floats((long long)rows * batch, N, K);
@@ -356,8 +370,14 @@ static int mlp_bwd(gw_plan* p, TrainState* T, const Mlp& m, const MlpTape& tape,
   int ldc = ld_dout;
   if (tape.z) {
     GW_TALLOC(dz, R * m.out[m.L]);
-    GW_OTHER(launch_ln_bwd(dOut, ld_dout, tape.z, m.out[m.L], m.out[m.L], m.ln_g, (long long)R, dz, m.out[m.L], grad_of(p, T, m.ln_g),
-                           grad_of(p, T, m.ln_b), T->st));
+    if (p->train_deterministic) {
+      GW_TRY(det_workspace(T, ln_bwd_det_workspace_floats((long long)R, m.out[m.L])));
+      GW_OTHER(launch_ln_bwd_det(dOut, ld_dout, tape.z, m.out[m.L], m.out[m.L], m.ln_g, (long long)R, dz, m.out[m.L], grad_of(p, T, m.ln_g),
+                                 grad_of(p, T, m.ln_b), T->det_ws.p, T->det_ws.n, T->st));
+    } else {
+      GW_OTHER(launch_ln_bwd(dOut, ld_dout, tape.z, m.out[m.L], m.out[m.L], m.ln_g, (long long)R, dz, m.out[m.L], grad_of(p, T, m.ln_g),
+                             grad_of(p, T, m.ln_b), T->st));
+    }
     cur = dz, ldc = m.out[m.L];
   }
   for (int l = m.L; l >= 1; --l) {
@@ -1406,5 +1426,13 @@ int gw_train_set_processor_segments(gw_plan* p, int32_t segments) {
   p->train_segments = segments;
   return 0;
 }
+
+int gw_train_set_deterministic(gw_plan* p, int32_t on) {
+  GW_CHECK(p != nullptr, "null plan");
+  p->train_deterministic = on != 0;
+  return 0;
+}
+
+int64_t gw_train_deterministic_bytes(const gw_plan* p) { return (p && p->train) ? (int64_t)p->train->det_ws.bytes() : 0; }
 
 }  // extern "C"

@@ -259,6 +259,12 @@ namespace wgt {
 constexpr int KB = 256;
 }  // namespace wgt
 
+cudaError_t launch_wgrad_sum(const float* part, const float* part_b, int S, int N, int K, float* dW, int ldw, float* db, cudaStream_t st) {
+  wgt::gw_wgrad_sum_kernel<<<4 * GRID_SMS, 256, 0, st>>>(part, part_b, S, N, K, dW, ldw, db);
+  count_launch();
+  return cudaGetLastError();
+}
+
 size_t wgrad_tc_workspace_floats(long long R, int N, int K) {
   const int S = wgt::splits_for(R, (N + wgt::OB - 1) / wgt::OB);
   return (size_t)S * N * std::min(K, wgt::KB) + (size_t)S * N + 2;

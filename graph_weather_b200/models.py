@@ -253,7 +253,8 @@ class _TrainFn(torch.autograd.Function):
     parameter, gradient map) per entry of `params` (`_grad_bindings()`).  The step returns each gradient shaped like the uploaded
     tensor; the map turns it into the parameter's gradient (None: it is the parameter's already).  `obs` (the assimilator's
     lat_lon_heights, else None) is built into the training plan's observation graph for this call, as inference builds it for
-    every call."""
+    every call.  Under torch.use_deterministic_algorithms(True), read when the backward runs, the backward sums every parameter
+    gradient in a fixed order (gw_train_set_deterministic): the same inputs and weights give the same gradients bit for bit."""
 
     @staticmethod
     def forward(ctx, model, features, obs, bindings, *params):
@@ -301,6 +302,7 @@ class _TrainFn(torch.autograd.Function):
         g = grad_out.detach().to(torch.float32).contiguous()
         gfeat = torch.empty(ctx.feat_shape, dtype=torch.float32, device=dev) if ctx.feat_grad else None
         grads = [torch.empty(s, dtype=torch.float32, device=dev) for s in ctx.pshapes]
+        ctx.plan.set_deterministic(torch.are_deterministic_algorithms_enabled())  # (its value when the backward runs counts)
         try:
             ctx.tape.backward(g, gfeat, list(zip(ctx.names, grads)))
         finally:  # consumed, or refused (weights replaced, plan closed): either way the tape is done
@@ -329,7 +331,8 @@ class _StageFn(torch.autograd.Function):
     stage's inputs and of every parameter).  The node owns its tape until the backward consumes it or the graph is dropped (which
     frees it): the semantics of `multi_step()` without the window, so a stage applied twice in one graph back-propagates through
     both calls.  One backward per forward.  The first `n_in` tensors are the stage's inputs (the tape reads them again in the
-    backward, so the node keeps them), the rest its parameters."""
+    backward, so the node keeps them), the rest its parameters.  The backward follows torch.use_deterministic_algorithms as
+    _TrainFn's does."""
 
     @staticmethod
     def forward(ctx, stage, n_in, *tensors):
@@ -356,6 +359,7 @@ class _StageFn(torch.autograd.Function):
                                "or graph, or .to()): its activations are gone (one backward per forward)")
         g = [x.detach().to(torch.float32).contiguous() for x in grad_outs]
         grads = [torch.empty(s, dtype=torch.float32, device=g[0].device) for s in stage.shapes]
+        stage.plan.set_deterministic(torch.are_deterministic_algorithms_enabled())
         try:
             gin = stage.backward(ctx.tape, g, list(zip(stage.names, grads)))
         finally:  # consumed, or refused: either way the tape is done

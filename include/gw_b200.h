@@ -207,6 +207,18 @@ int gw_train_decoder_backward_tape(gw_plan* plan, gw_tape* tape, const float* gr
  * changing it between a forward and its backward is harmless.  gw_tape_bytes and gw_train_peak_bytes depend on the shapes and
  * this value only.  Values below -1 fail. */
 int gw_train_set_processor_segments(gw_plan* plan, int32_t segments);
+/* Replaces: torch.use_deterministic_algorithms(True) for the training backward (the Python layer sets it from
+ * torch.are_deterministic_algorithms_enabled() right before each backward).  on != 0: the backwards that start after this call,
+ * on either training step, sum every parameter gradient in an order that follows from the shapes alone, so that the same inputs,
+ * weights and plan give the same gradients bit for bit on every run.  It switches the CUDA-core weight gradient (every weight in
+ * GW_PREC_FP32_SIMT, Linears with at most 16 inputs in the tensor-core precisions) and the LayerNorm backward (every precision) from
+ * float atomics to per-slab / per-CTA partials in a plan-shared workspace of at most 32 MiB (allocated on first use, released by
+ * gw_plan_destroy) that a second kernel adds in order.  Every other part of the step already sums in a fixed order, and the
+ * forward has nothing to switch.  Off (the default): the atomic kernels, whose gradients repeat to ~1e-7 relative only.  The
+ * results of the two modes are not bit-equal to each other. */
+int gw_train_set_deterministic(gw_plan* plan, int32_t on);
+/* Device bytes of that workspace now (0 before the first backward with the flag on). */
+int64_t gw_train_deterministic_bytes(const gw_plan* plan);
 /* High-water mark, in bytes, of the training step's stream-ordered working allocations -- every live tape plus the running step's
  * temporaries -- since a training forward last began while no other tape held memory (0 before the first step).  For one tape at
  * a time: over the last gw_train_forward_tape and the gw_train_backward_tape after it.  It depends on the shapes only, unlike device-wide

@@ -4,7 +4,7 @@ GraphWeatherAssimilator or RegionalForecaster.
                                      [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16] [--feature-dim F] [--aux-dim A]
                                      [--num-blocks NB] [--width W] [--constraint-type none|additive|multiplicative|softmax]
                                      [--use-checkpointing] [--fit-batch] [--n-obs N] [--rollout K [--compare-plain]]
-                                     [--extent DEG] [--max-points N] [--moving-region] [--processor-segments S]
+                                     [--extent DEG] [--max-points N] [--moving-region] [--processor-segments S] [--deterministic]
 The model defaults to the README's 78 + 24 features, 9 blocks, 256-wide.  --model graphcast: GraphCast(input_dim = output_dim =
 --feature-dim, hidden_dim = --width or 256); its bounded step is selected by --use-checkpointing (the same step
 GraphCastConfig.balanced_checkpointing / full_checkpointing select).  --model assimilator: GraphWeatherAssimilator(output_lat_lons =
@@ -34,6 +34,8 @@ graphs on the host, creates its plans and uploads the graphs and weights, so the
 --processor-segments S: processor.set_checkpoint_segments(S) -- the backward recomputes the processor in segments of S blocks
 (-1: one segment) instead of keeping its tape; "tape_bytes" (gw_tape_bytes of every tape of the last step, read before its backward)
 shows what that saves.
+--deterministic: torch.use_deterministic_algorithms(True) for the whole run, so that every backward sums its parameter gradients in
+a fixed order (gw_train_set_deterministic); "deterministic_ws_bytes" is the fixed-order workspace the plan holds after the run.
 With --constraint-type the step includes PhysicalConstraintLayer; the constraint backward
 (gw_constraint_backward, no timing tag of the plan) is also timed on its own with CUDA events around it, on the step's shapes."""
 import argparse
@@ -107,6 +109,7 @@ def main():
     ap.add_argument("--max-points", type=int, default=2000, help="points per region (--model regional)")
     ap.add_argument("--moving-region", action="store_true", help="a new region for every step (--model regional)")
     ap.add_argument("--processor-segments", type=int, default=0, help="processor.set_checkpoint_segments(S): 0 none, N blocks, -1 one")
+    ap.add_argument("--deterministic", action="store_true", help="torch.use_deterministic_algorithms(True): bit-repeatable gradients")
     a = ap.parse_args()
     if a.model == "regional" and (a.rollout or a.fit_batch):
         ap.error("--model regional: no --rollout or --fit-batch")
@@ -174,6 +177,7 @@ def main():
                                        use_checkpointing=a.use_checkpointing, **dims).cuda().train()  # fmt: skip
         n_in, f_in = len(ll), F + a.aux_dim
     model.processor.set_checkpoint_segments(a.processor_segments)
+    torch.use_deterministic_algorithms(a.deterministic)
     crit = torch.nn.functional.mse_loss if a.model == "regional" else NormalizedMSELoss([1.0] * F, ll, normalize=True)
     opt = torch.optim.SGD(model.parameters(), lr=1e-3)
     tape_bytes = []  # gw_tape_bytes of every tape of the last step, read before its backward
@@ -266,6 +270,7 @@ def main():
     cbwd = constraint_backward_time(model, x, F) if a.constraint_type != "none" else None
     print(json.dumps({"what": "training step (fwd + loss + bwd + SGD)", "model": a.model, "train_precision": a.train_precision, "grid": None if a.model == "regional" else a.grid, "batch": a.batch,
                       "use_checkpointing": a.use_checkpointing, "processor_segments": a.processor_segments,
+                      "deterministic": a.deterministic, "deterministic_ws_bytes": plan.deterministic_bytes(),
                       "tape_bytes": list(tape_bytes), "rollout": rollout, "train_peak_gib": round(train_peak / 2**30, 3),
                       "plan_device_gib": round(plan_bytes / 2**30, 3),
                       "dims": dims, "constraint_type": a.constraint_type, "constraint_backward": cbwd,
