@@ -46,7 +46,7 @@ void gw_launch_count_reset(void) { gw::g_launches = 0; }
 // inference scratch and weight constants of a plan (gw_plan_create; a training-only plan holds none of it)
 static int alloc_inference_scratch(gw_plan* p, size_t chunk) {
   const gw_dims& d = p->d;
-  const bool tc = d.precision != GW_PREC_FP32_SIMT;
+  const bool tc = gw::is_fused(p);  // (a layer-by-layer plan has the CUDA-core path's scratch, and its assembled operands)
   const size_t Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, Hn = d.hidden_node;
   const size_t max_hid = std::max({Dn, De, He, Hn, (size_t)d.hidden_dec, (size_t)d.out_dim});
   const size_t max_rows = std::max({(size_t)d.n_in, (size_t)d.n_out, (size_t)d.n_mesh, (size_t)d.n_lat_edges, (size_t)d.n_dec_edges});
@@ -79,6 +79,8 @@ static int alloc_inference_scratch(gw_plan* p, size_t chunk) {
     rc |= p->agg_grid.alloc(chunk * d.n_out * De);
     rc |= p->seg_carry.alloc(std::max(chunk * dec_tiles, B * (lat_tiles + 1)) * 2048);  // [samples][tiles][8 row groups][256]
   }
+  if (p->layered)  // [x ; per-node sums of e'] of the encoder / processor node MLPs, per-point sums of the decoder's
+    rc |= p->cat.alloc(std::max(B * d.n_mesh * (Dn + De), chunk * d.n_out * De));
   return rc;
 }
 
@@ -93,10 +95,17 @@ static int plan_create(const gw_dims* dims, gw_plan** out_plan, bool train_only)
            "residual_dim must equal out_dim (the reference adds start features of the same width, decoder.py:93)");
   GW_CHECK(d.max_batch >= 1, "max_batch must be >= 1");
   GW_CHECK(d.precision == GW_PREC_FP32_SIMT || d.precision == GW_PREC_FP32_TC || d.precision == GW_PREC_BF16_TC, "unknown precision");
+  // tensor-core plans: the fused chains for the reference's default trunk (256-wide node / edge / hidden, 2 hidden layers), and
+  // for a trunk at least 256 wide with a width above 256 (train/run.py's 1024-wide model), a plan that runs the forward layer by
+  // layer as tensor-core column blocks, any number of hidden layers
+  const int trunk[4] = {d.node_dim, d.edge_dim, d.hidden_node, d.hidden_edge};
+  const bool wide = *std::min_element(trunk, trunk + 4) >= 256 && *std::max_element(trunk, trunk + 4) > 256;
   if (d.precision != GW_PREC_FP32_SIMT) {
-    GW_CHECK(d.node_dim == 256 && d.edge_dim == 256 && d.hidden_node == 256 && d.hidden_edge == 256,
-             "the tensor-core chains are built for 256-wide node/edge/hidden dims (the reference default); use fp32_simt otherwise");
-    GW_CHECK(d.hidden_layers_node == 2 && d.hidden_layers_edge == 2, "the tensor-core chains are built for hidden_layers = 2");
+    GW_CHECK(wide || (d.node_dim == 256 && d.edge_dim == 256 && d.hidden_node == 256 && d.hidden_edge == 256),
+             "the tensor-core precisions need node/edge/hidden dims of 256 (the reference default) or a trunk at least 256 wide with "
+             "one width above 256; use fp32_simt otherwise");
+    GW_CHECK(wide || (d.hidden_layers_node == 2 && d.hidden_layers_edge == 2),
+             "the tensor-core chains of the 256-wide trunk are built for hidden_layers = 2");
     int cc_major = 0, cc_minor = 0, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, dev);
@@ -112,6 +121,9 @@ static int plan_create(const gw_dims* dims, gw_plan** out_plan, bool train_only)
   std::unique_ptr<gw_plan> p(new gw_plan());  // a failure below frees the plan and whatever it already holds
   p->d = d;
   p->train_only = train_only;
+  p->layered = d.precision != GW_PREC_FP32_SIMT && wide;
+  p->row_images.tag = gw::TAG_CONST;
+  GW_CHECK(!(train_only && p->layered), "the training step's tensor-core precisions need the 256-wide trunk; use fp32_simt");
   GW_CUDA(cudaGetDevice(&p->device));
   const size_t Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, Hn = d.hidden_node;
   const size_t max_hid = std::max({Dn, De, He, Hn, (size_t)d.hidden_dec, (size_t)d.out_dim});
@@ -119,11 +131,12 @@ static int plan_create(const gw_dims* dims, gw_plan** out_plan, bool train_only)
   // chunking: keep the per-pass scratch of the lat/lon-sized stages under ~24 GB (an 80 GB H100 also holds the caller's tensors).  The tensor-core path never writes the
   // decoder's e' rows (their per-point sums are formed in the edge chain's epilogue), and its hidden activations stay on
   // the SM, so its per-sample scratch is three lat/lon-sized row buffers; the CUDA-core path also needs e' and the ping-pong.
-  const bool tc = d.precision != GW_PREC_FP32_SIMT;
+  const bool tc = gw::is_fused(p.get());
   const size_t n_io = std::max((size_t)d.n_in, (size_t)d.n_out);
   const size_t dec_tiles = ((size_t)d.n_dec_edges + 127) / 128;
   const size_t per_sample = tc ? (n_io * Dn + (size_t)d.n_in * De + (size_t)d.n_out * De + dec_tiles * 2048) * sizeof(float)
-                               : (2 * max_rows * max_hid + std::max((size_t)d.n_in, (size_t)d.n_dec_edges) * De + n_io * Dn) * sizeof(float);
+                               : (2 * max_rows * max_hid + std::max((size_t)d.n_in, (size_t)d.n_dec_edges) * De + n_io * Dn +
+                                  (p->layered ? (size_t)d.n_out * De : 0)) * sizeof(float);
   size_t chunk = std::max<size_t>(1, std::min<size_t>(d.max_batch, (24ull << 30) / std::max<size_t>(per_sample, 1)));
   if (const char* force = getenv("GW_B200_CHUNK")) {  // test knob: exercise the chunked stage loops on small grids
     const long v = atol(force);
@@ -299,7 +312,8 @@ int gw_plan_set_weights(gw_plan* p, const gw_param* params, int32_t n, void* str
   }
   GW_TRY(gw::bind_all(p));
   if (p->train_only) return 0;  // (the training step packs its own weight images and computes the constants it needs)
-  if (gw::is_tc(p)) GW_TRY(gw::pack_tc_weights(p, st));
+  if (gw::is_fused(p)) GW_TRY(gw::pack_tc_weights(p, st));
+  if (p->layered) p->row_images.new_weights(p->wbuf.p);  // (packed on their first use, by the constants below)
   GW_TRY(gw::precompute_constants(p, st));
   return 0;
 }

@@ -16,7 +16,104 @@
 
 namespace gw {
 
-int run_op(gw_plan* p, const GemmOp& op, cudaStream_t st) {
+// the image of the weight view W [N rows of stride ldw, K columns], packed at its first use after a weight upload
+static int row_image(gw_plan* p, RowImages& im, const float* W, int ldw, int K, int N, RowImages::Image** out, cudaStream_t st) {
+  const int parts = p->d.precision == GW_PREC_FP32_TC ? 2 : 1;
+  RowImages::Image& w = im.images[{W, ((long long)ldw << 40) | ((long long)K << 20) | N}];
+  if (w.stamp != im.stamp) {
+    const size_t bytes = tc_packed_bytes(K, N, parts);
+    if (w.img.n != bytes) GW_TRY(w.img.alloc(bytes));
+    if (w.amax.n != 1) GW_TRY(w.amax.alloc(1));
+    p->cur_tag = im.tag;
+    TimedLaunch tl(p, st);
+    GW_CUDA(launch_pack_image(W, ldw, K, N, parts, w.img.p, w.amax.p, st));
+    w.stamp = im.stamp;
+  }
+  *out = &w;
+  return 0;
+}
+
+int tc_row_op(gw_plan* p, RowImages& im, const GemmOp& op, float* out_bound, int tag, cudaStream_t st) {
+  GW_CHECK(!out_bound || op.ln_gamma, "tensor-core row op: a result bound is kept for LayerNorm'd rows only");
+  const bool ln_rows = op.ln_gamma && (op.N > TC_COL_BLOCK || out_bound);
+  GemmOp g = op;
+  if (ln_rows) {  // the blocks store the value entering the LayerNorm in out; launch_ln_rows finishes the rows in place
+    GW_CHECK(!op.save_pre, "tensor-core row op: no pre-LayerNorm store for a LayerNorm finished after the column blocks");
+    g.ln_gamma = g.ln_beta = nullptr, g.residual = RowSrc();
+  }
+  TcChain ch;
+  GW_CHECK(tc_row_op_chain(g, &ch) == cudaSuccess, "tensor-core row op: no chain for an add[2] addend or a missing a[0]");
+  for (int n0 = 0; n0 < op.N; n0 += TC_COL_BLOCK) {
+    const int nb = std::min(TC_COL_BLOCK, op.N - n0);
+    TcChain blk;
+    GW_CUDA(tc_column_block(ch, n0, nb, &blk));
+    RowImages::Image* w = nullptr;
+    GW_TRY(row_image(p, im, op.W + (size_t)n0 * op.ldw, op.ldw, op.K, nb, &w, st));
+    blk.layer[0].Wp = w->img.p, blk.layer[0].wamax = w->amax.p;
+    p->cur_tag = tag;
+    GW_TRY(run_chain(p, blk, st));
+  }
+  if (ln_rows) {
+    TimedLaunch t(p, st);
+    GW_CUDA(launch_ln_rows(op, out_bound, st));
+  }
+  return 0;
+}
+
+// Layer-by-layer plans: a stage-0 operand the chain kernel cannot read as it is -- two sources, or a segment sum -- is assembled
+// in p->cat first, and its bound measured: op then reads one bounded stream
+static int tc_flatten(gw_plan* p, GemmOp& op, cudaStream_t st) {
+  if (op.a[1].kind == SRC_NONE && op.a[0].kind != SRC_SEGSUM) return 0;
+  const int rows = op.rows_per_sample, K = op.K;
+  const size_t R = (size_t)rows * op.batch;
+  GW_CHECK(R * K <= p->cat.n, "layer-by-layer row op: assembled operand larger than the plan's scratch");
+  TimedLaunch t(p, st);
+  int col = 0;
+  for (int a = 0; a < 2; ++a) {
+    const RowSrc& s = op.a[a];
+    if (s.kind == SRC_NONE) continue;
+    float* dst = p->cat.p + col;
+    const size_t w = (size_t)s.width * sizeof(float), dpitch = (size_t)K * sizeof(float), spitch = (size_t)s.ld * sizeof(float);
+    if (s.kind == SRC_SEGSUM) {
+      GW_CUDA(launch_segsum(s.base + s.col0, s.ld, s.width, s.ptr, s.perm, s.src_rows, rows, op.batch, dst, K, st));
+    } else if (s.kind == SRC_STREAM && s.src_rows == rows) {
+      GW_CUDA(cudaMemcpy2DAsync(dst, dpitch, s.base + s.col0, spitch, w, R, cudaMemcpyDeviceToDevice, st));
+    } else if (s.kind == SRC_BCAST) {
+      for (int b = 0; b < op.batch; ++b)
+        GW_CUDA(cudaMemcpy2DAsync(dst + (size_t)b * rows * K, dpitch, s.base + s.col0, spitch, w, rows, cudaMemcpyDeviceToDevice, st));
+    } else {
+      GW_CHECK(false, "layer-by-layer row op: no assembly for this operand source");
+    }
+    col += s.width;
+  }
+  GW_CHECK(col == K, "layer-by-layer row op: operand sources do not add up to K");
+  GW_CUDA(cudaMemsetAsync(sl(p, SL_CAT), 0, sizeof(float), st));
+  GW_CUDA(launch_absmax_flat(p->cat.p, (long long)(R * K), sl(p, SL_CAT), st));
+  op.a[0] = bounded(src_stream(p->cat.p, K, K, rows), sl(p, SL_CAT));
+  op.a[1] = RowSrc();
+  return 0;
+}
+
+// layer-by-layer plans: a bound slot the LayerNorm'd rows written next accumulate into starts at zero
+static int zero_bound(gw_plan* p, float* b, cudaStream_t st) {
+  if (p->layered) GW_CUDA(cudaMemsetAsync(b, 0, sizeof(float), st));
+  return 0;
+}
+
+int run_op(gw_plan* p, const GemmOp& op_in, cudaStream_t st, float* out_bound) {
+  if (p->layered) {
+    GemmOp op = op_in;
+    GW_TRY(tc_flatten(p, op, st));
+    if (p->d.precision == GW_PREC_FP32_TC)  // the fp16 hi/lo split is scaled from a bound of its operand: measure one not known
+      for (int a = 0; a < 2; ++a)
+        if (op.a[a].kind != SRC_NONE && !op.a[a].bound) {
+          TimedLaunch t(p, st);
+          GW_CUDA(cudaMemsetAsync(sl(p, SL_OPA0 + a), 0, sizeof(float), st));
+          GW_CUDA(launch_operand_bound(op.a[a], op.rows_per_sample, op.batch, sl(p, SL_OPA0 + a), st));
+        }
+    return tc_row_op(p, p->row_images, op, out_bound, p->cur_tag, st);
+  }
+  const GemmOp& op = op_in;
   cudaError_t e;
   {
     TimedLaunch t(p, st);
@@ -54,6 +151,7 @@ int run_chain(gw_plan* p, TcChain& ch, cudaStream_t st) {
   return 0;
 }
 bool is_tc(const gw_plan* p) { return p->d.precision != GW_PREC_FP32_SIMT; }
+bool is_fused(const gw_plan* p) { return is_tc(p) && !p->layered; }
 
 // layer = Linear `w` (+ bias b[l] of MLP m when l >= 0) (+ ReLU); magnitudes for the operand-range ladder travel along
 static TcLayer tc_layer(const TcWeights& w, const Mlp* m, int l, bool relu, bool feeds) {
@@ -71,9 +169,9 @@ static void tc_out(TcLayer& L, float* out, int ldo, int cols, float* bound = nul
 // Runs an MLP whose first Linear is described by `first` (A sources / addends / weight slice already set; its
 // W/K/ldw/bias may have been overridden by the caller for factored layer 1) and whose remaining layers stream
 // through the ping-pong scratch.  If `first_is_virtual`, layer 0 has already been applied by the A-assembly of
-// `first` (decoder edge MLP: relu(P[src]+E1)) and `first` describes Linear 1.
+// `first` (decoder edge MLP: relu(P[src]+E1)) and `first` describes Linear 1.  out_bound: see run_op.
 static int run_mlp(gw_plan* p, const Mlp& m, GemmOp first, bool first_is_virtual, bool use_ln, const RowSrc& residual,
-                   float* out, int ldo, cudaStream_t st) {
+                   float* out, int ldo, cudaStream_t st, float* out_bound = nullptr) {
   const int rows = first.rows_per_sample, batch = first.batch;
   float* ping = p->bufA.p;
   float* pong = p->bufB.p;
@@ -97,7 +195,7 @@ static int run_mlp(gw_plan* p, const Mlp& m, GemmOp first, bool first_is_virtual
       op.residual = residual;
       op.out = out, op.ldo = ldo;
     }
-    GW_TRY(run_op(p, op, st));
+    GW_TRY(run_op(p, op, st, l == m.L && use_ln && p->layered ? out_bound : nullptr));
     std::swap(ping, pong);
   }
   return 0;
@@ -370,12 +468,13 @@ int stage_encoder(gw_plan* p, const float* features, float* x_out, float* x_out_
   const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, N = p->n_in_cur, H = d.n_mesh;
   RowSrc none;
   if (is_tc(p)) GW_CUDA(cudaMemsetAsync(sl(p, SL_FEAT), 0, sizeof(float), st));
+  GW_TRY(zero_bound(p, x_out_bound, st));
   for (int s0 = 0; s0 < nb; s0 += p->chunk) {
     const int cb = std::min(p->chunk, nb - s0);
     const float* f = features + (size_t)s0 * N * d.in_dim;
     float* xg = p->rows_n.p;
     float* eprime = p->rows_e.p;
-    if (is_tc(p)) {
+    if (is_fused(p)) {
       // chain 1 (lat/lon rows): node_encoder (3 layers + LN) -> edge MLP of the encoder block (W1s . h + C1, 2 layers + LN)
       // + e_enc residual -> e' rows.  Six GEMMs per row without leaving the SM.
       p->cur_tag = TAG_ENC_GRID;
@@ -437,17 +536,23 @@ int stage_encoder(gw_plan* p, const float* features, float* x_out, float* x_out_
       }
       continue;
     }
-    // node_encoder on the lat/lon rows (encoder.py:205); the mesh rows are the constant xm0
+    // node_encoder on the lat/lon rows (encoder.py:205); the mesh rows are the constant xm0.  (Layer-by-layer plans: the bounds
+    // below scale the tensor-core operands, and the features' one flags a non-finite input; the CUDA-core kernels ignore them.)
     p->cur_tag = TAG_ENC_GRID;
+    if (p->layered) {
+      TimedLaunch t(p, st);
+      GW_CUDA(launch_absmax_flat(f, (long long)cb * N * d.in_dim, sl(p, SL_FEAT), st));
+    }
+    GW_TRY(zero_bound(p, sl(p, SL_ROWS_N), st));
     {
       const Mlp& m = p->enc_node;
-      GemmOp fo = first_op(N, cb, src_stream(f, d.in_dim, d.in_dim, N), none, m.W[0], m.in[0], m.in[0], m.b[0]);
-      GW_TRY(run_mlp(p, m, fo, false, true, none, xg, Dn, st));
+      GemmOp fo = first_op(N, cb, bounded(src_stream(f, d.in_dim, d.in_dim, N), sl(p, SL_FEAT)), none, m.W[0], m.in[0], m.in[0], m.b[0]);
+      GW_TRY(run_mlp(p, m, fo, false, true, none, xg, Dn, st, sl(p, SL_ROWS_N)));
     }
     // edge update e' = LN(MLP([x_src ; x_dst ; e])) + e   (graph_net_block.py:131-135); dst and e terms are in C1_enc
     {
       const Mlp& m = p->enc_blk_edge;
-      GemmOp fo = first_op(N, cb, src_stream(xg, Dn, Dn, N), none, m.W[0], Dn, m.in[0], nullptr);
+      GemmOp fo = first_op(N, cb, bounded(src_stream(xg, Dn, Dn, N), sl(p, SL_ROWS_N)), none, m.W[0], Dn, m.in[0], nullptr);
       fo.add[0] = src_bcast(p->C1_enc.p, He, He);
       GW_TRY(run_mlp(p, m, fo, false, true, src_bcast(p->e_enc.p, De, De), eprime, De, st));
     }
@@ -457,7 +562,7 @@ int stage_encoder(gw_plan* p, const float* features, float* x_out, float* x_out_
       const Mlp& m = p->enc_blk_node;
       GemmOp fo = first_op(H, cb, src_bcast(p->xm0.p, Dn, Dn),
                            src_segsum(eprime, De, De, p->enc_ptr.p, p->enc_perm.p, N), m.W[0], m.in[0], m.in[0], m.b[0]);
-      GW_TRY(run_mlp(p, m, fo, false, true, src_bcast(p->xm0.p, Dn, Dn), x_out + (size_t)s0 * H * Dn, Dn, st));
+      GW_TRY(run_mlp(p, m, fo, false, true, src_bcast(p->xm0.p, Dn, Dn), x_out + (size_t)s0 * H * Dn, Dn, st, x_out_bound));
     }
   }
   return 0;
@@ -479,11 +584,11 @@ int stage_processor(gw_plan* p, const ProcGraph& g, const float* x_in, float* x_
   auto es = [&](const float* buf) { return sl(p, buf == eb[0] ? SL_E0 : SL_E1); };
   // the per-node sums of e' are produced by the edge chain itself when every node collects at most 8 edges (icosahedral
   // meshes: 6 or 7); longer segments (arbitrary caller graphs) keep the separate reduction kernel
-  const bool fuse = is_tc(p) && p->fuse_seg && g.maxdeg >= 1 && g.maxdeg <= 8;
+  const bool fuse = is_fused(p) && p->fuse_seg && g.maxdeg >= 1 && g.maxdeg <= 8;
   for (int k = 0; k < d.num_blocks; ++k) {
     const Mlp& me = p->proc_edge[k];
     const Mlp& mn = p->proc_node[k];
-    if (is_tc(p)) {
+    if (is_fused(p)) {
       const bool last = k == d.num_blocks - 1;
       float* e_next = eb[k & 1];
       float* x_next = last ? x_out : xb[k & 1];
@@ -572,7 +677,7 @@ int stage_processor(gw_plan* p, const ProcGraph& g, const float* x_in, float* x_
     for (int h = 0; h < 2; ++h) {
       GemmOp t;
       t.rows_per_sample = H, t.batch = nb;
-      t.a[0] = src_stream(x_cur, Dn, Dn, H);
+      t.a[0] = bounded(src_stream(x_cur, Dn, Dn, H), xs(x_cur));
       t.W = me.W[0] + h * Dn, t.K = Dn, t.ldw = me.in[0], t.N = He;
       t.out = p->P.p + h * He, t.ldo = 2 * He;
       GW_TRY(run_op(p, t, st));
@@ -580,12 +685,13 @@ int stage_processor(gw_plan* p, const ProcGraph& g, const float* x_in, float* x_
     float* e_next = eb[k & 1];
     p->cur_tag = TAG_PROC_EDGE;
     {
-      RowSrc e_src = e_cur ? src_stream(e_cur, De, De, El)
-                           : (g.e0_broadcast ? src_bcast(g.e0, De, De) : src_stream(g.e0, De, De, El));
+      RowSrc e_src = e_cur ? bounded(src_stream(e_cur, De, De, El), es(e_cur))
+                           : bounded(g.e0_broadcast ? src_bcast(g.e0, De, De) : src_stream(g.e0, De, De, El), g.e0_bound);
       GemmOp fo = first_op(El, nb, e_src, RowSrc(), me.W[0] + 2 * Dn, De, me.in[0], me.b[0]);
       fo.add[0] = src_gather(p->P.p, 2 * He, He, g.src, H, 0);
       fo.add[1] = src_gather(p->P.p, 2 * He, He, g.dst, H, He);
-      GW_TRY(run_mlp(p, me, fo, false, true, e_src, e_next, De, st));
+      GW_TRY(zero_bound(p, es(e_next), st));
+      GW_TRY(run_mlp(p, me, fo, false, true, e_src, e_next, De, st, es(e_next)));
     }
     float* x_next = (k == d.num_blocks - 1) ? x_out : xb[k & 1];
     if (x_next == x_cur) x_next = xb[(k & 1) ^ 1];  // never update in place: node and edge passes both read old x
@@ -593,12 +699,16 @@ int stage_processor(gw_plan* p, const ProcGraph& g, const float* x_in, float* x_
     {
       GemmOp fo = first_op(H, nb, src_stream(x_cur, Dn, Dn, H), src_segsum(e_next, De, De, g.ptr, nullptr, El),
                            mn.W[0], mn.in[0], mn.in[0], mn.b[0]);
-      GW_TRY(run_mlp(p, mn, fo, false, true, src_stream(x_cur, Dn, Dn, H), x_next, Dn, st));
+      GW_TRY(zero_bound(p, xs(x_next), st));
+      GW_TRY(run_mlp(p, mn, fo, false, true, src_stream(x_cur, Dn, Dn, H), x_next, Dn, st, xs(x_next)));
     }
     x_cur = x_next;
     e_cur = e_next;
   }
-  if (x_cur != x_out) GW_CUDA(cudaMemcpyAsync(x_out, x_cur, (size_t)nb * H * Dn * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (x_cur != x_out) {
+    GW_CUDA(cudaMemcpyAsync(x_out, x_cur, (size_t)nb * H * Dn * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (p->layered) GW_CUDA(cudaMemcpyAsync(sl(p, x_out_slot), xs(x_cur), sizeof(float), cudaMemcpyDeviceToDevice, st));
+  }
   return 0;
 }
 ProcGraph latent_graph_of(gw_plan* p) {
@@ -630,8 +740,9 @@ int stage_decoder(gw_plan* p, const float* x_in, int x_in_slot, const float* sta
   const gw_dims& d = p->d;
   const int Dn = d.node_dim, De = d.edge_dim, He = d.hidden_edge, H = d.n_mesh, Ed = d.n_dec_edges, No = d.n_out;
   RowSrc none;
-  const bool fuse = is_tc(p) && p->fuse_seg && p->dec_maxdeg >= 1 && p->dec_maxdeg <= 8;
-  GW_CHECK(p->out_mode == 0 || (is_tc(p) && p->tc_dec_out_ok), "the fused loss-boundary gather needs the tensor-core output chain");
+  const bool fuse = is_fused(p) && p->fuse_seg && p->dec_maxdeg >= 1 && p->dec_maxdeg <= 8;
+  GW_CHECK(p->out_mode == 0 || (is_fused(p) && p->tc_dec_out_ok),
+           "the fused loss-boundary gather needs the tensor-core output chain of the 256-wide trunk");
   if (!fuse) GW_TRY(ensure_rows_e(p, (size_t)p->chunk * std::max((size_t)p->d.n_in, (size_t)Ed) * De));
   for (int s0 = 0; s0 < nb; s0 += p->chunk) {
     const int cb = std::min(p->chunk, nb - s0);
@@ -640,7 +751,7 @@ int stage_decoder(gw_plan* p, const float* x_in, int x_in_slot, const float* sta
     float* eprime = p->rows_e.p;
     float* xg = p->rows_n.p;
     const Mlp& me = p->dec_blk_edge;
-    if (is_tc(p)) {
+    if (is_fused(p)) {
       const Mlp& mn = p->dec_blk_node;
       p->cur_tag = TAG_DEC_P;
       {
@@ -763,16 +874,21 @@ int stage_decoder(gw_plan* p, const float* x_in, int x_in_slot, const float* sta
     {  // Pd = x W1s^T ; the dst operand (lat/lon nodes) is identically zero, assimilator_decoder.py:84,189-193
       GemmOp t;
       t.rows_per_sample = H, t.batch = cb;
-      t.a[0] = src_stream(x, Dn, Dn, H);
+      t.a[0] = bounded(src_stream(x, Dn, Dn, H), sl(p, x_in_slot));
       t.W = me.W[0], t.K = Dn, t.ldw = me.in[0], t.N = He;
       t.out = Pd, t.ldo = He;
       GW_TRY(run_op(p, t, st));
+      if (p->layered) {  // (the bound of the gathered operand below: the mesh-sized Pd, measured)
+        TimedLaunch tl(p, st);
+        GW_TRY(raw_bound(p, SL_P, Pd, (long long)cb * H * He, st));
+      }
     }
     p->cur_tag = TAG_DEC_EDGE;
     {  // edge MLP: layer 1 output = relu(Pd[src] + E1_dec) is assembled on the fly as the A operand of layer 2
       GemmOp fo;
       fo.rows_per_sample = Ed, fo.batch = cb;
-      fo.a[0] = src_gather_bcast_relu(Pd, He, He, p->dec_src.p, H, p->E1_dec.p, He);
+      fo.a[0] = bounded(src_gather_bcast_relu(Pd, He, He, p->dec_src.p, H, p->E1_dec.p, He), sl(p, SL_P));
+      fo.a[0].bound2 = sl(p, SL_E1DEC);
       fo.W = me.W[1], fo.K = me.in[1], fo.ldw = me.in[1], fo.bias = me.b[1];
       GW_TRY(run_mlp(p, me, fo, true, true, src_bcast(p->e_dec.p, De, De), eprime, De, st));
     }
@@ -780,11 +896,12 @@ int stage_decoder(gw_plan* p, const float* x_in, int x_in_slot, const float* sta
     {  // lat/lon node update: cat([0 ; agg]) -> only the agg half of W1 contributes; residual x == 0
       const Mlp& mn = p->dec_blk_node;
       GemmOp fo = first_op(No, cb, src_segsum(eprime, De, De, p->dec_ptr.p, nullptr, Ed), none, mn.W[0] + Dn, De, mn.in[0], mn.b[0]);
-      GW_TRY(run_mlp(p, mn, fo, false, true, none, xg, Dn, st));
+      GW_TRY(zero_bound(p, sl(p, SL_ROWS_N), st));
+      GW_TRY(run_mlp(p, mn, fo, false, true, none, xg, Dn, st, sl(p, SL_ROWS_N)));
     }
     {  // node_decoder (no norm) + start-feature residual (decoder.py:93)
       const Mlp& m = p->dec_node_dec;
-      GemmOp fo = first_op(No, cb, src_stream(xg, Dn, Dn, No), none, m.W[0], m.in[0], m.in[0], m.b[0]);
+      GemmOp fo = first_op(No, cb, bounded(src_stream(xg, Dn, Dn, No), sl(p, SL_ROWS_N)), none, m.W[0], m.in[0], m.in[0], m.b[0]);
       RowSrc res;
       if (start && d.residual_dim > 0) res = src_stream(start + (size_t)s0 * No * start_ld, start_ld, d.out_dim, No);
       GW_TRY(run_mlp(p, m, fo, false, m.ln_g != nullptr, res, out + (size_t)s0 * No * out_ld, out_ld, st));

@@ -18,6 +18,10 @@ void set_error(const std::string& msg);
 
 // exact-fp32 CUDA-core execution of one row op (gw_simt.cu)
 cudaError_t launch_rowop_simt(const GemmOp& op, cudaStream_t stream);
+// The LayerNorm of a row op whose rows another kernel left in op.out as the value entering it: out = residual + LN(out) in place
+// over op.N columns (eps 1e-5, two passes like torch).  amax (optional, zeroed by the caller): *amax = max(*amax, max |out|), inf
+// if a row is not finite.
+cudaError_t launch_ln_rows(const GemmOp& op, float* amax, cudaStream_t stream);
 
 cudaError_t launch_pad_rows(const float* src, int ld_src, int width, float* dst, int ld_dst, long long rows, float* amax, cudaStream_t stream);
 cudaError_t launch_absmax_flat(const float* p, long long n, float* amax, cudaStream_t stream);
@@ -67,8 +71,9 @@ cudaError_t launch_segsum(const float* base, int ld, int width, const int32_t* p
 // wgmma chain kernel (gw_tc3.cu)
 cudaError_t launch_chain_tc3(const TcChain& ch, cudaStream_t stream);
 bool tc3_chain_is_lean(const TcChain& ch);  // would the launch take the lean (perm32, 256-bit access) path?
-// A one-layer chain computes at most TC_COL_BLOCK output columns.  Wider training row ops (the encoder's data gradient into the
-// features, the decoder's output layer) run as column blocks: tc_column_block turns the layer of `ch`, which describes all its
+// A one-layer chain computes at most TC_COL_BLOCK output columns.  Wider row ops (the training step's data gradient into the
+// features and the decoder's output layer; every layer of a trunk wider than 256 on a layer-by-layer plan) run as column blocks
+// (gw_forward.cu, tc_row_op): tc_column_block turns the layer of `ch`, which describes all its
 // outputs, into the chain of columns n0 .. n0 + nb - 1 (bias, addends, residual, mask, pre-LayerNorm store and output shifted
 // by n0 columns; stage-0 sources and their bounds shared).  The caller sets the block's weight image (W rows n0 .. n0 + nb - 1).
 // A layer with a LayerNorm cannot be split: cudaErrorInvalidValue.

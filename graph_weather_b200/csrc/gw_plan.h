@@ -89,6 +89,21 @@ struct DevBuf {  // owns its allocation: freed by the destructor, moved but neve
   size_t bytes() const { return n * sizeof(T); }
 };
 
+// Weight images of the one-layer tensor-core row ops (tc_row_op), keyed by (weight view, ldw, K, N): each is packed on its first
+// use after a weight upload (new_weights), its scale taken on the device.  The training step keeps one table, a layer-by-layer
+// inference plan another.
+struct RowImages {
+  struct Image { DevBuf<unsigned char> img; DevBuf<float> amax; int stamp = -1; };
+  std::map<std::pair<const float*, long long>, Image> images;
+  const float* of = nullptr;  // wbuf the images were made for (a re-allocated weight buffer drops them)
+  int stamp = 0;              // bumped once per weight upload
+  int tag = 0;                // timing tag (KernelTag) the packs are recorded under
+  void new_weights(const float* wbuf) {
+    if (of != wbuf) images.clear(), of = wbuf;
+    ++stamp;
+  }
+};
+
 struct TrainState;  // gw_train.cu
 
 }  // namespace gw
@@ -103,6 +118,11 @@ struct gw_plan {
   int train_segments = 0;           // processor segments of later training forwards (gw_train_set_processor_segments)
   bool train_deterministic = false; // fixed-order weight and LayerNorm-parameter gradients in later backwards (gw_train_set_deterministic)
   gw_dims d;
+  // a tensor-core plan for a trunk at least 256 wide with one width above 256 (any number of hidden layers): no fused chains; every
+  // row op of the CUDA-core stages runs as tensor-core column blocks (run_op -> tc_row_op), its weight images in row_images
+  bool layered = false;
+  gw::RowImages row_images;
+  DevBuf<float> cat;  // layered plans: an operand assembled from two sources or a segment sum, [rows, K] (tc_flatten)
   int device = 0;
   int n_in_cur = 0;
   unsigned enc_graph_gen = 0;  // bumped whenever the encoder graph is replaced (the training step's chunk tables are built per graph)
@@ -214,7 +234,9 @@ inline RowSrc src_gather_bcast_relu(const float* base, int ld, int width, const 
 
 // magnitude-bound slots (gw_plan::bounds)
 enum BoundSlot { SL_FEAT = 0, SL_XIN, SL_XOUT, SL_X0, SL_X1, SL_E0, SL_E1, SL_EIN, SL_P, SL_AGG_MESH, SL_AGG_GRID, SL_ROWS_N, SL_ROWS_E,
-                 SL_EENC, SL_C1ENC, SL_XM0, SL_ELAT, SL_EDEC, SL_E1DEC, SL_SDEC, SL_COUNT };
+                 SL_EENC, SL_C1ENC, SL_XM0, SL_ELAT, SL_EDEC, SL_E1DEC, SL_SDEC,
+                 SL_CAT, SL_OPA0, SL_OPA1,  // layered plans: the assembled operand, measured stage-0 sources of a row op
+                 SL_COUNT };
 inline float* sl(gw_plan* p, int i) { return p->bounds.p + i; }
 inline RowSrc bounded(RowSrc s, const float* b, float mul = 1.f) {
   s.bound = b, s.bound_mul = mul;
@@ -283,9 +305,17 @@ struct ProcGraph {
 };
 
 // gw_forward.cu
-int run_op(gw_plan* p, const GemmOp& op, cudaStream_t st);
+// One row op of the plan's forward: exact fp32 on CUDA cores, or tensor-core column blocks on a layer-by-layer plan.  out_bound
+// (layer-by-layer plans, LayerNorm'd ops only; zeroed by the caller): *out_bound = max(*out_bound, max |out|).
+int run_op(gw_plan* p, const GemmOp& op, cudaStream_t st, float* out_bound = nullptr);
+// One row op on the tensor cores: the one-layer chain of tc_row_op_chain, cut into column blocks of at most TC_COL_BLOCK outputs
+// (tc_column_block), each with the image of its rows of W from `im`.  The stage-0 sources carry their bounds (set by the caller).
+// A LayerNorm wider than TC_COL_BLOCK, or one whose out_bound is asked for, is finished by launch_ln_rows after the blocks
+// (which store the value entering it); that pass also takes *out_bound (as in run_op).  tag: the timing tag of the chains.
+int tc_row_op(gw_plan* p, RowImages& im, const GemmOp& op, float* out_bound, int tag, cudaStream_t st);
 int run_chain(gw_plan* p, TcChain& ch, cudaStream_t st);
 bool is_tc(const gw_plan* p);
+bool is_fused(const gw_plan* p);  // a tensor-core plan that runs the fused chains (the 256-wide trunk)
 int bind_all(gw_plan* p);
 int pack_tc_weights(gw_plan* p, cudaStream_t st);
 int precompute_encoder_constants(gw_plan* p, cudaStream_t st);

@@ -912,8 +912,11 @@ cudaError_t launch_seg_carry(const float* carry, const int32_t* seg_dst, int row
 
 // Rows wider than one CTA column block (N > 256, e.g. the 1024-wide models of train/run.py:491-501): the row op above runs
 // without its LayerNorm / residual and this kernel finishes the rows in place: out = residual + LN(out).  One warp per row,
-// two passes over the (L2-resident) row like torch's LayerNorm (mean, then biased variance, eps 1e-5).
-__global__ void __launch_bounds__(256) gw_ln_rows_kernel(const GemmOp op) {
+// two passes over the (L2-resident) row like torch's LayerNorm (mean, then biased variance, eps 1e-5).  The tensor-core row ops
+// of a layer-by-layer plan (gw_forward.cu, tc_row_op) finish their LayerNorm'd rows here too; amax (optional, zeroed by the
+// caller: a tensor written in chunks accumulates) then takes max |out| of the rows written, the bound the next layer's fp16 hi/lo split is scaled from (infinite when a
+// row is not finite).
+__global__ void __launch_bounds__(256) gw_ln_rows_kernel(const GemmOp op, float* __restrict__ amax) {
   const int lane = threadIdx.x & 31;
   const long long R = (long long)op.rows_per_sample * op.batch;
   const long long gr = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -934,11 +937,26 @@ __global__ void __launch_bounds__(256) gw_ln_rows_kernel(const GemmOp op) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
   const float rstd = 1.0f / sqrtf(q / (float)N + 1e-5f);
+  float m = 0.f;
   for (int c = lane; c < N; c += 32) {
     float x = (row[c] - mean) * rstd * __ldg(op.ln_gamma + c) + __ldg(op.ln_beta + c);
     if (op.residual.kind != SRC_NONE) x += fetch_src(op.residual, b, li, c);
     row[c] = x;
+    m = amax1(m, x);
   }
+  if (amax) {
+    if (!(m <= 3.0e38f)) m = __int_as_float(0x7f800000);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if (lane == 0) atomicMax(reinterpret_cast<int*>(amax), __float_as_int(m));  // m >= 0: int order == float order
+  }
+}
+cudaError_t launch_ln_rows(const GemmOp& op, float* amax, cudaStream_t stream) {
+  const long long R = (long long)op.rows_per_sample * op.batch;
+  if (R <= 0 || op.N <= 0) return cudaSuccess;
+  gw_ln_rows_kernel<<<(unsigned)((R + 7) / 8), 256, 0, stream>>>(op, amax);
+  count_launch();
+  return cudaGetLastError();
 }
 
 cudaError_t launch_rowop_simt(const GemmOp& op, cudaStream_t stream) {
@@ -950,7 +968,7 @@ cudaError_t launch_rowop_simt(const GemmOp& op, cudaStream_t stream) {
     g.ln_gamma = g.ln_beta = nullptr;
     g.residual = RowSrc();
     gw_rowop_f32_kernel<<<grid, NT, 0, stream>>>(g);
-    gw_ln_rows_kernel<<<(unsigned)((R + 7) / 8), 256, 0, stream>>>(op);
+    gw_ln_rows_kernel<<<(unsigned)((R + 7) / 8), 256, 0, stream>>>(op, nullptr);
     count_launch(2);
     return cudaGetLastError();
   }

@@ -141,11 +141,7 @@ struct TrainState {
   std::vector<GridRange> enc_chunks, dec_chunks;
   DevBuf<int32_t> enc_slot_sorted;  // mesh slot of every position of enc_perm
   DevBuf<int32_t> dec_cperm, dec_cptr;  // per decoder chunk: its edges sorted by source (chunk-local ids) and the CSR over mesh slots
-  // tensor-core precisions: weight images keyed by (weight view, ldw, K, N), repacked on their first use after a weight upload
-  struct TcImage { DevBuf<unsigned char> img; DevBuf<float> amax; int stamp = -1; };
-  std::map<std::pair<const float*, long long>, TcImage> images;
-  const float* images_of = nullptr;  // wbuf the images were made for (a re-allocated weight buffer drops them)
-  int stamp = 0;                     // bumped once per weight upload
+  RowImages images;      // tensor-core precisions: the weight images of the step's row ops (tc_row_op)
   DevBuf<float> bslots;  // operand magnitude bounds of the current phase (reset at the start of the forward and of the backward)
   size_t bslot_used = 0;
   DevBuf<float> wg_ws;   // gw_wgrad_tc.cu partial sums
@@ -223,23 +219,6 @@ static float* grad_of(gw_plan* p, TrainState* T, const float* w) { return T->gbu
 
 static bool split_of(const gw_plan* p) { return p->d.precision == GW_PREC_FP32_TC; }
 
-// the operand image of the weight view W, packed at its first use after a weight upload [N rows of stride ldw, K columns] (tensor-core precisions)
-static int train_image(gw_plan* p, TrainState* T, const float* W, int ldw, int K, int N, TrainState::TcImage** out) {
-  const int parts = split_of(p) ? 2 : 1;
-  TrainState::TcImage& im = T->images[{W, ((long long)ldw << 40) | ((long long)K << 20) | N}];
-  if (im.stamp != T->stamp) {
-    const size_t bytes = tc_packed_bytes(K, N, parts);
-    if (im.img.n != bytes) GW_TRY(im.img.alloc(bytes));
-    if (im.amax.n != 1) GW_TRY(im.amax.alloc(1));
-    p->cur_tag = TAG_TRAIN_WEIGHTS;
-    TimedLaunch tl(p, T->st);
-    GW_CUDA(launch_pack_image(W, ldw, K, N, parts, im.img.p, im.amax.p, T->st));
-    im.stamp = T->stamp;
-  }
-  *out = &im;
-  return 0;
-}
-
 // device bound of a chain's stage-0 source (fp32 mode), in the next operand-bound slot
 static int operand_bound(gw_plan* p, TrainState* T, RowSrc& s, int rows, int batch) {
   GW_CHECK(T->bslot_used < T->bslots.n, "training step: out of operand-bound slots");
@@ -250,33 +229,22 @@ static int operand_bound(gw_plan* p, TrainState* T, RowSrc& s, int rows, int bat
   return 0;
 }
 
-// One row op of the step: exact fp32 on CUDA cores (fp32_simt plans) or one-layer wgmma chains (tensor-core plans: tc_row_op_chain),
-// one per block of TC_COL_BLOCK output columns (tc_column_block; each block has the weight image of its rows of W, the stage-0
-// operand and its bound are shared).  tag: the phase it is timed under (train_fwd / train_dgrad).  reads_input: the op's stage-0
-// operand is the caller's features; bf16 plans bound it too (fp32 plans bound every operand), so that an inf / NaN feature sets
-// status bit 3 in every tensor-core precision instead of passing through the epilogue's ReLU as a finite number.
+// One row op of the step: exact fp32 on CUDA cores (fp32_simt plans) or one-layer wgmma chains in column blocks (tensor-core
+// plans: tc_row_op; the stage-0 operand and its bound are shared by the blocks).  tag: the phase it is timed under (train_fwd /
+// train_dgrad).  reads_input: the op's stage-0 operand is the caller's features; bf16 plans bound it too (fp32 plans bound every
+// operand), so that an inf / NaN feature sets status bit 3 in every tensor-core precision instead of passing through the
+// epilogue's ReLU as a finite number.
 static int train_op(gw_plan* p, TrainState* T, GemmOp op, int tag, bool reads_input = false) {
   if (!is_tc(p)) {
     p->cur_tag = tag;
     return run_op(p, op, T->st);
   }
-  TcChain ch;
-  GW_CHECK(tc_row_op_chain(op, &ch) == cudaSuccess,
+  GW_CHECK(op.add[2].kind == SRC_NONE && op.a[0].kind != SRC_NONE && !(op.ln_gamma && op.N > TC_COL_BLOCK),
            "training row op: no tensor-core chain for an add[2] addend, a missing a[0] or a LayerNorm wider than 256 columns");
   if (split_of(p) || reads_input)
     for (int a = 0; a < 2; ++a)
-      if (ch.a0[a].kind != SRC_NONE) GW_TRY(operand_bound(p, T, ch.a0[a], op.rows_per_sample, op.batch));
-  for (int n0 = 0; n0 < op.N; n0 += TC_COL_BLOCK) {
-    const int nb = std::min(TC_COL_BLOCK, op.N - n0);
-    TcChain blk;
-    GW_CUDA(tc_column_block(ch, n0, nb, &blk));
-    TrainState::TcImage* im = nullptr;
-    GW_TRY(train_image(p, T, op.W + (size_t)n0 * op.ldw, op.ldw, op.K, nb, &im));
-    blk.layer[0].Wp = im->img.p, blk.layer[0].wamax = im->amax.p;
-    p->cur_tag = tag;
-    GW_TRY(run_chain(p, blk, T->st));
-  }
-  return 0;
+      if (op.a[a].kind != SRC_NONE) GW_TRY(operand_bound(p, T, op.a[a], op.rows_per_sample, op.batch));
+  return tc_row_op(p, T->images, op, nullptr, tag, T->st);
 }
 
 static int det_workspace(TrainState* T, size_t floats) {
@@ -503,12 +471,9 @@ static int train_prepare(gw_plan* p, TrainState* T, int batch, int need, cudaStr
         GW_CUDA(launch_transpose(kv.second.first, (int)r, (int)c, T->wT.p + (kv.second.first - p->wbuf.p), st));
       }
     }
-    if (is_tc(p)) {  // the weight images of these weights are packed on first use (train_image)
-      if (T->images_of != p->wbuf.p) {
-        T->images.clear();
-        T->images_of = p->wbuf.p;
-      }
-      ++T->stamp;
+    if (is_tc(p)) {  // the weight images of these weights are packed on first use (tc_row_op)
+      T->images.tag = TAG_TRAIN_WEIGHTS;
+      T->images.new_weights(p->wbuf.p);
     }
     T->wgen = p->wgen;
   }

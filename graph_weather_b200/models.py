@@ -122,14 +122,22 @@ def _tc_eligible(dims: dict) -> bool:
             and dims.get("hidden_edge") == 256 and dims.get("hidden_layers_node") == 2 and dims.get("hidden_layers_edge") == 2)  # fmt: skip
 
 
+def _tc_layered(dims: dict) -> bool:
+    """A trunk the tensor cores run layer by layer: every node / edge / hidden width at least 256 and one above 256 (train/run.py's
+    1024-wide model), any number of hidden layers."""
+    w = [dims.get(k, 0) for k in ("node_dim", "edge_dim", "hidden_node", "hidden_edge")]
+    return min(w) >= 256 and max(w) > 256
+
+
 def _validate_precision(precision: str, dims: dict):
     """Constructor-time check, so that an impossible request fails where the module is built, not at the first forward."""
     if precision not in ("auto",) + tuple(_capi.PRECISIONS):
         raise ValueError(f"precision={precision!r}: expected one of 'auto', {sorted(_capi.PRECISIONS)}")
-    if precision in ("fp32", "fp32_tc", "bf16") and not _tc_eligible(dims):
+    if precision in ("fp32", "fp32_tc", "bf16") and not (_tc_eligible(dims) or _tc_layered(dims)):
         raise ValueError(
-            f"precision={precision!r} runs the tensor-core chains, which are built for node/edge/hidden dims of 256 and 2 hidden "
-            "layers (the reference defaults); use precision='auto' (CUDA-core exact fp32 for other sizes) or 'fp32_simt'"
+            f"precision={precision!r} runs the tensor cores: the fused chains need node/edge/hidden dims of 256 and 2 hidden layers "
+            "(the reference defaults), the layer-by-layer forward a trunk at least 256 wide with one width above 256; use "
+            "precision='auto' (CUDA-core exact fp32 for other sizes) or 'fp32_simt'"
         )
 
 
