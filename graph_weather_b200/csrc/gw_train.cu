@@ -26,12 +26,15 @@
 //
 // Stages: the step is three stage functions (enc_stage_* / proc_stage_* / dec_stage_*) with explicit boundary tensors; the whole
 // network's forward and backward compose them, and the reference's standalone Encoder / Processor / Decoder train on one stage
-// alone (gw_train_{encoder,processor,decoder}_{forward,backward}_tape).
+// alone (gw_train_{encoder,processor,decoder}_{forward,backward}_tape).  A standalone encoder or decoder takes the step of its plan,
+// taped or chunked, as the whole network does; its plan holds only its own graphs, and build_chunks cuts only their tables.
 //
 // Memory: the grid-sized phases (the encoder's lat/lon side, the decoder) are written once over a GridRange.  The taped step runs
 // each on one whole range and keeps its tape from the forward.  A training-only plan (gw_plan_create_train, use_checkpointing=True)
 // runs them chunk by chunk: the forward keeps only agg_m and the output rows, and the backward recomputes each chunk's tape with the
-// same ops (and, in fp32 mode, the same per-chunk operand bounds) just before that chunk's backward, then frees it.  Processor
+// same ops (and, in fp32 mode, the same per-chunk operand bounds) just before that chunk's backward, then frees it.  A standalone
+// stage's chunks read the caller's rows (features; the decoder's x and residual rows) again through the forward's own row sources,
+// which the caller keeps alive until the backward.  Processor
 // segments (gw_train_set_processor_segments, either step) do the same for the mesh-sized processor: the forward keeps x and e at the
 // start of every segment, and the backward recomputes a segment's blocks with block_fwd right before their block_bwd.
 //
@@ -382,11 +385,21 @@ static int chunk_points(const gw_plan* p, int batch, double rows_per_point) {
 // The decoder tables are built once per batch size.  The encoder tables are built per batch size and encoder graph (gw_plan::
 // enc_graph_gen): the assimilator's observation graph changes on every call, and chunks of an earlier graph would cover the wrong
 // points.  Building them copies enc_ptr to the host, so a step whose encoder graph changed synchronises its stream once (every
-// bounded step of the assimilator; the taped step builds no chunk tables).
+// bounded step of the assimilator and of a standalone AssimilatorEncoder; the taped step builds no chunk tables).  Only the tables
+// of the stages the plan holds are built: a standalone encoder's plan has no decoder graph, a standalone decoder's no encoder graph.
+// Both phases index iota: encoder chunks by mesh slot, decoder chunks by point.
 static int build_chunks(gw_plan* p, TrainState* T, int batch) {
   const gw_dims& d = p->d;
   const int H = d.n_mesh, N = p->n_in_cur, No = d.n_out, Ed = d.n_dec_edges;
-  if (T->enc_chunks_batch != batch || T->enc_chunks_gen != p->enc_graph_gen) {
+  const size_t n_iota = std::max(p->have_enc ? H : 0, p->have_dec ? No : 0);
+  if (T->iota.n < n_iota) {
+    std::vector<int32_t> iota(n_iota);
+    for (size_t i = 0; i < iota.size(); ++i) iota[i] = (int32_t)i;
+    GW_TRY(T->iota.alloc(iota.size()));
+    GW_CUDA(cudaMemcpyAsync(T->iota.p, iota.data(), iota.size() * sizeof(int32_t), cudaMemcpyHostToDevice, T->st));
+    GW_CUDA(cudaStreamSynchronize(T->st));  // (the copy reads `iota`, which goes out of scope with this block)
+  }
+  if (p->have_enc && (T->enc_chunks_batch != batch || T->enc_chunks_gen != p->enc_graph_gen)) {
     std::vector<int32_t> eptr(H + 1), slot(std::max(N, 1));
     GW_CUDA(cudaMemcpyAsync(eptr.data(), p->enc_ptr.p, (H + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, T->st));
     GW_CUDA(cudaStreamSynchronize(T->st));
@@ -416,14 +429,10 @@ static int build_chunks(gw_plan* p, TrainState* T, int batch) {
     GW_CHECK(most <= INT32_MAX, "training step: one chunk of the grid-sized stages holds more than 2^31 rows (lower the batch)");
     T->enc_chunks_batch = batch, T->enc_chunks_gen = p->enc_graph_gen;
   }
-  if (T->dec_chunks_batch != batch) {
-    std::vector<int32_t> dptr(No + 1), iota(std::max(No, H));
+  if (p->have_dec && T->dec_chunks_batch != batch) {
+    std::vector<int32_t> dptr(No + 1);
     GW_CUDA(cudaMemcpyAsync(dptr.data(), p->dec_ptr.p, (No + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, T->st));
     GW_CUDA(cudaStreamSynchronize(T->st));
-    for (size_t i = 0; i < iota.size(); ++i) iota[i] = (int32_t)i;
-    if (T->iota.n < iota.size()) GW_TRY(T->iota.alloc(iota.size()));
-    GW_CUDA(cudaMemcpyAsync(T->iota.p, iota.data(), iota.size() * sizeof(int32_t), cudaMemcpyHostToDevice, T->st));
-    GW_CUDA(cudaStreamSynchronize(T->st));  // (the copy reads `iota`, which goes out of scope with this block)
     long long most = 0;
     T->dec_chunks.clear();
     const int pd = chunk_points(p, batch, (double)Ed / std::max(No, 1));
@@ -1313,14 +1322,16 @@ int gw_train_backward_tape(gw_plan* p, gw_tape* k, const float* grad_out, float*
   return hand_out_grads(p, grads, n, "gw_train_backward_tape", st);
 }
 
-// the stages alone: the taped step of a gw_plan_create plan
-static const char* const kStagePlan = "the stage training calls run the taped step: they need a gw_plan_create plan, not a training-only one";
+// The stages alone.  The encoder and decoder run the step of their plan: the taped step on a gw_plan_create plan, the bounded one
+// on a training-only plan (their grid-sized work chunked as in the whole network).  The processor has no grid-sized work, so its
+// bounded step would be its taped one; its memory is bounded by processor segments, and it takes a gw_plan_create plan only.
+static const char* const kProcPlan = "the processor's training calls run the taped step: they need a gw_plan_create plan, not a training-only one "
+                                     "(bound its memory with gw_train_set_processor_segments)";
 
 int gw_train_encoder_forward_tape(gw_plan* p, gw_tape* k, const float* features, float* x_out, float* e_lat_out, int32_t batch, void* stream) {
   GW_TRY(check_tape(p, k));
   GW_TRY(gw::check_ready(p, batch, gw::NEED_ENC));
   GW_CHECK(features && x_out && e_lat_out, "null argument");
-  GW_CHECK(!p->train_only, kStagePlan);
   cudaStream_t st = (cudaStream_t)stream;
   const int rc = gw::encoder_forward(p, p->train, k, features, x_out, e_lat_out, batch, st);
   if (rc) gw::tape_release(p->train, k, st);
@@ -1343,7 +1354,7 @@ int gw_train_processor_forward_tape(gw_plan* p, gw_tape* k, const float* x_in, f
   GW_TRY(gw::check_ready(p, 1, gw::NEED_PROC));
   GW_CHECK(x_in && x_out && edge_attr && src && dst && ptr, "null argument");
   GW_CHECK(x_out != x_in, "the training forward reads x_in again in its backward: x_out must be another buffer");
-  GW_CHECK(!p->train_only, kStagePlan);
+  GW_CHECK(!p->train_only, kProcPlan);
   GW_CHECK(n_nodes >= 1 && n_edges >= 1, "the graph needs at least one node and one edge");
   cudaStream_t st = (cudaStream_t)stream;
   const int rc = gw::processor_forward(p, p->train, k, x_in, x_out, edge_attr, n_nodes, n_edges, src, dst, ptr, st);
@@ -1367,7 +1378,6 @@ int gw_train_decoder_forward_tape(gw_plan* p, gw_tape* k, const float* x_in, con
   GW_TRY(gw::check_ready(p, batch, gw::NEED_DEC));
   GW_CHECK(x_in && out, "null argument");
   GW_CHECK(p->d.residual_dim == 0 || (start_features && start_ld >= p->d.residual_dim), "start features required (decoder.py:93)");
-  GW_CHECK(!p->train_only, kStagePlan);
   cudaStream_t st = (cudaStream_t)stream;
   const int rc = gw::decoder_forward(p, p->train, k, x_in, start_features, start_ld, out, batch, st);
   if (rc) gw::tape_release(p->train, k, st);

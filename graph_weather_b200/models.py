@@ -363,8 +363,8 @@ class _StageFn(torch.autograd.Function):
             raise RuntimeError("graph_weather_b200: backward of a sub-module's training forward whose activations were consumed by an "
                                "earlier backward (one backward per forward)")
         if stage.eng.plan is not stage.plan:
-            raise RuntimeError("graph_weather_b200: backward of a sub-module's training forward whose plan was replaced (a larger batch "
-                               "or graph, or .to()): its activations are gone (one backward per forward)")
+            raise RuntimeError("graph_weather_b200: backward of a sub-module's training forward whose plan was replaced (a switch of the "
+                               "training step, a larger batch or graph, or .to()): its activations are gone (one backward per forward)")
         g = [x.detach().to(torch.float32).contiguous() for x in grad_outs]
         grads = [torch.empty(s, dtype=torch.float32, device=g[0].device) for s in stage.shapes]
         stage.plan.set_deterministic(torch.are_deterministic_algorithms_enabled())
@@ -385,13 +385,17 @@ def _stage_wants_grad(module, *inputs):
             and (any(t is not None and t.requires_grad for t in inputs) or any(q.requires_grad for q in module.parameters())))  # fmt: skip
 
 
-def _stage_engine(module, dims, uploaders) -> _Engine:
-    """The training engine of a standalone sub-module, of precision `train_precision` (created on first use; its inference engine
-    stays as it is).  It runs the taped step: the bounded-memory step of use_checkpointing=True is the wrappers' alone."""
-    eng = module.__dict__.get("_train_engine")
-    if eng is None:
-        eng = _new_engine(dims, module.train_precision, uploaders)
-        module.__dict__["_train_engine"] = eng
+def _stage_engine(module, dims, uploaders, bounded=False) -> _Engine:
+    """The training engine of a standalone sub-module, of precision `train_precision`; its inference engine stays as it is.
+    `bounded` (the Encoder's and decoders' use_checkpointing, read at every training forward) selects the step as a wrapper's
+    `_bounded_step()` does: a training-only plan whose step keeps only the mesh-sized activations and recomputes the lat/lon side
+    chunk by chunk in the backward, or the taped step (the default).  One engine per step, each created on first use; switching
+    closes the other's plan (`_switch_training_engine`).  The chosen engine is `module._train_engine`."""
+    def make(b):
+        return _new_engine(dims, module.train_precision, uploaders, train_only=b)
+
+    eng = _switch_training_engine(module.__dict__.setdefault("_train_engines", {}), bool(bounded), make)
+    module.__dict__["_train_engine"] = eng
     return eng
 
 
@@ -457,10 +461,12 @@ class Encoder(nn.Module):
                  efficient_batching: bool = False, precision: str = "auto", train_precision: Optional[str] = None):  # fmt: skip
         """encoder.py:36-151.  train_precision=None (the default) keeps the module inference-only: its output has no autograd graph.
         'fp32_simt' | 'fp32' | 'bf16' (as for GraphWeatherForecaster) make a train-mode call with autograd on run the encoder's
-        training step, so that `x` and `edge_attr` carry gradients to the features and every parameter.  That is the taped step;
-        use_checkpointing does not bound it here."""
+        training step, so that `x` and `edge_attr` carry gradients to the features and every parameter.  use_checkpointing, read
+        at every training forward, selects the step as for GraphWeatherForecaster: False (the default) the taped step, True the
+        bounded-memory step, which keeps only the mesh-sized activations and recomputes the lat/lon side chunk by chunk in the
+        backward (the 0.25 degree grid trains on one 80 GB card)."""
         super().__init__()
-        self.use_checkpointing = use_checkpointing  # accepted for API parity; GraphWeatherForecaster(use_checkpointing=True) selects its bounded-memory training step
+        self.use_checkpointing = use_checkpointing  # with a train_precision: the bounded-memory training step (_stage_engine)
         self.efficient_batching = efficient_batching
         self.output_dim = output_dim
         self.num_latlons = len(lat_lons)
@@ -521,7 +527,7 @@ class Encoder(nn.Module):
         both differentiable.  edge_attr is formed from the sorted latent edge features by torch ops (the inverse of the plan's
         edge order, then one copy per sample), so autograd sums the copies' gradients.  lat_lon_heights gets no gradient."""
         B = features.shape[0]
-        eng = _stage_engine(self, self._dims, [self._upload_graphs])
+        eng = _stage_engine(self, self._dims, [self._upload_graphs], self.use_checkpointing)
         grow = None if lat_lon_heights is None else dict(n_in=lat_lon_heights.shape[0])
         plan = eng.ensure(features.device, B, _prefixed("encoder", self), grow=grow)
         if lat_lon_heights is not None:
@@ -583,8 +589,9 @@ class Processor(nn.Module):
         """processor.py:17-68.  train_precision=None (the default) keeps the module inference-only.  'fp32_simt' | 'fp32' | 'bf16'
         make a train-mode call with autograd on run the processor's training step on the call's graph: `x`, `edge_attr` (in the
         caller's edge order) and every parameter get gradients, with `checkpoint_segments` read at every call.  Each call keeps its
-        own tape, so a processor applied several times in one graph back-propagates through every call.  That is the taped step;
-        use_checkpointing does not bound it here."""
+        own tape, so a processor applied several times in one graph back-propagates through every call.  The processor has no
+        grid-sized work: it always takes the taped step, and `set_checkpoint_segments` bounds its memory (use_checkpointing is
+        passed on to the GraphProcessor, as in the reference)."""
         super().__init__()
         if use_thermalizer:
             raise NotImplementedError("use_thermalizer=True: the stochastic ThermalizerLayer is outside the accelerated path")
@@ -682,8 +689,9 @@ class AssimilatorDecoder(nn.Module):
                  precision: str = "auto", train_precision: Optional[str] = None):  # fmt: skip
         """assimilator_decoder.py:36-129 (Decoder: decoder.py:24-77).  train_precision=None (the default) keeps the module
         inference-only.  'fp32_simt' | 'fp32' | 'bf16' make a train-mode call with autograd on run the decoder's training step:
-        processor_features, start_features (the Decoder's residual) and every parameter get gradients.  That is the taped step;
-        use_checkpointing does not bound it here."""
+        processor_features, start_features (the Decoder's residual) and every parameter get gradients.  use_checkpointing, read at
+        every training forward, selects the step as for Encoder: True keeps only the mesh-sized activations and recomputes the
+        decoder chunk by chunk in the backward."""
         super().__init__()
         self.use_checkpointing = use_checkpointing
         self.efficient_batching = efficient_batching
@@ -734,7 +742,8 @@ class AssimilatorDecoder(nn.Module):
         if x.numel() != batch_size * self.num_h3 * self._dims["node_dim"]:
             raise RuntimeError(f"processor_features: expected {batch_size} x {self.num_h3} mesh rows of width {self._dims['node_dim']}, "
                                f"got {tuple(processor_features.shape)}")  # fmt: skip
-        eng = _stage_engine(self, dict(self._dims, residual_dim=self.output_dim if self._residual else 0), [self._upload_graphs])
+        eng = _stage_engine(self, dict(self._dims, residual_dim=self.output_dim if self._residual else 0), [self._upload_graphs],
+                            self.use_checkpointing)  # fmt: skip
         plan = eng.ensure(x.device, batch_size, _prefixed("decoder", self))
         out_shape, x_shape = (batch_size, self.num_latlons, self.output_dim), tuple(x.shape)
 
@@ -787,7 +796,8 @@ class AssimilatorEncoder(nn.Module):
         """assimilator_encoder.py:36-168.  train_precision as for Encoder: None keeps the module inference-only; a value makes a
         train-mode call with autograd on differentiable in the observation values and every parameter (not in lat_lon_heights).
         The observation graph belongs to the plan, so of two training forwards alive at once only the later one can run its
-        backward (the earlier one's raises)."""
+        backward (the earlier one's raises).  use_checkpointing selects the bounded-memory step as for Encoder; as the observation
+        graph changes with every call, each bounded step copies its slot table to the host once to cut the chunks."""
         super().__init__()
         self.use_checkpointing = use_checkpointing
         self.output_dim = output_dim

@@ -74,7 +74,8 @@ int gw_plan_create(const gw_dims* dims, gw_plan** out_plan);
 int gw_plan_destroy(gw_plan* plan);
 /* A plan for training only (GraphWeatherForecaster(use_checkpointing=True)): graphs, weights and the training state, none of
  * the inference scratch, packed inference weights or weight constants.  gw_plan_set_weights on it binds the weights only;
- * gw_forward, gw_forward_strided, the stage entry points and gw_latent_edge_features on it fail.  Its training step is the
+ * gw_forward, gw_forward_strided, the stage entry points and gw_latent_edge_features on it fail.  Its training step (the
+ * whole network's, and the standalone encoder's and decoder's, gw_train_{encoder,decoder}_*_tape) is the
  * bounded-memory one: gw_train_forward_tape keeps only the mesh-sized activations and the output, and gw_train_backward_tape recomputes
  * the grid-sized stages (the encoder's lat/lon side, the decoder) chunk by chunk with the forward's own ops, releasing each
  * chunk's temporaries before the next.  Its peak working memory grows with the grid by at most one chunk.  Chunks hold a fixed
@@ -164,8 +165,12 @@ int gw_train_forward_tape(gw_plan* plan, gw_tape* tape, const float* features, f
 int gw_train_backward_tape(gw_plan* plan, gw_tape* tape, const float* grad_out, float* grad_features, const gw_param* grads,
                            int32_t n, void* stream);
 int64_t gw_tape_bytes(const gw_tape* tape);
-/* The training step of one stage alone, on a tape of a gw_plan_create plan that holds that stage (the reference's sub-modules are
- * ordinary differentiable modules, tests/test_model.py:20-119).  Replaces the autograd backward of Encoder.forward (encoder.py:153-242)
+/* The training step of one stage alone, on a tape of a plan that holds that stage (the reference's sub-modules are ordinary
+ * differentiable modules, tests/test_model.py:20-119).  The encoder and decoder calls run the step of their plan: the taped step on
+ * a gw_plan_create plan; on a gw_plan_create_train plan the bounded-memory step (Encoder / Decoder(use_checkpointing=True)), whose
+ * forward keeps only the mesh-sized activations and whose backward recomputes the lat/lon side chunk by chunk, as the whole
+ * network's.  The processor calls take a gw_plan_create plan only: the processor has no grid-sized work, and
+ * gw_train_set_processor_segments bounds its memory.  Replaces the autograd backward of Encoder.forward (encoder.py:153-242)
  * and AssimilatorEncoder.forward (assimilator_encoder.py:118-168), Processor.forward (processor.py:83-128), Decoder.forward
  * (decoder.py:79-94) and AssimilatorDecoder.forward (assimilator_decoder.py:131-200).  The whole-network step above is these three
  * stages composed.  Conventions as for gw_train_forward_tape / gw_train_backward_tape: one backward per forward, on the tape of a
@@ -178,13 +183,15 @@ int64_t gw_tape_bytes(const gw_tape* tape);
  *              latent edge features in the plan's target-sorted order, as gw_latent_edge_features returns them (the reference
  *              repeats them per sample).  Backward: grad_x, grad_e_lat (summed over the samples; NULL: zero) -> parameter gradients
  *              and, unless grad_features is NULL, the features' gradient.  A backward fails once the encoder graph was replaced
- *              after its forward (the assimilator's per-call observation graph).
+ *              after its forward (the assimilator's per-call observation graph).  On a training-only plan, a forward on a new
+ *              encoder graph copies its slot CSR to the host once to cut the chunks (a stream synchronisation per observation set).
  *   processor  on a caller-supplied graph, as gw_processor_forward_graph (copied onto the tape with its source-sorted CSR, so it
  *              may change on every call); x_out must not alias x_in.  Backward: grad_x_out [n_nodes, node_dim] -> parameter
  *              gradients, grad_x_in [n_nodes, node_dim] and grad_edge_attr [n_edges, edge_dim] per edge (either may be NULL).
  *   decoder    x_in [batch*n_mesh, node_dim] (+ start_features [batch, n_out, start_ld] when the plan has a residual) -> out.
  *              Backward: grad_out [batch, n_out, out_dim] -> parameter gradients and grad_x_in (NULL: none).  The residual's
- *              gradient, grad_out itself, is the caller's to add to start_features' gradient. */
+ *              gradient, grad_out itself, is the caller's to add to start_features' gradient.  On a training-only plan the backward
+ *              reads x_in and start_features again chunk by chunk. */
 int gw_train_encoder_forward_tape(gw_plan* plan, gw_tape* tape, const float* features, float* x_out, float* e_lat_out, int32_t batch,
                                   void* stream);
 int gw_train_encoder_backward_tape(gw_plan* plan, gw_tape* tape, const float* grad_x, const float* grad_e_lat, float* grad_features,

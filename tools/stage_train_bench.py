@@ -1,13 +1,18 @@
 """Times the training step of Encoder -> Processor -> Decoder composed by hand (the reference's tests/test_model.py::test_end2end,
 each stage built with `train_precision`) against GraphWeatherForecaster's own step on the same weights.
-    python tools/stage_train_bench.py [--grid 1deg|2deg|5deg|10deg] [--batch B] [--steps K] [--train-precision fp32_simt|fp32|bf16]
-One step = forward + NormalizedMSELoss + backward + SGD update.  The two steps alternate step by step after two warm-up steps each,
-CUDA events around each step; prints one JSON line with both medians, the card name, power limit and SM clocks read in the same run."""
+    python tools/stage_train_bench.py [--grid 0.25deg|1deg|2deg|5deg|10deg] [--batch B] [--steps K]
+                                      [--train-precision fp32_simt|fp32|bf16] [--use-checkpointing]
+One step = forward + NormalizedMSELoss + backward + SGD update.  --use-checkpointing builds the Encoder, the Decoder and the wrapper
+with use_checkpointing=True: both sides take the bounded-memory step (the processor stays taped).  0.25deg is the 721 x 1440 ERA5
+grid.  The two steps alternate step by step after two warm-up steps each, CUDA events around each step; prints one JSON line with
+both medians, each plan's train_peak_bytes and device bytes after the last step, and the card name, power limit and SM clocks read
+in the same run."""
 import argparse
 import json
 import os
 import sys
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -17,10 +22,11 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--grid", default="1deg", choices=["1deg", "2deg", "5deg", "10deg"])
+    ap.add_argument("--grid", default="1deg", choices=["0.25deg", "1deg", "2deg", "5deg", "10deg"])
     ap.add_argument("--batch", type=int, default=2)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--train-precision", default="bf16", choices=["fp32_simt", "fp32", "bf16"])
+    ap.add_argument("--use-checkpointing", action="store_true")
     a = ap.parse_args()
     import __graft_entry__ as ge
 
@@ -29,12 +35,16 @@ def main():
 
     from graph_weather_b200 import Decoder, Encoder, GraphWeatherForecaster, NormalizedMSELoss, Processor
 
-    step = {"1deg": 1, "2deg": 2, "5deg": 5, "10deg": 10}[a.grid]
-    ll = [(float(lat), float(lon)) for lat in range(-90, 90, step) for lon in range(0, 360, step)]
+    if a.grid == "0.25deg":
+        ll = [(float(lat), float(lon)) for lat in np.linspace(-90.0, 90.0, 721) for lon in np.arange(0.0, 360.0, 0.25)]
+    else:
+        step = {"1deg": 1, "2deg": 2, "5deg": 5, "10deg": 10}[a.grid]
+        ll = [(float(lat), float(lon)) for lat in range(-90, 90, step) for lon in range(0, 360, step)]
     torch.manual_seed(0)
-    tp = a.train_precision
-    wrapper = GraphWeatherForecaster(ll, train_precision=tp).cuda().train()
-    stages = [Encoder(ll, input_dim=102, train_precision=tp), Processor(train_precision=tp), Decoder(ll, train_precision=tp)]
+    tp, cp = a.train_precision, a.use_checkpointing
+    wrapper = GraphWeatherForecaster(ll, train_precision=tp, use_checkpointing=cp).cuda().train()
+    stages = [Encoder(ll, input_dim=102, train_precision=tp, use_checkpointing=cp), Processor(train_precision=tp),
+              Decoder(ll, train_precision=tp, use_checkpointing=cp)]  # fmt: skip
     for m, name in zip(stages, ("encoder", "processor", "decoder")):
         m.load_state_dict(getattr(wrapper, name).state_dict())
     enc, proc, dec = [m.cuda().train() for m in stages]
@@ -65,12 +75,16 @@ def main():
         e1.record()
         torch.cuda.synchronize()
         times[kind].append(e0.elapsed_time(e1))
-    for m in (enc, proc, dec, wrapper):
+    mods = {"encoder": enc, "processor": proc, "decoder": dec, "wrapper": wrapper}
+    for m in mods.values():
         m._train_engine.plan.status()
     med = {k: round(sorted(v)[len(v) // 2], 2) for k, v in times.items()}
     print(json.dumps({"what": "training step (fwd + loss + bwd + SGD), stages composed vs the wrapper", "train_precision": tp,
-                      "grid": a.grid, "batch": a.batch, "steps": a.steps, "median_ms": med,
-                      "ratio": round(med["composed"] / med["wrapper"], 3), "card": card()}))  # fmt: skip
+                      "grid": a.grid, "batch": a.batch, "steps": a.steps, "use_checkpointing": cp, "median_ms": med,
+                      "ratio": round(med["composed"] / med["wrapper"], 3),
+                      "train_only": {k: m._train_engine.plan.train_only for k, m in mods.items()},
+                      "train_peak_bytes": {k: m._train_engine.plan.train_peak_bytes() for k, m in mods.items()},
+                      "plan_bytes": {k: m._train_engine.plan.device_bytes() for k, m in mods.items()}, "card": card()}))  # fmt: skip
 
 
 if __name__ == "__main__":
