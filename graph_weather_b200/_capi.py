@@ -52,6 +52,8 @@ _SIGNATURES = {
     "gw_plan_set_latent_graph": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "gw_plan_set_decoder_graph": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp]),
     "gw_plan_set_weights": (ctypes.c_int, [_vp, ctypes.POINTER(GwParam), _i32, _vp]),
+    "gw_plan_set_h3_nodes": (ctypes.c_int, [_vp, _vp, _vp]),
+    "gw_segment_sum": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp]),
     "gw_forward": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp]),
     "gw_encoder_forward": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp]),
     "gw_processor_forward": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp]),
@@ -143,6 +145,16 @@ def _ptr(t, dtype, device):
 def _opt_ptr(t, device):
     """An optional float32 tensor argument: NULL for None."""
     return _vp() if t is None else _ptr(t, torch.float32, device)
+
+
+def segment_sum(rows, perm, ptr, out):
+    """gw_segment_sum: out[s] = sum of rows[perm[j]] over j in [ptr[s], ptr[s+1]), in j order, on the current stream (rows
+    [n_rows, width] and out [n_seg, width] float32, perm and ptr int32, one device)."""
+    d = rows.device
+    with torch.cuda.device(d):
+        st = ctypes.c_void_p(torch.cuda.current_stream(d).cuda_stream)
+        _check(load().gw_segment_sum(_ptr(rows, torch.float32, d), int(rows.shape[0]), int(rows.shape[1]), _ptr(perm, torch.int32, d),
+                                     _ptr(ptr, torch.int32, d), int(out.shape[0]), _ptr(out, torch.float32, d), st))  # fmt: skip
 
 
 def launch_count() -> int:
@@ -287,6 +299,12 @@ class Plan:
         with self._on_stream() as st:
             _check(self.lib.gw_plan_set_weights(self.handle, arr, len(items), st))
             torch.cuda.current_stream(d).synchronize()
+
+    def set_h3_nodes(self, rows):
+        """gw_plan_set_h3_nodes: rows [n_mesh, in_dim] float32 on the plan's device replace the bound encoder.h3_nodes table, after
+        the graph uploads of a call; the weight constants are recomputed on the plan's current graphs, no weight is re-packed."""
+        with self._on_stream() as st:
+            _check(self.lib.gw_plan_set_h3_nodes(self.handle, _ptr(rows, torch.float32, self.device), st))
 
     def forward(self, features, out, out_ld=None):
         """out: [batch, n_out, out_dim] contiguous, or (out_ld given) the first out_dim columns of rows `out_ld` floats apart."""

@@ -291,6 +291,28 @@ int gw_plan_set_decoder_graph(gw_plan* p, const int32_t* src, const int32_t* ptr
   return 0;
 }
 
+int gw_plan_set_h3_nodes(gw_plan* p, const float* rows, void* stream) {
+  GW_CHECK(p && rows, "null argument");
+  auto it = p->params.find("encoder.h3_nodes");
+  GW_CHECK(it != p->params.end() && p->b_enc && p->h3_nodes == it->second.first,
+           "gw_plan_set_h3_nodes: the plan's weights bind no encoder.h3_nodes (gw_plan_set_weights first, with an encoder.* group)");
+  cudaStream_t st = (cudaStream_t)stream;
+  GW_CUDA(cudaSetDevice(p->device));
+  GW_CUDA(cudaMemcpyAsync(const_cast<float*>(p->h3_nodes), rows, (size_t)p->d.n_mesh * p->d.in_dim * 4, cudaMemcpyDeviceToDevice, st));
+  ++p->graph_gen;  // (a tape's backward differentiates the rows its forward read)
+  p->w_enc = p->b_enc, p->w_proc = p->b_proc, p->w_dec = p->b_dec;  // the views stay valid: only the constants follow the graphs
+  if (!p->train_only) GW_TRY(gw::precompute_constants(p, st));
+  return 0;
+}
+
+int gw_segment_sum(const float* rows, int64_t n_rows, int32_t width, const int32_t* perm, const int32_t* ptr, int32_t n_seg, float* out,
+                   void* stream) {
+  GW_CHECK(rows && perm && ptr && out, "null argument");
+  GW_CHECK(n_rows >= 0 && n_rows <= INT32_MAX && width >= 1 && n_seg >= 1, "bad sizes");
+  GW_CUDA(gw::launch_segsum(rows, width, width, ptr, perm, (int)n_rows, n_seg, 1, out, width, (cudaStream_t)stream));
+  return 0;
+}
+
 int gw_plan_set_weights(gw_plan* p, const gw_param* params, int32_t n, void* stream) {
   GW_CHECK(p && params && n > 0, "null argument");
   cudaStream_t st = (cudaStream_t)stream;

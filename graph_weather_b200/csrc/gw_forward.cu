@@ -246,6 +246,7 @@ int bind_all(gw_plan* p) {
   const int Ln = d.hidden_layers_node, Le = d.hidden_layers_edge;
   auto has = [&](const char* k) { return p->params.count(k) != 0; };
   p->w_enc = p->w_proc = p->w_dec = false;
+  p->b_enc = p->b_proc = p->b_dec = false;  // (a failed upload leaves nothing for gw_plan_set_h3_nodes to rebind)
   if (has("encoder.node_encoder.model.0.weight")) {
     GW_TRY(bind_mlp(p, "encoder.node_encoder", d.in_dim, Hn, Dn, Ln, true, &p->enc_node));
     GW_TRY(bind_mlp(p, "encoder.edge_encoder", d.enc_edge_attr_dim, He, De, Le, true, &p->enc_edge_enc));
@@ -283,6 +284,7 @@ int bind_all(gw_plan* p) {
     p->w_dec = true;
   }
   GW_CHECK(p->w_enc || p->w_proc || p->w_dec, "no encoder./processor./decoder. parameter group found in the table");
+  p->b_enc = p->w_enc, p->b_proc = p->w_proc, p->b_dec = p->w_dec;
   return 0;
 }
 

@@ -126,13 +126,15 @@ struct gw_plan {
   int device = 0;
   int n_in_cur = 0;
   unsigned enc_graph_gen = 0;  // bumped whenever the encoder graph is replaced (the training step's chunk tables are built per graph)
-  unsigned graph_gen = 0;      // bumped whenever the latent or decoder graph is replaced (the training step's source-sorted copies follow it)
+  unsigned graph_gen = 0;      // bumped whenever the latent or decoder graph or the h3_nodes rows are replaced (the training step's
+                               // source-sorted copies follow it; a tape's backward refuses once it moved)
   unsigned wgen = 0;           // bumped by every gw_plan_set_weights (the training step's per-weight work and its tapes key on it)
   // graphs
   DevBuf<int32_t> enc_mesh, enc_perm, enc_ptr, lat_src, lat_dst, lat_ptr, dec_src, dec_ptr;
   DevBuf<float> enc_attr, lat_attr, dec_attr;
   bool have_enc = false, have_lat = false, have_dec = false;   // graphs uploaded
   bool w_enc = false, w_proc = false, w_dec = false;            // weight groups bound (standalone sub-modules bind one)
+  bool b_enc = false, b_proc = false, b_dec = false;            // the groups the last gw_plan_set_weights bound (gw_plan_set_h3_nodes rebinds them)
   // weights (plan-owned copy) and views
   DevBuf<float> wbuf;
   std::map<std::string, std::pair<const float*, std::pair<int64_t, int64_t>>> params;

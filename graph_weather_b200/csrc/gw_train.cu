@@ -106,6 +106,7 @@ struct gw_tape {
   bool have_tape = false;  // a forward's activations, not yet consumed by a backward
   int stage = gw::TAPE_NET;        // the forward that made it: the whole network or one stage
   unsigned enc_gen = 0;            // gw_plan::enc_graph_gen its encoder ran on
+  unsigned graph_gen = 0;          // gw_plan::graph_gen of the latent and decoder graphs and h3_nodes rows it ran on
   bool caller_input = false;       // the processor's / decoder's input rows are the caller's: their stage-0 ops bound them (train_op)
   const float* features = nullptr;
   const float* start = nullptr;    // the decoder's residual rows (the features in the whole network), row stride start_ld
@@ -140,7 +141,7 @@ struct TrainState {
   // chunked step (training-only plans): chunk tables for a batch size (and, for the encoder, an encoder graph), built by the forward
   // and, when a tape of another batch size ran since, again by the backward
   int enc_chunks_batch = 0, dec_chunks_batch = 0;
-  unsigned enc_chunks_gen = 0;
+  unsigned enc_chunks_gen = 0, dec_chunks_gen = 0;  // gw_plan::enc_graph_gen / graph_gen the tables were built for
   std::vector<GridRange> enc_chunks, dec_chunks;
   DevBuf<int32_t> enc_slot_sorted;  // mesh slot of every position of enc_perm
   DevBuf<int32_t> dec_cperm, dec_cptr;  // per decoder chunk: its edges sorted by source (chunk-local ids) and the CSR over mesh slots
@@ -382,9 +383,10 @@ static int chunk_points(const gw_plan* p, int batch, double rows_per_point) {
 
 // Encoder chunks: whole mesh slots in enc_perm order (a slot's sum is never split; a slot larger than the budget is a chunk of its
 // own).  Decoder chunks: runs of consecutive points, whose edges are consecutive too, each with the source-sorted CSR of its edges.
-// The decoder tables are built once per batch size.  The encoder tables are built per batch size and encoder graph (gw_plan::
-// enc_graph_gen): the assimilator's observation graph changes on every call, and chunks of an earlier graph would cover the wrong
-// points.  Building them copies enc_ptr to the host, so a step whose encoder graph changed synchronises its stream once (every
+// The decoder tables are built per batch size and graph generation (gw_plan::graph_gen): RegionalForecaster.forward_regions uploads
+// a new decoder graph on every call, and source-sorted edges of an earlier graph would send each gradient to the wrong cell.  The
+// encoder tables are built per batch size and encoder graph (gw_plan::enc_graph_gen): the assimilator's observation graph changes on
+// every call, and chunks of an earlier graph would cover the wrong points.  Building them copies enc_ptr to the host, so a step whose encoder graph changed synchronises its stream once (every
 // bounded step of the assimilator and of a standalone AssimilatorEncoder; the taped step builds no chunk tables).  Only the tables
 // of the stages the plan holds are built: a standalone encoder's plan has no decoder graph, a standalone decoder's no encoder graph.
 // Both phases index iota: encoder chunks by mesh slot, decoder chunks by point.
@@ -429,7 +431,7 @@ static int build_chunks(gw_plan* p, TrainState* T, int batch) {
     GW_CHECK(most <= INT32_MAX, "training step: one chunk of the grid-sized stages holds more than 2^31 rows (lower the batch)");
     T->enc_chunks_batch = batch, T->enc_chunks_gen = p->enc_graph_gen;
   }
-  if (p->have_dec && T->dec_chunks_batch != batch) {
+  if (p->have_dec && (T->dec_chunks_batch != batch || T->dec_chunks_gen != p->graph_gen)) {
     std::vector<int32_t> dptr(No + 1);
     GW_CUDA(cudaMemcpyAsync(dptr.data(), p->dec_ptr.p, (No + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, T->st));
     GW_CUDA(cudaStreamSynchronize(T->st));
@@ -451,7 +453,7 @@ static int build_chunks(gw_plan* p, TrainState* T, int batch) {
       else
         GW_CUDA(launch_sort_csr(p->dec_src.p + r.e0, r.e1 - r.e0, H, T->dec_cperm.p + r.e0, cptr, T->sort_ws.p, T->sort_ws.n, T->st));
     }
-    T->dec_chunks_batch = batch;
+    T->dec_chunks_batch = batch, T->dec_chunks_gen = p->graph_gen;
   }
   return 0;
 }
@@ -906,6 +908,7 @@ static int forward_begin(gw_plan* p, TrainState* T, gw_tape* K, int stage, int n
   GW_TRY(train_prepare(p, T, B, need, st));
   GW_TRY(reset_bounds(T));
   K->batch = B, K->wgen = p->wgen, K->segments = p->train_segments, K->stage = stage, K->enc_gen = p->enc_graph_gen;
+  K->graph_gen = p->graph_gen;
   K->features = nullptr, K->start = nullptr, K->start_ld = 0, K->xd = nullptr, K->caller_input = false;
   K->g = LatGraph();
   if (p->have_lat) {
@@ -1026,6 +1029,9 @@ static int backward_begin(gw_plan* p, TrainState* T, gw_tape* K, int stage, cuda
                                "its gradient would be taken at other weights");
   GW_CHECK(stage != TAPE_ENC || K->enc_gen == p->enc_graph_gen,
            "encoder backward: the plan's encoder graph was replaced after this tape's forward; its gradient would be taken on another graph");
+  GW_CHECK(stage == TAPE_PROC || (K->enc_gen == p->enc_graph_gen && K->graph_gen == p->graph_gen),
+           "training backward: the plan's graphs or h3_nodes rows were replaced after this tape's forward (a later call on other regions); "
+           "its gradient would be taken on other graphs");
   T->st = st;
   T->tp = K;
   if (p->train_only) GW_TRY(build_chunks(p, T, K->batch));  // (a tape of another batch size may have run since this one's forward)

@@ -10,10 +10,20 @@ the reference's parameter names (`node_encoder`, `encoder_gnn`, `decoder_edge_en
 and hands them to the plan under the names the C ABI binds (include/gw_b200.h), with the region's embedding rows as
 `encoder.h3_nodes`.  A plan is sized for one region; a region with other counts gets its own plan (a handful are kept).
 
+`forward_regions(features, regions, global_context)` runs B regions in one call, as one sample whose graphs are the disjoint union
+of the regions' graphs (`_RegionBatch`: each region's point, cell and edge ids offset by the regions before it, its edge order
+kept, so every per-target sum adds in the order of a single-region call).  The union is padded with inert rows up to a capacity
+(points, cells, latent edges; powers of two, grown when a batch does not fit and never shrunk), so one plan per step kind serves
+every batch within it: a new set of regions costs its host graphs, their upload and the inference plan's per-graph constants
+(gw_plan_set_h3_nodes), never a new plan, a weight upload or a weight-image repack.  Output i is `forward` on region i alone.
+
 Training (`train_precision`, as on the other wrappers): in train mode with autograd on, a forward runs the forecaster's CUDA
 training step on training plans of the region (`use_checkpointing=True`: the bounded-memory step).  `h3_embeddings.grad` is
 table-shaped, as the reference's: the region's rows at their cells, zero elsewhere.  A region's plans are kept while a backward
 still needs one of their tapes, so the losses of more regions than the cache holds can be summed into one `backward()`.
+`forward_regions` trains the same way on its union plans; a cell two regions share gets the sum of their rows' gradients, added
+in a fixed order on the device (gw_segment_sum).  The union plan holds the graphs of its last call, so a backward after a later
+`forward_regions` raises, and `forward_regions` refuses to train inside `multi_step()`.
 
 Optional boundary nudging (:44-130): a distance-based relaxation prior plus a learned one-hidden-layer correction, blended
 with a caller-supplied global forecast.  It is a [B, N, 2F+1] -> 1 element-wise tail outside the GNN; it runs as device
@@ -23,6 +33,7 @@ tensor ops (no kernels of this library), exactly the reference's arithmetic.
 from __future__ import annotations
 
 import math
+import time
 from collections import OrderedDict
 from dataclasses import dataclass
 from typing import Optional
@@ -31,7 +42,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import graphs, h3lite
+from . import _capi, graphs, h3lite
 from .dynamic_graph_builder import DynamicGraphBuilder
 from .models import (MLP, GraphProcessor, Processor, _maybe_check, _new_engine, _no_host_path, _pending_tape, _switch_training_engine,
                      _TrainFn, _validate_precision, _validate_train_precision, _Wrapper, _wants_grad)  # fmt: skip
@@ -127,6 +138,71 @@ class _RegionGraphs:
         plan.set_decoder_graph(self.dec_src, self.dec_ptr, self.enc_attr)
 
 
+def _pow2(n: int) -> int:
+    return 1 << max(0, int(n) - 1).bit_length()
+
+
+def _spread(n_items: int, first: int, n_slots: int) -> np.ndarray:
+    """Slots first .. first + n_slots - 1 for n_items padding rows, non-decreasing and as even as the counts allow."""
+    return (first + (np.arange(n_items, dtype=np.int64) * n_slots) // max(n_items, 1)).astype(np.int32)
+
+
+class _RegionBatch:
+    """B regions' graphs as one graph (the disjoint union), padded to a capacity `cap` of points (n_in = n_out = n_dec_edges),
+    cells (n_mesh) and latent edges (n_lat_edges).  Region i's points, cells and edges follow those of regions 0 .. i-1, in its
+    own order.  The padding is inert: padding points (zero features and edge attributes) feed, and are decoded from, padding cells
+    only; padding cells (zero h3_nodes rows) carry only self loops with zero attributes.  No padding edge touches a real row, every
+    row stays finite, and real rows see exactly their region's edges.  There is always at least one padding cell."""
+
+    def __init__(self, graphs: list, cap: dict):
+        self.graphs = graphs
+        n = [g.n_obs for g in graphs]
+        m = [g.n_mesh for g in graphs]
+        e = [g.n_lat_edges for g in graphs]
+        self.n_real, self.m_real, self.e_real = sum(n), sum(m), sum(e)
+        P, C, E = cap["n_in"], cap["n_mesh"], cap["n_lat_edges"]
+        if P < self.n_real or C <= self.m_real or E < max(self.e_real, 1):
+            raise ValueError(f"capacity {cap} does not hold {self.n_real} points, {self.m_real} + 1 cells and {self.e_real} latent edges")
+        self.cap = dict(cap)
+        po = np.concatenate([[0], np.cumsum(n)]).astype(np.int64)
+        co = np.concatenate([[0], np.cumsum(m)]).astype(np.int64)
+        eo = np.concatenate([[0], np.cumsum(e)]).astype(np.int64)
+        self.point_offsets, self.cell_offsets, self.edge_offsets = po, co, eo
+        n_pad, c_pad, e_pad = P - self.n_real, C - self.m_real, E - self.e_real
+        pad_cell = _spread(n_pad, self.m_real, c_pad)
+        self.mesh_local = np.concatenate([g.mesh_local + co[i] for i, g in enumerate(graphs)] + [pad_cell]).astype(np.int32)
+        self.enc_perm = np.concatenate([g.enc_perm + po[i] for i, g in enumerate(graphs)]
+                                       + [np.arange(self.n_real, P)]).astype(np.int32)  # fmt: skip
+        self.enc_ptr = np.zeros(C + 1, dtype=np.int32)
+        np.cumsum(np.bincount(self.mesh_local, minlength=C), out=self.enc_ptr[1:])
+        self.enc_attr = np.concatenate([g.enc_attr for g in graphs] + [np.zeros((n_pad, 2), np.float32)]).astype(np.float32)
+        pad_self = _spread(e_pad, self.m_real, c_pad)
+        self.lat_src = np.concatenate([g.lat_src + co[i] for i, g in enumerate(graphs)] + [pad_self]).astype(np.int32)
+        self.lat_dst = np.concatenate([g.lat_dst + co[i] for i, g in enumerate(graphs)] + [pad_self]).astype(np.int32)
+        self.lat_ptr = np.zeros(C + 1, dtype=np.int32)
+        np.cumsum(np.bincount(self.lat_dst, minlength=C), out=self.lat_ptr[1:])
+        self.lat_attr = np.concatenate([g.lat_attr for g in graphs] + [np.zeros((e_pad, 2), np.float32)]).astype(np.float32)
+        self.dec_src = self.mesh_local
+        self.dec_ptr = np.arange(P + 1, dtype=np.int32)
+        self.h3_indices = np.concatenate([g.h3_indices for g in graphs]).astype(np.int64)  # cell of every real union row
+        # the table gradient: union rows grouped by cell (stable: region order inside a cell), CSR over the whole table
+        self.by_cell = np.argsort(self.h3_indices, kind="stable").astype(np.int32)
+        self.n_obs = P
+
+    def cell_ptr(self, n_cells: int) -> np.ndarray:
+        ptr = np.zeros(n_cells + 1, dtype=np.int32)
+        np.cumsum(np.bincount(self.h3_indices, minlength=n_cells), out=ptr[1:])
+        return ptr
+
+    def upload(self, plan, h3_rows):
+        """The union's graphs, then its h3_nodes rows (which also recompute the constants on the new graphs).  The latent graph goes
+        first: it unbinds the weights, so the encoder graph's upload does not recompute constants on the previous graphs."""
+        plan.set_latent_graph(self.lat_src, self.lat_dst, self.lat_ptr, self.lat_attr)
+        plan.set_encoder_graph(self.mesh_local, self.enc_perm, self.enc_ptr, self.enc_attr)
+        plan.set_decoder_graph(self.dec_src, self.dec_ptr, self.enc_attr)
+        plan.set_h3_nodes(h3_rows)
+
+
 class RegionalForecaster(nn.Module):
     """RegionalForecaster(config)(features, lat_lons, global_context=None) -> [B, N_obs, output_dim]  (regional_forecast.py:133-298)."""
 
@@ -180,7 +256,13 @@ class RegionalForecaster(nn.Module):
         self.use_checkpointing = c.use_checkpointing
         # per-region state: graphs are cached like the reference's builder caches them (same list object -> same graphs)
         self.__dict__["_regions"] = OrderedDict()  # id(lat_lons) -> (lat_lons, _RegionGraphs, engines)
-        self.__dict__["_active"] = None  # (graphs, engines) of the region of the current training forward
+        self.__dict__["_active"] = None  # (graphs, engines) of the region (or _RegionBatch) of the current training forward
+        # forward_regions: one engine per step kind ({"infer", False: taped, True: bounded}) over the union's capacity
+        self.__dict__["_batch_engines"] = {}
+        self.__dict__["_batch_cap"] = None
+        self.__dict__["_zero_rows"] = None  # the h3_nodes table the union plans' weight uploads carry (its rows come per call)
+        # forward_regions: host seconds of the last call's graph build, weight upload (only after a weight change) and graph upload
+        self.__dict__["last_setup_s"] = None
 
     # ---- the plan's view of the parameters -------------------------------------------------------------------------------
     _RENAME = (
@@ -194,9 +276,12 @@ class RegionalForecaster(nn.Module):
         ("node_decoder.", "decoder.node_decoder."),
     )
 
-    def _plan_named(self, region: _RegionGraphs):
+    def _plan_named(self, region):
         out = []
         for k, v in self.state_dict(keep_vars=True).items():
+            if k == "h3_embeddings" and isinstance(region, _RegionBatch):  # rows uploaded per call (_RegionBatch.upload)
+                out.append(("encoder.h3_nodes", self._zero_rows))
+                continue
             if k == "h3_embeddings":  # the region's rows of the global table (:243); re-gathered only when the table changed
                 key = (v.data_ptr(), v._version, str(v.device))
                 if getattr(region, "_h3_key", None) != key:
@@ -224,7 +309,8 @@ class RegionalForecaster(nn.Module):
         region, engines = self._active
 
         def make(bounded):
-            return _new_engine(engines["infer"].dims, self.train_precision, [region.upload], train_only=bounded)
+            uploaders = [] if isinstance(region, _RegionBatch) else [region.upload]  # (the union's: forward_regions, every call)
+            return _new_engine(engines["infer"].dims, self.train_precision, uploaders, train_only=bounded)
 
         eng = _switch_training_engine(engines, bool(self.use_checkpointing), make)
         self.__dict__["_train_engine"] = eng
@@ -240,6 +326,8 @@ class RegionalForecaster(nn.Module):
         parameters are differentiated by torch."""
         named = self._named()
         table, idx = self.h3_embeddings, self._active[0].h3_idx
+        if isinstance(self._active[0], _RegionBatch):
+            return [(k, v, table, self._active[0].to_table) if k == "encoder.h3_nodes" else (k, v, v, None) for k, v in named]
 
         def to_table(g):
             full = g.new_zeros(table.shape)
@@ -306,3 +394,109 @@ class RegionalForecaster(nn.Module):
         if self.nudging is not None and global_context is not None:
             out = self.nudging(out, global_context.to(out.device), lat_lons)
         return out
+
+    # ---- a batch of regions in one call ------------------------------------------------------------------------------------
+    def _batch(self, regions: list, device) -> tuple:
+        """The union of the regions' graphs, padded to the capacity (grown to the next power of two of each count when the union does
+        not fit, never shrunk), with its h3_nodes rows, its table-gradient map and its rows on the device; and the batch engines.
+        Returns (_RegionBatch, engines)."""
+        t0 = time.perf_counter()
+        graphs = [_RegionGraphs(self.graph_builder, r) for r in regions]
+        need = dict(n_in=sum(g.n_obs for g in graphs), n_mesh=sum(g.n_mesh for g in graphs) + 1,
+                    n_lat_edges=max(1, sum(g.n_lat_edges for g in graphs)))  # fmt: skip
+        cap = self._batch_cap or {}
+        if any(need[k] > cap.get(k, 0) for k in need):
+            cap = {k: max(cap.get(k, 0), _pow2(need[k])) for k in need}
+            cap.update(n_out=cap["n_in"], n_dec_edges=cap["n_in"])
+            self.__dict__["_batch_cap"] = cap
+        batch = _RegionBatch(graphs, cap)
+        t1 = time.perf_counter()
+        table = self.h3_embeddings
+        if self._zero_rows is None or tuple(self._zero_rows.shape) != (cap["n_mesh"], table.shape[1]) or self._zero_rows.device != device:
+            self.__dict__["_zero_rows"] = torch.zeros((cap["n_mesh"], table.shape[1]), dtype=torch.float32, device=device)
+        engines = self._batch_engines
+        if "infer" not in engines:
+            engines["infer"] = _new_engine(dict(self._base_dims, n_in=1, n_out=1, n_mesh=2, n_lat_edges=1, n_dec_edges=1),
+                                           self.config.precision, [])  # fmt: skip
+        batch.h3_idx = torch.from_numpy(batch.h3_indices).to(device)
+        batch.by_cell_d = torch.from_numpy(batch.by_cell).to(device)
+        batch.cell_ptr_d = torch.from_numpy(batch.cell_ptr(table.shape[0])).to(device)
+
+        def to_table(g):  # h3_nodes gradient [n_mesh, in_dim] -> table gradient: per cell, the sum of its rows in region order
+            out = g.new_empty(table.shape)
+            _capi.segment_sum(g.contiguous(), batch.by_cell_d, batch.cell_ptr_d, out)
+            return out
+
+        batch.to_table = to_table
+        rows = torch.zeros((cap["n_mesh"], table.shape[1]), dtype=torch.float32, device=device)
+        rows[: batch.m_real] = table.detach()[batch.h3_idx]
+        batch.h3_rows = rows
+        self.__dict__["last_setup_s"] = {"build": t1 - t0}
+        return batch, engines
+
+    def _batch_plan(self, eng, batch, device):
+        """`eng`'s plan at the batch's capacity with the current weights, the union's graphs and rows uploaded."""
+        t0 = time.perf_counter()
+        plan = eng.ensure(device, 1, self._plan_named(batch), grow=batch.cap)
+        t1 = time.perf_counter()
+        batch.upload(plan, batch.h3_rows)
+        self.last_setup_s.update(weights=t1 - t0, upload=time.perf_counter() - t1)
+        return plan
+
+    def forward_regions(self, features, regions: list, global_context=None):
+        """B regions in one call: output i is `self(features[i:i+1], regions[i], global_context[i:i+1])[0]`, nudging included.
+
+        regions: B coordinate lists (each as forward's lat_lons).  features: [B, N, F] when every region has N points, or a list of B
+        tensors [N_i, F]; global_context: the output's form, or None.  Returns [B, N, output_dim] or a list of [N_i, output_dim], in
+        the form of `features`.  In train mode with autograd on (and a train_precision) it is differentiable: the gradients of a loss
+        over its outputs are those of the sum of the B single-region steps, up to the order of float sums.  The regions run as one
+        graph on one plan per step kind, kept from call to call (see the module docstring).  Training inside `multi_step()` raises:
+        the plan holds one set of regions, so only the last call's forward can be differentiated."""
+        stacked = torch.is_tensor(features)
+        feats = list(features.unbind(0)) if stacked else list(features)
+        if len(feats) != len(regions) or not regions:
+            raise ValueError(f"{len(feats)} feature sets for {len(regions)} regions (need one per region, at least one)")
+        device = feats[0].device
+        if device.type != "cuda":
+            _no_host_path("RegionalForecaster.forward_regions")
+        for f, r in zip(feats, regions):
+            if f.dim() != 2 or f.shape[0] != len(r):
+                raise ValueError(f"a region's features must be [{len(r)}, F] (one row per coordinate), got {tuple(f.shape)}")
+            if f.shape[1] < self.output_dim:
+                raise RuntimeError(f"features needs at least output_dim ({self.output_dim}) channels for the residual add (:288)")
+        F = feats[0].shape[1]
+        if any(f.shape[1] != F for f in feats):
+            raise ValueError("every region's features need the same number of channels")
+        train = torch.is_grad_enabled() and self.training and (any(f.requires_grad for f in feats)
+                                                               or any(q.requires_grad for q in self.parameters()))  # fmt: skip
+        if train and self.train_precision is None:
+            raise NotImplementedError("RegionalForecaster: training needs RegionalForecasterConfig.train_precision ('fp32_simt', 'fp32' "
+                                      "or 'bf16'); call under torch.no_grad() or in eval() mode for inference")
+        if train and self.__dict__.get("_multi_step", 0):
+            raise NotImplementedError("RegionalForecaster.forward_regions inside multi_step(): the union graph a training forward runs on "
+                                      "belongs to the plan, not to the forward, so several calls cannot stay differentiable at once")
+        batch, engines = self._batch(regions, device)
+        P = batch.n_obs
+        pad = feats[0].new_zeros((P - batch.n_real, F))
+        union = torch.cat([f.to(torch.float32) for f in feats] + [pad.to(torch.float32)])[None]
+        if train:
+            self.__dict__["_active"] = (batch, engines)
+            try:
+                self._batch_plan(self._training_engine(), batch, device)
+                bindings = self._grad_bindings()
+                out = _TrainFn.apply(self, union, None, bindings, *[q for _, _, q, _ in bindings])
+            finally:
+                self.__dict__["_active"] = None
+        else:
+            plan = self._batch_plan(engines["infer"], batch, device)
+            out = torch.empty((1, P, self.output_dim), dtype=torch.float32, device=device)
+            plan.forward(union.detach().contiguous(), out)
+            _maybe_check(plan)
+        po = batch.point_offsets
+        outs = [out[0, po[i]: po[i + 1]] for i in range(len(regions))]
+        if self.nudging is not None and global_context is not None:
+            gcs = list(global_context.unbind(0)) if torch.is_tensor(global_context) else list(global_context)
+            if len(gcs) != len(regions):
+                raise ValueError(f"{len(gcs)} global contexts for {len(regions)} regions")
+            outs = [self.nudging(o[None], g.to(o.device)[None], r)[0] for o, g, r in zip(outs, gcs, regions)]
+        return torch.stack(outs) if stacked else outs

@@ -125,6 +125,19 @@ int gw_plan_set_decoder_graph(gw_plan* plan, const int32_t* src, const int32_t* 
  * its node decoder with the configured norm (regional_forecast.py:224-231), the forecaster / assimilator decoders without. */
 int gw_plan_set_weights(gw_plan* plan, const gw_param* params, int32_t n, void* stream);
 
+/* Plans whose graphs change between calls without a weight change (RegionalForecaster.forward_regions: a batch of regions run
+ * as one graph, a new set of regions per call).  After the call's graph uploads, gw_plan_set_h3_nodes copies rows [n_mesh, in_dim]
+ * (device) over the "encoder.h3_nodes" table gw_plan_set_weights bound, binds again the weight groups that upload bound (graph
+ * uploads unbind them) and recomputes the weight constants on the new graphs -- without copying or re-packing any weight.  Like a
+ * latent or decoder graph upload it moves the plan's graph generation: a training backward whose forward ran on the earlier
+ * graphs or rows refuses.
+ * gw_segment_sum: out[s, :] = sum of rows[perm[j], :] over j in [ptr[s], ptr[s+1]), in j order (rows [n_rows, width], perm, ptr
+ * [n_seg + 1], out [n_seg, width]; all device).  A fixed-order sum without atomics: forward_regions adds the h3_nodes gradient
+ * rows of a cell that several regions share into the cell's row of the table. */
+int gw_plan_set_h3_nodes(gw_plan* plan, const float* rows, void* stream);
+int gw_segment_sum(const float* rows, int64_t n_rows, int32_t width, const int32_t* perm, const int32_t* ptr, int32_t n_seg, float* out,
+                   void* stream);
+
 /* Replaces: GraphWeatherForecaster.forward (forecast.py:215-247, constraint_type="none") and
  * GraphWeatherAssimilator.forward (analysis.py:136-150) after its per-call input graph is uploaded.
  *   features [batch, n_in, in_dim]  ->  out [batch, n_out, out_dim];  batch <= max_batch.                     */
